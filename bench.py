@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- candidate-fits/sec of the cross-validated grid search (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--workload c2] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--workload c2] [--impl ours|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...      (N > 1)
 
 A "step" is one pass of the hot path over the whole workload: every (candidate, fold) fit+score task of
@@ -20,8 +20,10 @@ roofline: the dominant kernel (batched SMO): algorithmic HBM bytes (2 gathered f
          the Gram build north_star names (algorithmic bytes / its event time).
 secondary: BASELINE configs 4 (SVC 16x16), 3 (LogisticRegression random 256) and 5 (Ridge 512 alphas) measured in
          the same run, STRONG-scaled over the N ranks (candidates dealt, one score all-gather): fits/s, e2e, parity
-         against the committed scikit-learn goldens, and a roofline each (tensor-pipe fraction of the tcgen05
+         against the committed scikit-learn goldens, and a roofline each (tensor-pipe fraction of the wgmma
          contraction kernel against a TF32 peak measured here with cuBLAS for configs 3 and 5).
+--dump-outputs DIR: after the timed steps, the per-(candidate, split) test and train scores of the last timed step of every
+         workload of the run (what cv_results_ is built from) as DIR/<workload>_{test,train}_scores.npy, float64.
 cpu_baseline / --impl reference: scikit-learn's own GridSearchCV (the reference's CPU path, joblib) with ONE
          (candidate, fold) task per host core per step: `cores` candidates whose predicted cost is nearest the grid
          mean, one fold -- every core is busy for the whole step and the sample's mean cost is the grid's.
@@ -44,16 +46,12 @@ GOLDEN = {"c2": "c2_svc_rbf_8x8", "c4": "c4_svc_rbf_16x16", "c3": "c3_logreg_ran
 
 
 # ----------------------------------------------------------------------------- helpers ----------
-def measured_peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        d = json.load(open(p))
-        return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+def hbm_peak():
+    return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s), not measured"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -208,7 +206,7 @@ def parity_block(w, test_scores):
 
 
 def tf32_peak_tflops():
-    """cuBLAS TF32 GEMM throughput on this GPU (the denominator for the tcgen05 kind::tf32 contraction kernel)."""
+    """cuBLAS TF32 GEMM throughput on this GPU (the denominator for the wgmma tf32 contraction kernel)."""
     import torch
     old = torch.backends.cuda.matmul.allow_tf32
     torch.backends.cuda.matmul.allow_tf32 = True
@@ -310,11 +308,11 @@ class Runner:
         r = dict(zip(keys_max + ["wall", "e2e_wall"], [float(x) for x in tm.cpu()]))
         r.update(zip(keys_sum, [float(x) for x in ts.cpu()]))
         r["phase_mean"] = dict(zip(keys_max, [float(x) / max(self.world, 1) for x in tavg.cpu()]))
-        r.update(test=out["test"], e2e_prof=e2e_prof, clocks=clocks, steps=steps)
+        r.update(test=out["test"], train=out["train"], e2e_prof=e2e_prof, clocks=clocks, steps=steps)
         return r
 
 
-def secondary_entry(key, rank, world, local_rank, dist, steps, peaks):
+def secondary_entry(key, rank, world, local_rank, dist, steps, peaks, dump):
     """One BASELINE config, strong-scaled over the ranks: value, e2e, parity vs golden, roofline of its dominant kernel."""
     from spark_sklearn_b200 import workloads as WL
     w = WL.make_workload(key)
@@ -323,6 +321,7 @@ def secondary_entry(key, rank, world, local_rank, dist, steps, peaks):
     m = run.measure(steps, 2)
     if rank != 0:
         return None
+    dump[key] = m
     fits, K = run.fits, steps
     ent = {"workload": "%s: %s(%s), %dx%d, %d candidates x cv=%d = %d fits" % (
                w["name"], "GridSearchCV" if w["search"] == "grid" else "RandomizedSearchCV", w["estimator"],
@@ -340,7 +339,7 @@ def secondary_entry(key, rank, world, local_rank, dist, steps, peaks):
                            "note": "per-rank algorithmic bytes (n_iter * 2 rows * l * 4 B) / solve-phase event time (max over ranks)"}
     else:
         ach = m["tensor_flops"] / max(world, 1) / (m["ms_tensor"] * 1e-3) / 1e12 if m["ms_tensor"] > 0 else 0.0
-        ent["roofline"] = {"kernel": "gemm_nt_tf32x3_kernel (tcgen05 kind::tf32, TMA operands, 3xTF32 split)", "bound": "tensor",
+        ent["roofline"] = {"kernel": "gemm_nt_tf32x3_kernel (wgmma tf32, TMA operands, 3xTF32 split)", "bound": "tensor",
                            "achieved": ach, "peak": tf32, "unit": "TFLOP/s", "frac": ach / tf32 if tf32 else None, "traffic": None,
                            "tensor_ms_per_step": m["ms_tensor"] / K, "share_of_step": m["ms_tensor"] / m["ms_total"] if m["ms_total"] else None,
                            "note": "executed TF32 tensor flops (3 MMAs per fp32-faithful product) of all contraction launches of a step / "
@@ -359,7 +358,12 @@ def main():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-secondary", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None)
     a = ap.parse_args()
+    if a.steps < 1:
+        ap.error("--steps must be >= 1")
+    if a.dump_outputs and a.impl != "ours":
+        ap.error("--dump-outputs writes what the GPU path computed: it needs --impl ours")
     # stdout carries exactly ONE line (the JSON): libraries that print there (NCCL's version banner, joblib) go to stderr
     sys.stdout.flush()
     real_stdout = os.fdopen(os.dup(1), "w")
@@ -417,13 +421,14 @@ def main():
     test_scores = m["test"]
     fits = run.fits
 
-    peak, peak_src = measured_peaks()
+    peak, peak_src = hbm_peak()
+    dump = {a.workload: m}
     secondary = None
     if not a.no_secondary and a.workload == "c2":
         tf32 = tf32_peak_tflops() if rank == 0 else 0.0
         secondary = {}
         for key in ("c4", "c3", "c5"):
-            ent = secondary_entry(key, rank, world, local_rank, dist, min(max(a.steps, 1), 5), (peak, tf32))
+            ent = secondary_entry(key, rank, world, local_rank, dist, a.steps, (peak, tf32), dump)
             if rank == 0:
                 secondary[key] = ent
         if rank == 0:
@@ -436,17 +441,17 @@ def main():
             dist.destroy_process_group()
         return
 
-    K = max(a.steps, 1)
+    if a.dump_outputs:
+        os.makedirs(a.dump_outputs, exist_ok=True)
+        for key, mk in dump.items():
+            for part in ("test", "train"):
+                np.save(os.path.join(a.dump_outputs, "%s_%s_scores.npy" % (key, part)), np.asarray(mk[part], np.float64))
+    K = a.steps
     # roofline of the dominant kernel: batched SMO, HBM-bound by design (row gathers)
     per_launch_bytes = m["solve_bytes"] / K / max(world, 1)
     per_launch_s = m["ms_solve"] / K * 1e-3
     achieved = per_launch_bytes / per_launch_s / 1e9 if per_launch_s > 0 else 0.0
     traffic, traffic_src = None, None
-    tp = os.path.join(ROOT, "profiles", "traffic.json")      # DRAM bytes of the SMO launches of one step, from an ncu capture
-    if os.path.exists(tp) and world <= 1:
-        t = json.load(open(tp)).get(a.workload)
-        if t:
-            traffic, traffic_src = float(t["dram_bytes_per_step"]), t["source"]
     roofline = {"kernel": "smo_lean_kernel (one CTA per sub-problem, two per SM) + smo_colown_kernel (thread-block cluster per critical-path "
                           "sub-problem), launched concurrently: batched exact-trajectory C-SVC SMO", "bound": "hbm",
                 "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "peak_source": peak_src,

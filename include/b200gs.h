@@ -1,5 +1,5 @@
 /*
- * b200gs.h -- C ABI of libb200gs.so, the B200 (sm_100a) cross-validated grid-search engine.
+ * b200gs.h -- C ABI of libb200gs.so, the H100 (sm_90a) cross-validated grid-search engine.
  *
  * Drop-in boundary.  The reference (databricks/spark-sklearn) is pure Python and has no FFI of
  * its own; the seam this library replaces is the per-task closure that the reference maps over
@@ -19,7 +19,7 @@
  * negative gs_status, never throws; gs_last_error() returns a human-readable message for the last
  * failure on that handle.  All pointers are HOST pointers owned by the caller and need only live
  * for the duration of the call.  A handle is bound to one CUDA device and is not thread-safe.
- * There is no CPU fallback: without a usable sm_100 device gs_create fails.
+ * There is no CPU fallback: without a usable sm_90 device gs_create fails.
  */
 #ifndef B200GS_H
 #define B200GS_H
@@ -46,7 +46,7 @@ enum gs_dtype { GS_F32 = 0, GS_F64 = 1 };
 
 enum gs_flags {
     GS_RETURN_TRAIN = 1,     /* also fill train_scores (reference return_train_score=True)   */
-    GS_GRAM_TENSOR = 2,      /* build the Gram on tcgen05 tensor cores (3xTF32 split, fp32-faithful)
+    GS_GRAM_TENSOR = 2,      /* build the Gram on wgmma tensor cores (3xTF32 split, fp32-faithful)
                                 instead of the float64 Gram that reproduces libsvm bit for bit */
     GS_NO_SHRINKING = 4      /* SVC(shrinking=False)                                         */
 };
@@ -94,7 +94,7 @@ enum {
 };
 int gs_set_scoring(gs_handle *h, int32_t kind, int32_t pos_class);   /* gs_set_data resets scoring, class and sample weights to their defaults */
 
-/* Number of sm_100 GPUs this process can drive (0: none).  Replaces: the executor count Spark reports to the driver
+/* Number of sm_90 GPUs this process can drive (0: none).  Replaces: the executor count Spark reports to the driver
  * (reference base_search.py:62 sc.parallelize(..., len(tasks)) leaves placement to Spark); the in-process scheduler of
  * spark_sklearn_b200/base_search.py opens one handle per device and deals the candidates over them. */
 int gs_device_count(void);
@@ -182,7 +182,7 @@ int gs_debug_gram(gs_handle *h, double *S_out, double *xsq_out);
 /* K_out [n][n] float32 kernel matrix (the SMO solver's Q without the y_i*y_j sign), original order. */
 int gs_debug_kernel_matrix(gs_handle *h, int32_t kernel, double gamma, float *K_out);
 
-/* C[M][N] = sum_k A[M][k]*B[N][k] on the tcgen05 tensor-core path (3xTF32 split), host fp32 row-major in/out. */
+/* C[M][N] = sum_k A[M][k]*B[N][k] on the wgmma tensor-core path (3xTF32 split), host fp32 row-major in/out. */
 int gs_debug_gemm_nt(gs_handle *h, const float *A, int32_t M, const float *B, int32_t N, int32_t K, float *C);
 
 /* ---- planning helpers (host only, no device work; used by gs_svc itself and by the multi-GPU host driver) -------- */
@@ -216,7 +216,7 @@ typedef struct gs_profile {
     double gram_bytes;         /* algorithmic bytes of the Gram build                           */
     int64_t h2d_bytes;         /* bytes copied host->device by gs_set_data + the search         */
     int64_t d2h_bytes;         /* bytes copied device->host by the search                       */
-    float ms_tensor;           /* CUDA-event time of the tcgen05 contraction launches of the call */
+    float ms_tensor;           /* CUDA-event time of the wgmma contraction launches of the call */
     double tensor_flops;       /* TF32 tensor-core flops those launches executed (3 MMAs per product) */
 } gs_profile;
 int gs_get_profile(const gs_handle *h, gs_profile *out);

@@ -1,4 +1,4 @@
-"""Search driver: the B200 counterpart of ``SparkBaseSearchCV._fit``
+"""Search driver: the H100 counterpart of ``SparkBaseSearchCV._fit``
 (reference python/spark_sklearn/base_search.py:21-175).
 
 Same steps, same order, same result layout as the reference -- ``check_cv`` / reseed

@@ -1,4 +1,4 @@
-"""Build libb200gs.so in-tree with nvcc for sm_100a (cross-compiles without a GPU)."""
+"""Build libb200gs.so in-tree with nvcc for sm_90a (cross-compiles without a GPU)."""
 import os
 import subprocess
 import sys
@@ -7,7 +7,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libb200gs.so")
 SOURCES = ["api.cu", "gram.cu", "smo.cu", "smo_lean.cu", "smo_colown.cu", "score.cu", "linear.cu", "logreg.cu", "gemm_tc.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-cudart", "static"]
 
 

@@ -151,7 +151,7 @@ int gs_device_count(void)
     if (cudaGetDeviceCount(&count) != cudaSuccess) return 0;
     for (int d = 0; d < count; d++) {
         cudaDeviceProp prop;
-        if (cudaGetDeviceProperties(&prop, d) == cudaSuccess && prop.major == 10) usable = d + 1;   // handles index devices 0..n-1
+        if (cudaGetDeviceProperties(&prop, d) == cudaSuccess && prop.major == 9 && prop.minor == 0) usable = d + 1;   // handles index devices 0..n-1
     }
     return usable;
 }
@@ -171,8 +171,8 @@ int gs_create(int device, gs_handle **out)
     if (device < 0 || device >= count) { g_create_error = "device index out of range"; return GS_ERR_ARG; }
     cudaDeviceProp prop;
     if ((e = cudaGetDeviceProperties(&prop, device)) != cudaSuccess) { g_create_error = cudaGetErrorString(e); return GS_ERR_CUDA; }
-    if (prop.major != 10) {
-        g_create_error = "libb200gs is built for sm_100a only; device is sm_" + std::to_string(prop.major * 10 + prop.minor);
+    if (prop.major != 9 || prop.minor != 0) {
+        g_create_error = "libb200gs is built for sm_90a only; device is sm_" + std::to_string(prop.major * 10 + prop.minor);
         return GS_ERR_UNSUPPORTED;
     }
     if ((e = cudaSetDevice(device)) != cudaSuccess) { g_create_error = cudaGetErrorString(e); return GS_ERR_CUDA; }
@@ -342,10 +342,10 @@ extern "C" double gs_svc_predicted_iterations(int32_t kernel, double C, double g
 
 // Number n of (predicted-longest) problems on 4-CTA clusters that minimises the predicted makespan
 //   f(n) = max( throughput bound [sum_rest + 2.0 * sum_clustered] / SMs,   (a cluster iteration costs 2x the SM-time)
-//               0.9 * cost of the longest problem left on one SM,         (tail of the run: 6.4 vs 7.1 us per iteration)
-//               0.5 * cost of the longest clustered problem )             (3.5 vs 7.1 us per iteration)
+//               0.9 * cost of the longest problem left on one SM,         (tail of the run: a problem alone runs faster)
+//               0.5 * cost of the longest clustered problem )             (a cluster halves the time per iteration)
 // in units of (predicted iterations x single-CTA iteration time); only cost RATIOS matter.  Near-ties go to the smaller n
-// (measured on config 2: 10 clusters 297 ms, 14 clusters 313 ms, 19 clusters 323 ms -- the model is optimistic about clusters).
+// (on config 2 more clusters than it picks made the solve slower on the 148-SM GPU the kernels were first tuned on: the model is optimistic about clusters).
 extern "C" int32_t gs_svc_cluster_count(const double *cost_desc, int32_t n, int32_t sm_count)
 {
     if (!cost_desc || n < 2 || sm_count < 4) return 0;
@@ -364,8 +364,10 @@ extern "C" int32_t gs_svc_cluster_count(const double *cost_desc, int32_t n, int3
 
 // Three-tier schedule of the slot-layout solver (smo_lean.cu): how many of the predicted-longest problems go on 4-CTA
 // clusters (n_cluster) and how many of the next-longest get an SM to themselves (n_exclusive); the rest run two per SM.
-// Measured per-iteration times of an 8000-row sub-problem (profiles/r02_smo_*): 3.55 us on a 4-CTA cluster, 5.4-5.5 us alone on
-// an SM (1024 threads x 8 slots), 10.5 us when two share an SM (= 5.25 us of SM time per iteration; a cluster costs 14.2).  Only the RATIOS enter:
+// Per-iteration times of an 8000-row sub-problem, calibrated on the 148-SM GPU the kernels were first tuned on: 3.55 us on a 4-CTA cluster,
+// 5.4-5.5 us alone on an SM (1024 threads x 8 slots), 10.5 us when two share an SM (= 5.25 us of SM time per iteration; a
+// cluster costs 14.2).  Only the RATIOS enter; on an H100 (config 2, B200GS_SMO_TIMELINE) cluster and alone-on-an-SM run at
+// 3.7 and 5.5-5.8 us, the same ratio.
 //   T(n_cl, n_ex) = max( 0.34 c[0]                                       longest clustered problem
 //                        0.52 c[n_cl]                                    longest exclusive problem
 //                        0.50 sum(rest) / SMs left, 0.78 c[n_cl + n_ex]  shared SMs: throughput, and the longest shared
@@ -396,14 +398,9 @@ static void schedule_closed_form(const double *cost_desc, int32_t n, int32_t sm_
 
 // Alternative (B200GS_SCHEDULE=simulate; also the test hook gs_svc_simulate): the makespan of a candidate split is SIMULATED,
 // not bounded by a formula: the block scheduler hands every SM that a finished cluster or exclusive problem gives back to
-// the pending CTAs of the shared launch, so "SMs left for the shared tier" is not a constant.  Measured (1 x B200 and
-// 8 x B200, tools/exp_sched2.sh, tools/exp_scale8.sh): config 2 255.0 vs 254.7 ms of solve, config 4 identical, the 8-GPU
-// weak-scaling step 321.9 vs 315.7 ms (its choice of 15 clusters for the ranks that hold a second class of long problems
-// did not shorten their solve phase) -- no gain, so the closed form above stays the default.  Inputs are the measured
-// per-iteration times of an 8000-row sub-problem (profiles/r02_smo_*; only their RATIOS matter): 3.55 us on a 4-CTA
-// cluster, 5.45 us alone on an SM, 9.4 us each when two share an SM.  Checked against tier timelines measured on config 2
-// (B200GS_SMO_TIMELINE) and against forced splits of config 4 (0 / 20 / 40 / 70 exclusive problems: the order is right,
-// the values 3 % high).
+// the pending CTAs of the shared launch, so "SMs left for the shared tier" is not a constant.  It was no faster than the
+// closed form above where it was calibrated (148-SM GPUs), so that stays the default.  Inputs: per-iteration time RATIOS of
+// an 8000-row sub-problem from the same calibration: 3.55 us on a 4-CTA cluster, 5.45 alone on an SM, 9.4 when two share one.
 namespace {
 constexpr double RATE_CLUSTER = 3.55, RATE_SOLO = 5.45, RATE_PAIR = 9.4;
 
@@ -567,7 +564,7 @@ static int svc_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
     tm.mark(-1);
 
     // ---- 1. Gram X X^T (shared by every candidate, fold and pair) ----
-    // default: float64 on the FP64 pipe (libsvm-faithful, gram.cu).  GS_GRAM_TENSOR: tcgen05 tensor cores, 3xTF32 split,
+    // default: float64 on the FP64 pipe (libsvm-faithful, gram.cu).  GS_GRAM_TENSOR: wgmma tensor cores, 3xTF32 split,
     // TMA-fed (gemm_tc.cu) -- fp32-faithful, so scores agree with scikit-learn to solver tolerance, not bit for bit.
     GS_CUDA(h->dS.reserve((size_t)n * n * 8));
     GS_CUDA(h->dXsq.reserve((size_t)n * 8));
@@ -670,7 +667,7 @@ static int svc_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
     int gpb = n_groups;
     if (h->dK.cap < kbytes * (size_t)n_groups) {
         // Ask the driver only when the buffer has to grow: cudaMemGetInfo takes anything from 0.1 to 100+ ms on a busy box
-        // (measured as 16-119 ms outliers of this phase with the Gram already in flight), and a repeated search of the same
+        // (it showed as outliers of this phase with the Gram already in flight), and a repeated search of the same
         // shape needs no new plan.
         size_t free_b = 0, total_b = 0;
         GS_CUDA(cudaMemGetInfo(&free_b, &total_b));
@@ -815,13 +812,11 @@ static int svc_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
         pf.h2d_bytes += (size_t)np * sizeof(SmoProblem) + (size_t)np * 4 + vtasks.size() * sizeof(VoteTask);
         tm.mark(4);
         // -- solve --
-        // Policy (measured on config 2 / config 4, profiles/): a 4-CTA cluster solves one problem at 3.5 us per iteration
-        // against 6.4-7.1 us for the single-CTA kernel, but costs twice the SM-time per iteration.  So clusters are for the
-        // critical path only:
+        // Policy: a 4-CTA cluster solves one problem in about half the time per iteration of the single-CTA kernel, but costs
+        // twice the SM-time per iteration.  So clusters are for the critical path only:
         //   * fewer problems than SMs: everything on the widest cluster that fits;
         //   * otherwise the number of clustered problems minimises a three-term makespan model (below): none for a
-        //     throughput-bound search (config 4), exactly the ten 66-68k-iteration problems for config 2 (leaving ONE of
-        //     them on a single SM costs +33 %), nineteen for the denser 8-GPU weak-scaling grid.
+        //     throughput-bound search (config 4), exactly the ten 66-68k-iteration problems for config 2 (at 148 and 132 SMs).
         // Development switches: B200GS_SMO_CLUSTER (0/2/4/8),
         // B200GS_SMO_CLUSTER_N.
         std::string why;
@@ -841,7 +836,7 @@ static int svc_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
             }
             return cudaSuccess;
         };
-        // Policy (measured on config 2 / config 4, profiles/): clusters and exclusive SMs buy LATENCY for the critical path at
+        // Policy: clusters and exclusive SMs buy LATENCY for the critical path at
         // the price of SM time (gs_svc_schedule above); a throughput-bound search (config 4) uses neither.
         //   * fewer problems than SMs: everything on the widest cluster that fits;
         //   * otherwise the three-tier schedule of the slot-layout kernel, or -- when a problem has no slot layout -- the
@@ -868,7 +863,7 @@ static int svc_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
         n_ex = std::max(0, std::min(n_ex, np - n_cl));
         if (n_cl > 0 || n_ex > 0) {
             // The latency tiers must get their SMs before the shared-SM launch floods the GPU (a late start of the critical
-            // path costs the makespan that much: measured 292 vs 333 ms when the order of arrival flipped).  So the cluster
+            // path costs the makespan that much).  So the cluster
             // kernel goes on the engine stream itself, in order behind the uploads; the exclusive and the shared launches go
             // on two more streams behind the same point plus a 30 / 60 us delay kernel; the engine stream joins them afterwards.
             cudaEvent_t ready = h->evp.get();

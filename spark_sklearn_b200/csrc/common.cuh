@@ -1,4 +1,4 @@
-// common.cuh -- shared declarations of the libb200gs.so translation units (sm_100a only).
+// common.cuh -- shared declarations of the libb200gs.so translation units (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -87,7 +87,7 @@ __device__ __forceinline__ bool split_train(const SplitMasks &m, int r, int k)  
 
 struct gs_handle {
     int device = 0;
-    int sm_count = 148;
+    int sm_count = 132;
     cudaStream_t stream = nullptr;
     cudaStream_t stream_hi = nullptr;   // second stream: the single-CTA SMO launch when a cluster launch runs beside it
     cudaStream_t stream_lo = nullptr;   // third stream: the shared-SM launch when cluster and exclusive-SM launches run beside it
@@ -177,7 +177,7 @@ cudaError_t launch_smo_colown(const SmoProblem *d_probs, const int *d_order, int
 // dec[c][r] = sum_j k64(r, j) * coef[c][j]  (float64 kernel values recomputed from S, not the
 // float32-rounded K: svm.cpp:2821 svm_predict_values uses k_function in double).
 // decision_chunks: into how many slabs the support-row range of one launch is split so that its CTAs fill the GPU in whole
-// rounds (157 row blocks on 592 resident CTAs: 4 slabs = 628 CTAs = two rounds for 1.06 rounds of work; 15 slabs = 3.98).
+// rounds (157 row blocks on 528 resident CTAs of 132 SMs: 4 slabs = 628 CTAs = two rounds for 1.19 rounds of work; 10 slabs = 2.97).
 int decision_chunks(int n, int ncols, int sms);
 cudaError_t launch_decision(const double *S, const double *xsq, int n, int kernel, double gamma,
                             const double *coef, int ncols, double *dec, double *part, int jchunks, cudaStream_t st);
@@ -202,7 +202,7 @@ cudaError_t launch_auc_pairs_f32(const float *score, int64_t ld, int n, int n_a,
 // score of one (task, split) from the class counts cnt[class][3] (float64, scikit-learn's formulas); NaN when undefined
 double gs_score_from_counts(int kind, int pos_class, int n_classes, const int *cnt);
 
-// ---- gemm_tc.cu: tcgen05 + TMA contraction  C[M][N] = sum_k A[M][k] B[N][k]  (3xTF32 split, fp32 accumulate) ----
+// ---- gemm_tc.cu: wgmma + TMA contraction  C[M][N] = sum_k A[M][k] B[N][k]  (3xTF32 split, fp32 accumulate) ----
 struct alignas(64) TcMap { unsigned char bytes[128]; };            // CUtensorMap
 struct TcBatch {                                                    // one GEMM of a batched launch (blockIdx.z)
     int a_row0, b_row0;   // first row of the A / B operand inside their tensor maps
@@ -212,7 +212,7 @@ struct TcBatch {                                                    // one GEMM 
 };
 cudaError_t tc_make_map(TcMap *out, const float *base, int64_t rows, int64_t cols, int64_t ld);
 cudaError_t launch_split_tf32(const float *x, float *hi, float *lo, size_t n, cudaStream_t st);
-constexpr int TC_KCHUNK = 512;   // longest accumulation chain kept inside the (truncating) TMEM accumulator
+constexpr int TC_KCHUNK = 512;   // longest accumulation chain kept inside the (not round-to-nearest) tensor-core accumulator
 cudaError_t launch_sum_partials(const float *partial, int n_chunks, int64_t per, float *out, cudaStream_t st);
 // symmetric: the A and B operands are the same matrix (M == N): tiles below the diagonal are not computed, their values are
 // stored as transposes of the tiles above it (bitwise symmetric result)

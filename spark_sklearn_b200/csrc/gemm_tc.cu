@@ -1,10 +1,10 @@
-// gemm_tc.cu -- C[M][N] = sum_k A[M][k] * B[N][k]  ("NT", both operands K-major) on the 5th-generation
-// tensor cores: tcgen05.mma kind::tf32 with the accumulator in TMEM, operands staged by TMA
-// (cp.async.bulk.tensor, SWIZZLE_128B) through a 3-stage mbarrier pipeline.  sm_100a only.
+// gemm_tc.cu -- C[M][N] = sum_k A[M][k] * B[N][k]  ("NT", both operands K-major) on the Hopper tensor cores:
+// wgmma.mma_async tf32 with the accumulator in registers, operands staged by TMA (cp.async.bulk.tensor,
+// SWIZZLE_128B) through a 3-stage mbarrier pipeline.  sm_90a only.
 //
 // fp32-faithful on TF32 tensor cores ("3xTF32"): every fp32 operand is pre-split into
 //   hi = x with the low 13 mantissa bits cleared (exactly a TF32 value),  lo = x - hi (exact in fp32)
-// and each K-step issues hi*hi + hi*lo + lo*hi into the same fp32 TMEM accumulator.  The dropped
+// and each K-step issues hi*hi + hi*lo + lo*hi into the same fp32 accumulator.  The dropped
 // lo*lo term and the truncation of lo to 11 bits are ~2^-22 relative, i.e. at the level of the fp32
 // accumulation itself -- the precision scikit-learn's own fp32 BLAS calls have on this path
 // (Ridge: sklearn/linear_model/_ridge.py:215-227 keeps float32 throughout).
@@ -12,19 +12,15 @@
 // Replaces (reference path -> scikit-learn): safe_sparse_dot(X.T, X) of _solve_cholesky (_ridge.py:219),
 // X @ w and X.T @ grad of the logistic objective (_linear_loss.py), and -- opt-in -- the libsvm kernel rows.
 //
-// The TMEM accumulator adds with truncation, so a long contraction drifts by ~sqrt(K)*2^-24 of sum|a||b| -- harmless
+// The fp32 tensor-core accumulator does not round to nearest, so a long contraction drifts by ~sqrt(K)*2^-24 of sum|a||b| -- harmless
 // for a Gram diagonal, ruinous for a heavily cancelled sum such as a gradient near its zero.  Callers therefore
 // bound every accumulation chain to TC_KCHUNK terms (one TcBatch per K-chunk) and add the partial tiles in float64
 // on the CUDA cores (launch_sum_partials).
 //
-// Tile: 128 x 128 x 32 (fp32) per stage.  PERSISTENT, warp-specialised CTAs (one per SM, 6 warps), tiles dealt round-robin:
-//   warp 0 / lane 0: TMA producer (3-stage ring over ALL its tiles -- the ring never drains between tiles)
-//   warp 1 / lane 0: MMA issuer (12 MMAs per stage) into one of TWO 128-column TMEM accumulators
-//   warps 2-5: epilogue of the other accumulator: tcgen05.ld 32x32b.x32 -> padded shared-memory transpose -> COALESCED
-//              global stores (a TMEM lane is a tile row: storing straight from registers touches 32 cache lines per request).
-// The contractions of this package are short (K <= TC_KCHUNK = 512 per accumulation chain, see above), so a tile is
-// ~16 k-steps: with one tile per CTA the barrier/TMEM set-up and the epilogue were half of its life (31 % tensor pipe,
-// profiles/r01_gram_tc_ncu_summary.txt); now they overlap the next tile's main loop.
+// Tile: 128 x 128 x 32 (fp32) per stage.  PERSISTENT, warp-specialised CTAs (one per SM, 9 warps), tiles dealt round-robin:
+//   warps 0-7 (two warpgroups): warpgroup g owns tile rows [64 g, 64 g + 64) in 64 fp32 registers per thread, issues 12
+//              wgmma m64n128k8 per stage and stores straight from the accumulator fragment (float2 column pairs)
+//   warp 8 / lane 0: TMA producer (3-stage ring over ALL tiles of the CTA: the next tile loads during the last one's stores)
 // symmetric (A == B, M == N): only tiles on or above the diagonal are computed and their transposes stored too.
 // Batched: per-batch row offsets into A and B, K range and output pointer.
 #include "common.cuh"
@@ -38,15 +34,8 @@ constexpr int BM = 128, BN = 128, BK = 32;            // BK fp32 = 128 B = one S
 constexpr int STAGES = 3;
 constexpr int TILE_BYTES = BM * BK * 4;               // 16 KB per operand tile
 constexpr int STAGE_BYTES = 4 * TILE_BYTES;           // A_hi, A_lo, B_hi, B_lo
-constexpr int EPI_WARPS = 4, NTHREADS = 64 + EPI_WARPS * 32;
-constexpr int STG_LD = 33;                            // padded row of the epilogue transpose buffers
-constexpr int STG_BYTES = EPI_WARPS * 32 * STG_LD * 4;
-constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + STG_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
-constexpr uint32_t TMEM_COLS = 256;                   // two 128-column fp32 accumulators
-
-// instruction descriptor (cute/arch/mma_sm100_desc.hpp InstrDescriptor): c_format F32 (1) @4, a/b format
-// TF32 (2) @7/@10, K-major both, N>>3 @17, M>>4 @24
-constexpr uint32_t IDESC = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
+constexpr int CONSUMER_WARPS = 8, NTHREADS = (CONSUMER_WARPS + 1) * 32;
+constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -75,21 +64,38 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap *map
     asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
                  ::"r"(dst), "l"(map), "r"(c0), "r"(c1), "r"(bar) : "memory");
 }
-// shared-memory matrix descriptor, K-major, SWIZZLE_128B (cute SmemDescriptor): start>>4 @0, LBO=1 @16,
-// SBO = 8 rows * 128 B = 1024 B (>>4 = 64) @32, version 1 @46, layout_type 2 (SWIZZLE_128B) @61
+// wgmma shared-memory matrix descriptor, K-major, SWIZZLE_128B: start>>4 @0, LBO (unused for swizzled K-major) = 1 @16,
+// SBO = 8 rows * 128 B = 1024 B (>>4 = 64) @32, base offset 0 (every operand tile is 1024-byte aligned), layout 1 (128B) @62
 __device__ __forceinline__ uint64_t make_desc(uint32_t saddr)
 {
-    return (uint64_t)((saddr >> 4) & 0x3fff) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
+    return (uint64_t)((saddr >> 4) & 0x3fff) | (1ull << 16) | (64ull << 32) | (1ull << 62);
 }
-__device__ __forceinline__ void umma_tf32(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t accumulate)
+
+// d[64] += A[64 x 8] * B[128 x 8]^T, tf32 operands from shared memory; fragment of thread (warp w, lane l) of the
+// warpgroup: d[4 j + 2 h + e] = row 16 w + l / 4 + 8 h, column 8 j + 2 (l % 4) + e
+__device__ __forceinline__ void wgmma_tf32(float (&d)[64], uint64_t adesc, uint64_t bdesc)
 {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-                 "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-                 ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(IDESC), "r"(accumulate) : "memory");
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, "
+                 "%23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, "
+                 "%44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+                 "%64, %65, p, 1, 1;\n\t}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+                   "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+                   "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+                   "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+                   "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+                   "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+                   "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+                   "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+                 : "l"(adesc), "l"(bdesc), "r"(1));
 }
-__device__ __forceinline__ void umma_commit(uint32_t bar)
+// keeps the compiler from moving accumulator reads or writes across the asynchronous wgmma window
+__device__ __forceinline__ void fence_acc(float (&d)[64])
 {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
+#pragma unroll
+    for (int i = 0; i < 64; i++) asm volatile("" : "+f"(d[i])::"memory");
 }
 
 __device__ __forceinline__ void mbar_arrive(uint32_t bar)
@@ -109,6 +115,12 @@ __device__ __forceinline__ void decode_tile(int t, int tiles_m, int tiles_n, int
     ni = mi + r;
 }
 
+__device__ __forceinline__ void store_c(float *c, int64_t ldc, int row, int col, float v, int accumulate_c)
+{
+    float *dst = c + (size_t)row * ldc + col;
+    *dst = accumulate_c ? *dst + v : v;
+}
+
 __global__ void __launch_bounds__(NTHREADS, 1)
 gemm_nt_tf32x3_kernel(const __grid_constant__ CUtensorMap a_hi, const __grid_constant__ CUtensorMap a_lo,
                       const __grid_constant__ CUtensorMap b_hi, const __grid_constant__ CUtensorMap b_lo,
@@ -116,30 +128,19 @@ gemm_nt_tf32x3_kernel(const __grid_constant__ CUtensorMap a_hi, const __grid_con
 {
     extern __shared__ unsigned char smem_dyn[];
     unsigned char *smem = (unsigned char *)(((uintptr_t)smem_dyn + 1023) & ~(uintptr_t)1023);
-    float *stg_all = reinterpret_cast<float *>(smem + STAGES * STAGE_BYTES);
-    uint64_t *bars = reinterpret_cast<uint64_t *>(smem + STAGES * STAGE_BYTES + STG_BYTES);   // full[S], empty[S], tfull[2], tempty[2]
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(bars + 2 * STAGES + 4);
+    uint64_t *bars = reinterpret_cast<uint64_t *>(smem + STAGES * STAGE_BYTES);   // full[S], empty[S]
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int tiles_m = (M + BM - 1) / BM, tiles_n = (N + BN - 1) / BN;
     const int n_tiles = n_batches * (symmetric ? tiles_m * (tiles_m + 1) / 2 : tiles_m * tiles_n);
-    const uint32_t b_full = smem_u32(&bars[0]), b_empty = smem_u32(&bars[STAGES]), b_tfull = smem_u32(&bars[2 * STAGES]),
-                   b_tempty = smem_u32(&bars[2 * STAGES + 2]);
+    const uint32_t b_full = smem_u32(&bars[0]), b_empty = smem_u32(&bars[STAGES]);
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < STAGES; s++) { mbar_init(b_full + 8 * s, 1); mbar_init(b_empty + 8 * s, 1); }
-        for (int q = 0; q < 2; q++) { mbar_init(b_tfull + 8 * q, 1); mbar_init(b_tempty + 8 * q, EPI_WARPS); }
+        for (int s = 0; s < STAGES; s++) { mbar_init(b_full + 8 * s, 1); mbar_init(b_empty + 8 * s, CONSUMER_WARPS); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
+    if (warp == CONSUMER_WARPS) {
         if (lane == 0) {
             // ---------------- TMA producer: one ring over all tiles of this CTA ----------------
             int it = 0;
@@ -163,113 +164,75 @@ gemm_nt_tf32x3_kernel(const __grid_constant__ CUtensorMap a_hi, const __grid_con
                 }
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            // ---------------- MMA issuer: accumulator buffers alternate between tiles ----------------
-            int it = 0, ti = 0;
-            for (int t = blockIdx.x; t < n_tiles; t += gridDim.x, ti++) {
-                int z, mi, ni;
-                decode_tile(t, tiles_m, tiles_n, symmetric, z, mi, ni);
-                const TcBatch bt = batches[z];
-                const int nkb = (bt.k1 - bt.k0 + BK - 1) / BK;
-                const int buf = ti & 1;
-                mbar_wait(b_tempty + 8 * buf, (((uint32_t)ti >> 1) & 1u) ^ 1u);      // the epilogue drained this accumulator
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t d_tmem = tmem_base + (uint32_t)(buf * BN);
-                for (int kb = 0; kb < nkb; kb++, it++) {
-                    const int s = it % STAGES;
-                    const uint32_t ph = (uint32_t)(it / STAGES) & 1u;
-                    mbar_wait(b_full + 8 * s, ph);                               // TMA bytes landed
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                    const uint32_t base = smem_u32(smem + s * STAGE_BYTES);
-                    const uint64_t dah = make_desc(base), dal = make_desc(base + TILE_BYTES);
-                    const uint64_t dbh = make_desc(base + 2 * TILE_BYTES), dbl = make_desc(base + 3 * TILE_BYTES);
+        return;
+    }
+
+    // ---------------- consumers: warpgroup wg computes and stores rows [64 wg, 64 wg + 64) of every tile ----------------
+    const int wg = warp >> 2;
+    const uint32_t a_off = (uint32_t)wg * 64 * BK * 4;                            // 8 KB: a multiple of the 1 KB swizzle atom
+    float d[64];
+    int it = 0;
+    for (int t = blockIdx.x; t < n_tiles; t += gridDim.x) {
+        int z, mi, ni;
+        decode_tile(t, tiles_m, tiles_n, symmetric, z, mi, ni);
+        const TcBatch bt = batches[z];
+        const int nkb = (bt.k1 - bt.k0 + BK - 1) / BK;
 #pragma unroll
-                    for (int k = 0; k < BK / 8; k++) {                           // UMMA_K = 8 for tf32: 32 B per step
-                        const uint64_t off = (uint64_t)(k * 32 >> 4);            // advance inside the swizzle atom
-                        umma_tf32(d_tmem, dah + off, dbh + off, (kb | k) != 0);
-                        umma_tf32(d_tmem, dah + off, dbl + off, 1);
-                        umma_tf32(d_tmem, dal + off, dbh + off, 1);
-                    }
-                    umma_commit(b_empty + 8 * s);                                // frees the smem slot when the MMAs retire
-                }
-                umma_commit(b_tfull + 8 * buf);                                  // accumulator complete
+        for (int i = 0; i < 64; i++) d[i] = 0.f;
+        for (int kb = 0; kb < nkb; kb++, it++) {
+            const int s = it % STAGES;
+            mbar_wait(b_full + 8 * s, (uint32_t)(it / STAGES) & 1u);            // TMA bytes landed
+            const uint32_t base = smem_u32(smem + s * STAGE_BYTES);
+            const uint64_t dah = make_desc(base + a_off), dal = make_desc(base + TILE_BYTES + a_off);
+            const uint64_t dbh = make_desc(base + 2 * TILE_BYTES), dbl = make_desc(base + 3 * TILE_BYTES);
+            fence_acc(d);
+            asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+#pragma unroll
+            for (int k = 0; k < BK / 8; k++) {                                   // K = 8 per tf32 wgmma: 32 B per step
+                const uint64_t off = (uint64_t)(k * 32 >> 4);                    // advance inside the swizzle atom
+                wgmma_tf32(d, dah + off, dbh + off);
+                wgmma_tf32(d, dah + off, dbl + off);
+                wgmma_tf32(d, dal + off, dbh + off);
             }
+            asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+            // the previous stage's group has retired: its slot may be refilled while this one runs
+            asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory");
+            fence_acc(d);
+            if (kb > 0 && lane == 0) mbar_arrive(b_empty + 8 * ((it - 1) % STAGES));
         }
-    } else {
-        // ---------------- epilogue warps: TMEM -> registers -> smem transpose -> coalesced global ----------------
-        const int q = warp & 3;                                                  // the TMEM lane quarter this warp may read
-        float *stg = stg_all + (size_t)(warp - 2) * 32 * STG_LD;
-        int ti = 0;
-        for (int t = blockIdx.x; t < n_tiles; t += gridDim.x, ti++) {
-            int z, mi, ni;
-            decode_tile(t, tiles_m, tiles_n, symmetric, z, mi, ni);
-            const TcBatch bt = batches[z];
-            const int nkb = (bt.k1 - bt.k0 + BK - 1) / BK;
-            const int buf = ti & 1;
-            mbar_wait(b_tfull + 8 * buf, ((uint32_t)ti >> 1) & 1u);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const int m0 = mi * BM + q * 32, n0 = ni * BN;
-            const bool diag = symmetric && mi == ni;       // diagonal tile: store j >= i, mirror the strict upper part (bitwise symmetric:
-                                                           // the hi*lo and lo*hi products of C[i][j] and C[j][i] accumulate in swapped order)
-            const bool mirror = symmetric != 0;
-#pragma unroll 1
-            for (int c0 = 0; c0 < BN; c0 += 32) {
-                uint32_t r[32];
-                if (nkb > 0) {
-                    const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf * BN + c0);
-                    asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                                 "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-                                   "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-                                   "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-                                   "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-                                 : "r"(taddr));
-                    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                } else {
+        asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+        fence_acc(d);
+        if (nkb > 0 && lane == 0) mbar_arrive(b_empty + 8 * ((it - 1) % STAGES));
+
+        // ---------------- epilogue: straight from the accumulator fragment to global memory ----------------
+        const int r0 = mi * BM + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+        const int c0 = ni * BN + 2 * (lane & 3);
+        const bool diag = symmetric && mi == ni;       // diagonal tile: store j >= i, mirror the strict upper part (bitwise symmetric:
+                                                       // the hi*lo and lo*hi products of C[i][j] and C[j][i] accumulate in swapped order)
+        // columns col, col + 1 of a row are one float2 (4 lanes fill a 32-byte sector) except on diagonal tiles and odd ldc;
+        // mirrored stores: 8 lanes write 8 consecutive floats of one row of C
+        const bool vec = !diag && (bt.ldc & 1) == 0 && ((uintptr_t)bt.c & 7) == 0;
 #pragma unroll
-                    for (int j = 0; j < 32; j++) r[j] = 0u;
-                }
-#pragma unroll
-                for (int j = 0; j < 32; j++) stg[lane * STG_LD + j] = alpha * __uint_as_float(r[j]);   // lane == tile row
-                __syncwarp();
-                const int col = n0 + c0 + lane;
-                if (col < N) {
-#pragma unroll 4
-                    for (int rr = 0; rr < 32; rr++) {                            // a warp request = 32 consecutive columns of one row
-                        const int row = m0 + rr;
-                        if (row < M && !(diag && col < row)) {
-                            float *dst = bt.c + (size_t)row * bt.ldc + col;
-                            const float v = stg[rr * STG_LD + lane];
-                            *dst = accumulate_c ? *dst + v : v;
-                        }
-                    }
-                }
-                if (mirror) {                                                    // C[n][m] = C[m][n]: columns become rows
-                    const int mcol = m0 + lane;
-                    if (mcol < M) {
-#pragma unroll 4
-                        for (int jj = 0; jj < 32; jj++) {
-                            const int mrow = n0 + c0 + jj;
-                            if (mrow < N && !(diag && mrow <= mcol)) {
-                                float *dst = bt.c + (size_t)mrow * bt.ldc + mcol;
-                                const float v = stg[lane * STG_LD + jj];
-                                *dst = accumulate_c ? *dst + v : v;
-                            }
-                        }
-                    }
-                }
-                __syncwarp();
+        for (int i = 0; i < 64; i += 2) {
+            const int row = r0 + 8 * ((i >> 1) & 1), col = c0 + 8 * (i >> 2);
+            if (row >= M || col >= N) continue;
+            const float v0 = alpha * d[i], v1 = alpha * d[i + 1];
+            const bool two = col + 1 < N;
+            if (vec && two) {
+                float2 *dst = reinterpret_cast<float2 *>(bt.c + (size_t)row * bt.ldc + col);
+                float2 o = make_float2(v0, v1);
+                if (accumulate_c) { const float2 p = *dst; o.x += p.x; o.y += p.y; }
+                *dst = o;
+            } else {
+                if (!(diag && col < row)) store_c(bt.c, bt.ldc, row, col, v0, accumulate_c);
+                if (two && !(diag && col + 1 < row)) store_c(bt.c, bt.ldc, row, col + 1, v1, accumulate_c);
             }
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            if (lane == 0) mbar_arrive(b_tempty + 8 * buf);                      // this warp has drained its quarter
+            if (symmetric) {                                                     // C[n][m] = C[m][n]
+                if (!(diag && col <= row)) store_c(bt.c, bt.ldc, col, row, v0, accumulate_c);
+                if (two && !(diag && col + 1 <= row)) store_c(bt.c, bt.ldc, col + 1, row, v1, accumulate_c);
+            }
         }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 1)
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
 }
 
 // hi = x with the low 13 mantissa bits cleared (a TF32 value), lo = x - hi (exact)
@@ -329,13 +292,13 @@ cudaError_t tc_make_map(TcMap *out, const float *base, int64_t rows, int64_t col
 
 cudaError_t launch_sum_partials(const float *partial, int n_chunks, int64_t per, float *out, cudaStream_t st)
 {
-    sum_partials_kernel<<<(unsigned)std::min<int64_t>((per + 255) / 256, 1184), 256, 0, st>>>(partial, n_chunks, per, out);
+    sum_partials_kernel<<<(unsigned)std::min<int64_t>((per + 255) / 256, 1056), 256, 0, st>>>(partial, n_chunks, per, out);
     return cudaGetLastError();
 }
 
 cudaError_t launch_split_tf32(const float *x, float *hi, float *lo, size_t n, cudaStream_t st)
 {
-    split_tf32_kernel<<<592, 256, 0, st>>>(x, hi, lo, n);
+    split_tf32_kernel<<<528, 256, 0, st>>>(x, hi, lo, n);
     return cudaGetLastError();
 }
 
@@ -347,7 +310,7 @@ cudaError_t launch_gemm_nt_tf32x3(const TcMap &a_hi, const TcMap &a_lo, const Tc
     cudaError_t e = cudaFuncSetAttribute(gemm_nt_tf32x3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
     if (e != cudaSuccess) return e;
     if (symmetric && M != N) return cudaErrorInvalidValue;
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const int tm = (M + BM - 1) / BM, tn = (N + BN - 1) / BN;
     const long long tiles = (long long)n_batches * (symmetric ? (long long)tm * (tm + 1) / 2 : (long long)tm * tn);

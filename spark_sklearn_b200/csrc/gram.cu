@@ -1,4 +1,4 @@
-// gram.cu -- float64 Gram matrix and float32 kernel-matrix materialisation (sm_100a).
+// gram.cu -- float64 Gram matrix and float32 kernel-matrix materialisation (sm_90a).
 //
 // Why float64 here: libsvm (sklearn svm.cpp:336-347, 1439-1449) evaluates every kernel entry in
 // float64 from float64 features and only then rounds to float32 (Qfloat).  X arrives as float32,
@@ -6,7 +6,7 @@
 // BLAS ddot only in summation order (~1e-16 relative); after the exp and the float32 rounding the
 // stored Q entries agree with libsvm's on all but ~2^-29 of the entries.  That is what lets the
 // SMO kernel reproduce libsvm's iterate sequence, and therefore its scores, bit for bit.  A
-// tensor-core (tcgen05) Gram cannot do this: fp32 accumulation perturbs every entry by a few ulp.
+// tensor-core (wgmma) Gram cannot do this: fp32 accumulation perturbs every entry by a few ulp.
 //
 // gram_f64_kernel: S = X X^T, 128x128 output tile per CTA, 8x8 float64 micro-tile per thread,
 // upper-triangular tiles only (mirror-written), operands converted to float64 once when staged

@@ -3,7 +3,7 @@
 // Ridge path (replaces sklearn Ridge.fit/score reached from reference base_search.py:83-87:
 // linear_model/_ridge.py:919 fit, :964 _preprocess_data centring, :215-227 _solve_cholesky, base.py:716 r2):
 //   1. Z = [X | y | 1]  (n x (d+2)); per CV fold k the Gram  G_k = Z_k^T Z_k  holds X^T X, X^T y, column sums,
-//      y^T y, sum y and the row count of the fold at once.  One tcgen05 contraction per fold (gemm_tc.cu, 3xTF32
+//      y^T y, sum y and the row count of the fold at once.  One wgmma contraction per fold (gemm_tc.cu, 3xTF32
 //      split, K-range = the fold's contiguous rows).  scikit-learn recomputes X^T X for each of the
 //      n_alpha x n_folds fits (SURVEY.md 8a-a9); here it is built ONCE and the training statistics of fold k are
 //      T - G_k with T = sum_k G_k (float64).
@@ -82,7 +82,7 @@ __global__ void build_zt_kernel(const float *__restrict__ X, const float *__rest
     }
 }
 
-// The Gram of a row block is contracted in chunks of <= TC_KCHUNK rows (the TMEM accumulator truncates); the chunk
+// The Gram of a row block is contracted in chunks of <= TC_KCHUNK rows (the tensor-core accumulator does not round to nearest); the chunk
 // partials Gq are added here in float64: G_b = sum of the chunks of block b (chunks qs[b] .. qs[b+1]), T = sum_b G_b.
 __global__ void sum_grams_kernel(const float *__restrict__ Gq, const int *__restrict__ qs, int n_blocks, int n_plain, int64_t per,
                                  float *__restrict__ G, double *__restrict__ T, double *__restrict__ Tw)
@@ -675,7 +675,7 @@ int ridge_run(gs_handle *h, int n_cand, const double *alpha, int fit_intercept, 
     h->tt.begin(h->evp, st);
     GS_CUDA(launch_gemm_nt_tf32x3(mzh, mzl, mzh, mzl, dBatchG, nq, D, D, 1.0f, false, st, true));   // Gram: upper tiles + mirror
     h->tt.end(h->evp, st, 3.0 * 2.0 * (double)D * D * (double)ldz * (((D + 127) / 128 + 1) / (2.0 * ((D + 127) / 128))));   // tiles on/above the diagonal
-    sum_grams_kernel<<<592, 256, 0, st>>>(dGq, dQs, nb, nb_plain, (int64_t)Dp * Dp, bG.as<float>(), dT, weighted ? dTw : nullptr);
+    sum_grams_kernel<<<528, 256, 0, st>>>(dGq, dQs, nb, nb_plain, (int64_t)Dp * Dp, bG.as<float>(), dT, weighted ? dTw : nullptr);
     GS_CUDA(cudaGetLastError());
     launches += 5;
     cudaEventRecord(ev[1], st);

@@ -24,7 +24,7 @@ decision_kernel(const double *__restrict__ S, const double *__restrict__ xsq, in
 {
     // blockIdx.z = chunk of the j (support-row) range: chunk z sums j in [z*jlen, (z+1)*jlen) into slab z of `dec`
     // (slab stride ncols*n); sum_slabs_kernel adds the slabs in ascending order.  One chunk per row block leaves one
-    // 8-warp block per SM and a two-wave tail (157 blocks on 148 SMs at n = 10000): 3.1 ms per gamma instead of ~1.
+    // 8-warp block per SM and a two-wave tail (157 blocks on 132 SMs at n = 10000).
     constexpr int CPT = TC / 8;                       // columns per thread
     __shared__ __align__(16) double E[TJ][TR + 2];
     __shared__ __align__(16) double Cf[TJ][TC + 2];
@@ -301,8 +301,8 @@ static int decision_ctas_per_sm(int tc)
 
 // part: workspace of at least jchunks * ncols * n doubles when jchunks > 1.
 // The CTAs of a launch take the same time, so a launch costs ceil(CTAs / resident CTAs) rounds; the slab count with the
-// fewest rounds per unit of work wins (config 2: 40 columns, 4 CTAs/SM -> 15 slabs instead of 4: 3.98 rounds of 1/15 against
-// 2 rounds of 1/4).  Short ranges are not split (each slab keeps >= 8 tiles of TJ support rows).
+// fewest rounds per unit of work wins (config 2 on 132 SMs: 40 columns, 4 CTAs/SM -> 10 slabs instead of 4: 2.97 rounds of 1/10
+// against 2 rounds of 1/4).  Short ranges are not split (each slab keeps >= 8 tiles of TJ support rows).
 int decision_chunks(int n, int ncols, int sms)
 {
     if (n < 4096 || ncols <= 0) return 1;

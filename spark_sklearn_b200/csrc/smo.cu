@@ -21,7 +21,7 @@
 //   G_bar:     mbar_t += fl(c*K_it),  c = -/+ y_i*C_i                                       (:876-905)
 // where K is the UNSIGNED float32 kernel row.  Set membership is two precomputed flag bits.
 //
-// Throughput design (B200: 64 FP64 lanes/SM, 4 issue slots/clk/SM -- this kernel is FP64-pipe and
+// Throughput design (H100: 64 FP64 lanes/SM, 4 issue slots/clk/SM -- this kernel is FP64-pipe and
 // issue bound, then latency bound; see DESIGN.md):
 //   * the exact float64 division of WSS2 is evaluated only for elements that survive an approximate
 //     filter (float32 arithmetic for rbf, a 20-bit reciprocal otherwise) with a provably safe band; the
@@ -45,7 +45,7 @@ using namespace smo;
 // ROWBUF: the two K rows of an iteration are brought into shared memory by ONE bulk asynchronous copy each
 // (cp.async.bulk, mbarrier-signalled) and gathered from there.  A row gathered with per-thread LDGs is throttled by
 // the SM's outstanding-miss capacity (~64 lines x ~900 cycles of DRAM latency = ~18 GB/s per SM, 2.5 us per 32 KB row,
-// measured); the bulk copy streams the whole 40 KB row at the SM's full fill rate.  G_bar then lives in global memory.
+// on the 148-SM GPU the kernels were first tuned on); the bulk copy streams the whole 40 KB row at the SM's full fill rate.  G_bar then lives in global memory.
 template <int NT, int KPT, bool SMEM_STATE, bool FAST, bool PROF, bool ROWBUF>
 __global__ void __launch_bounds__(NT, 1)
 smo_kernel(const SmoProblem *__restrict__ probs, const int *__restrict__ order, int rowcap)
@@ -128,7 +128,7 @@ smo_kernel(const SmoProblem *__restrict__ probs, const int *__restrict__ order, 
     auto fetch_row = [&](int r) {
         if constexpr (ROWBUF) {
             // up to four bulk copies in flight at once (1.7k cycles from HBM for a 40 KB row instead of 2.05k for one copy,
-            // measured), and only the column ranges this sub-problem reads
+            // on the 148-SM GPU the kernels were first tuned on), and only the column ranges this sub-problem reads
             const unsigned bar = (unsigned)__cvta_generic_to_shared(&rowbar);
             if (tid == 0) asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(cp_total * 4u) : "memory");
             if (cp_cnt)

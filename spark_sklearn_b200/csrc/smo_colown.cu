@@ -283,7 +283,7 @@ smo_colown_kernel(const SmoProblem *__restrict__ probs, const int *__restrict__ 
         ph ^= 1u << b;
     };
     // worker <-> leader hand-offs inside the CTA use HARDWARE named barriers (waiting warps are parked, not polling:
-    // fifteen warps spinning on an mbarrier starve the leader of issue slots -- measured 1.9k cycles per stage vs 0.6k)
+    // fifteen warps spinning on an mbarrier starve the leader of issue slots -- 1.9k cycles per stage vs 0.6k on the 148-SM GPU the kernels were first tuned on)
     auto nb_arrive = [&](int id) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(NT) : "memory"); };
     auto nb_sync = [&](int id) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(NT) : "memory"); };
     // leader: send the CTA record (W words, uniform registers c[]) to slot [rank] of every CTA, then wait for all CL records

@@ -711,7 +711,7 @@ smo_lean_kernel(const SmoProblem *__restrict__ probs, const int *__restrict__ or
         load_row(col_j, kvj);                                    // in flight during the scalar update
         // analytic two-variable update.  SOLO: evaluated by EVERY warp (uniform) -- its ~250 dependent instructions run under
         // the row-j fetch that each warp waits for anyway and the CTA needs no third barrier (a single warp computing it kept
-        // the other fifteen parked for ~0.9 us, measured).  Shared SM: warp 0 alone (4000 fewer warp-instructions per iteration).
+        // the other fifteen parked).  Shared SM: warp 0 alone (4000 fewer warp-instructions per iteration).
         double a = 0, b = 0, ai_new = 0, aj_new = 0;
         int sti = 0, stj = 0;
         const bool yi = slot_i < ysplit, yj = slot_j < ysplit;
@@ -972,16 +972,13 @@ cudaError_t launch_smo_lean(const SmoProblem *d_probs, const int *d_order, int n
     if (n_prob <= 0) return cudaSuccess;
     const bool prof = env_int("B200GS_SMO_PROF", 0) != 0;                    // development switch: per-phase cycle counters
     if (env_int("B200GS_SMO_NOFAST", 0)) fast = false;
-    int dev = 0, sms = 148;
-    if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     // Two instances of the two-variable update: warp 0 evaluates it behind a third barrier, or every warp evaluates it
-    // redundantly (SOLO).  Same-box A/B on config 2 (tools/exp_solo2.sh): the barrier instance is faster in BOTH tiers
-    // (exclusive SM: 5.62 vs 5.83-5.92 us per iteration; shared SMs finish at 233 vs 248 ms), so it is the default.
+    // redundantly (SOLO).  The barrier instance is the default: config 2's solve phase takes 331.8 ms with it and 342.2 ms with
+    // SOLO (one H100 SXM capped at 400 W, B200GS_SMO_TIMELINE, same run).
     bool solo = false;
     if (const char *e = getenv("B200GS_LEAN_SOLO")) solo = atoi(e) != 0;      // development switch
-    (void)sms;
-    // A problem alone on its SM spreads over 1024 threads x 8 slots instead of 512 x 16: 5.38-5.49 against 5.65-5.72 us per
-    // iteration on config 2's 8000-row problems (tools/exp_wide.sh; bit-identical trajectories).  B200GS_LEAN_EXCL_WIDE=0: off.
+    // A problem alone on its SM spreads over 1024 threads x 8 slots instead of 512 x 16 (bit-identical trajectories): config 2's
+    // solve phase takes 331.8 ms with it and 352.6 ms without (same H100 run as above).  B200GS_LEAN_EXCL_WIDE=0: off.
     if (exclusive && max_slots > 4096 && max_slots <= 8192 && env_int("B200GS_LEAN_EXCL_WIDE", 1))
         return launch_lean_cfg<1024, 2>(d_probs, d_order, n_prob, fast, prof, exclusive, solo, st);
     if (max_slots <= 2048) return launch_lean_cfg<128, 4>(d_probs, d_order, n_prob, fast, prof, exclusive, solo, st);

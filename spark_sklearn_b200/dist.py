@@ -21,7 +21,7 @@ def rank_world():
 
 
 def local_devices():
-    """GPUs one plain ``fit()`` drives when torch.distributed is NOT initialised: every visible sm_100 device by default
+    """GPUs one plain ``fit()`` drives when torch.distributed is NOT initialised: every visible sm_90 device by default
     (B200GS_DEVICES = "all" | a count | a comma-separated list of indices; "1" keeps the search on one GPU)."""
     import os
     from .engine import device_count

@@ -1,6 +1,6 @@
 """ctypes binding of libb200gs.so (include/b200gs.h) -- the only way the package computes.
 
-There is deliberately no CPU fallback: if the CUDA library is missing or no sm_100 GPU is visible,
+There is deliberately no CPU fallback: if the CUDA library is missing or no sm_90 GPU is visible,
 ``Engine()`` raises.  The oracle under ``oracle/`` is test infrastructure and is never imported here.
 """
 import ctypes
@@ -40,7 +40,7 @@ def load_library():
     if not os.path.exists(LIB_PATH):
         raise RuntimeError(
             "spark_sklearn_b200: %s is missing -- build it with `python -m spark_sklearn_b200.build` "
-            "(nvcc, sm_100a).  There is no CPU fallback." % LIB_PATH)
+            "(nvcc, sm_90a).  There is no CPU fallback." % LIB_PATH)
     L = ctypes.CDLL(LIB_PATH)
     c = ctypes
     vp, i32, i64, u32, dbl = c.c_void_p, c.c_int32, c.c_int64, c.c_uint32, c.c_double
@@ -95,7 +95,7 @@ _device_count = None
 
 
 def device_count():
-    """sm_100 GPUs visible to this process (0 without a GPU or without the library's CUDA runtime); asked once per process."""
+    """sm_90 GPUs visible to this process (0 without a GPU or without the library's CUDA runtime); asked once per process."""
     global _device_count
     if _device_count is None:
         _device_count = int(load_library().gs_device_count())

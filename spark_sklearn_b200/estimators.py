@@ -274,7 +274,7 @@ class SVCPlan(_Plan):
     """sklearn.svm.SVC (C-SVC).  Scalars per candidate: kernel, C, gamma (resolved per fold)."""
     scorers = CLASSIFICATION_SCORERS
     # what one more (kernel, gamma) group costs a GPU, in the units of costs() (thousands of SMO iterations of one candidate's
-    # folds): a kernel matrix (0.3 ms) + a float64 decision-value pass (~1 ms) against ~0.18 ms per unit on a 148-SM GPU
+    # folds): a kernel matrix + a float64 decision-value pass, against the SMO time of one unit (ratio calibrated on a 148-SM GPU)
     group_cost = 7.0
 
     def __init__(self, estimator, cands, X, y, fold_id, n_splits, device=None):
@@ -360,7 +360,7 @@ class SVCPlan(_Plan):
             C = [float(params[j]["C"]) for j in idx]
             gam = np.array([[self._gamma(params[j]["gamma"], k) if params[j]["kernel"] == "rbf" else 0.0
                              for k in range(ns)] for j in idx])
-            # B200GS_GRAM=tensor: opt-in tcgen05 Gram (fp32-faithful; scores match to solver tolerance, not bit for bit)
+            # B200GS_GRAM=tensor: opt-in wgmma Gram (fp32-faithful; scores match to solver tolerance, not bit for bit)
             import os
             flags = 2 if os.environ.get("B200GS_GRAM", "exact") == "tensor" else 0
             self.engine.set_scoring(self.score_kind, self.score_pos)

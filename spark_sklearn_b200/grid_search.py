@@ -1,5 +1,5 @@
 """``GridSearchCV`` with the reference's constructor and ``fit`` (reference
-python/spark_sklearn/grid_search.py:212-246), evaluated on B200 GPUs instead of a Spark cluster."""
+python/spark_sklearn/grid_search.py:212-246), evaluated on H100 GPUs instead of a Spark cluster."""
 from collections.abc import Mapping, Sequence
 
 import numpy as np
@@ -26,7 +26,7 @@ def _check_param_grid(param_grid):
 
 
 class GridSearchCV(B200BaseSearchCV):
-    """Exhaustive search over specified parameter values for an estimator, on B200 GPUs.
+    """Exhaustive search over specified parameter values for an estimator, on H100 GPUs.
 
     Signature, defaults (``cv=3``, ``iid=True``, ``return_train_score=True``, ``error_score='raise'``)
     and fitted attributes follow ``spark_sklearn.GridSearchCV`` (reference grid_search.py:10-246).

@@ -1,12 +1,12 @@
 """``RandomizedSearchCV`` with the reference's constructor and ``fit`` (reference
-python/spark_sklearn/random_search.py:186-226), evaluated on B200 GPUs instead of a Spark cluster."""
+python/spark_sklearn/random_search.py:186-226), evaluated on H100 GPUs instead of a Spark cluster."""
 from sklearn.model_selection import ParameterSampler
 
 from .base_search import B200BaseSearchCV
 
 
 class RandomizedSearchCV(B200BaseSearchCV):
-    """Randomized search on hyper parameters, on B200 GPUs.
+    """Randomized search on hyper parameters, on H100 GPUs.
 
     Follows ``spark_sklearn.RandomizedSearchCV`` (reference random_search.py:9-226): candidates are drawn
     by scikit-learn's own ``ParameterSampler(param_distributions, n_iter, random_state)`` so the

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (run under gpurun); everything else runs on CPU")
+    config.addinivalue_line("markers", "gpu: needs an H100; everything else runs on CPU")
 
 
 @pytest.fixture(scope="session")

@@ -1,4 +1,4 @@
-"""GPU: the tcgen05 + TMA contraction kernel (3xTF32 split) against a float64 numpy reference."""
+"""GPU: the wgmma + TMA contraction kernel (3xTF32 split) against a float64 numpy reference."""
 import numpy as np
 import pytest
 
@@ -31,13 +31,13 @@ def test_gemm_gram_mode_is_symmetric_and_exact_enough(engine, M, K):
     err = np.abs(C - ref) / np.maximum(scale, 1e-30)
     off = err.copy(); np.fill_diagonal(off, 0.0)
     assert off.max() < 2e-6, off.max()
-    # a Gram DIAGONAL sums only positive products, so the truncating TMEM accumulator (gemm_tc.cu header) drifts one way:
+    # a Gram DIAGONAL sums only positive products, so the tensor cores' not-round-to-nearest accumulation (gemm_tc.cu header) drifts one way:
     # ~2^-25 per accumulation, 3 * K / 8 accumulations -- the reason callers bound every chain to TC_KCHUNK = 512 terms
     assert np.diag(err).max() < 2e-6 + 3.0 * K / 8 * 2.0 ** -23, np.diag(err).max()
 
 
 def test_gemm_many_tiles_per_cta(engine):
-    """More tiles than SMs: every persistent CTA walks several tiles through both TMEM accumulators and the smem ring."""
+    """More tiles than SMs: every persistent CTA walks several tiles through the smem ring."""
     rng = np.random.RandomState(5)
     A = rng.randn(2500, 96).astype(np.float32)
     B = rng.randn(1700, 96).astype(np.float32)                      # 20 x 14 = 280 tiles

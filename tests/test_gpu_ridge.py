@@ -1,4 +1,4 @@
-"""GPU parity tests for the Ridge path (tcgen05 fold Grams + batched CG + Gram-statistics R^2) through the C ABI.
+"""GPU parity tests for the Ridge path (wgmma fold Grams + batched CG + Gram-statistics R^2) through the C ABI.
 
 Checker: goldens made by scikit-learn 1.9.0 (Ridge keeps float32 throughout, LAPACK posv) and the numpy oracle.
 Floating point: tolerance 2e-5 on per-split R^2 (both sides carry ~1e-6 of float32 solve error); BASELINE asks for

@@ -1,4 +1,4 @@
-"""GPU parity tests for the SVC path, through the C ABI (libb200gs.so) -- run under gpurun.
+"""GPU parity tests for the SVC path, through the C ABI (libb200gs.so).
 
 Checker: the oracle (oracle/svc_oracle.c, pinned against scikit-learn in test_oracle.py) on the same
 seeded inputs, and the committed goldens (scikit-learn 1.9.0 itself).  Bar: integer work (n_iter,
@@ -254,7 +254,7 @@ def test_c4_full_size_vs_golden(engine):
 
 
 def test_tensor_core_gram_mode(engine):
-    """GS_GRAM_TENSOR: the Gram on tcgen05 tensor cores (3xTF32).  fp32-faithful Q entries differ from libsvm's by an
+    """GS_GRAM_TENSOR: the Gram on wgmma tensor cores (3xTF32).  fp32-faithful Q entries differ from libsvm's by an
     ulp or two, so trajectories diverge within libsvm's own stopping tolerance: scores agree to a few margin flips."""
     from spark_sklearn_b200.engine import GS_GRAM_TENSOR
     w, fold_id, ns = _setup(engine, "c2_mid")

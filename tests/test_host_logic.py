@@ -50,10 +50,11 @@ def test_planning_helpers_against_measured_iteration_counts():
         assert spearmanr(np.repeat(pred, it.shape[1]), it.ravel())[0] >= 0.97
         assert np.median(np.abs(pred * 1000 / it.mean(1) - 1)) <= 0.2          # and is roughly calibrated (thousands)
         cost = np.sort(np.repeat(pred, it.shape[1]))[::-1].copy()
-        picks[name] = L.gs_svc_cluster_count(cost.ctypes.data, len(cost), 148)
         true = np.sort(it.ravel().astype(float))[::-1].copy()                     # with the true counts as costs
-        assert L.gs_svc_cluster_count(true.ctypes.data, len(true), 148) == picks[name]
-    assert picks == {"c2_svc_rbf_8x8": 10, "c4_svc_rbf_16x16": 0}
+        for sms in (148, 132):                                                    # the calibration GPU and the H100
+            picks[name, sms] = L.gs_svc_cluster_count(cost.ctypes.data, len(cost), sms)
+            assert L.gs_svc_cluster_count(true.ctypes.data, len(true), sms) == picks[name, sms]
+    assert picks == {("c2_svc_rbf_8x8", 148): 10, ("c4_svc_rbf_16x16", 148): 0, ("c2_svc_rbf_8x8", 132): 10, ("c4_svc_rbf_16x16", 132): 0}
     assert L.gs_svc_predicted_iterations(0, 3.0, 0.0, 512) == 3.0                  # linear: grows with C
     assert L.gs_svc_cluster_count(None, 0, 148) == 0
 
@@ -228,8 +229,12 @@ def test_three_tier_schedule_on_measured_and_synthetic_costs():
     _, _, it4 = _golden_svc("c4_svc_rbf_16x16")
     nc, ne, c = sched(it2.ravel())
     assert 10 <= nc <= 20 and 10 <= ne <= 40 and 4 * nc + ne <= 140           # the 66-68k group on clusters, the 43-48k tier alone
-    assert makespan(c, nc, ne) <= 0.75 * makespan(c, 0, 0)                     # measured: 279 ms vs 442 ms all shared
+    assert makespan(c, nc, ne) <= 0.75 * makespan(c, 0, 0)
     assert sched(it4.ravel())[:2] == (0, 0)                                    # 1280 problems: throughput-bound
+    nc, ne, c = sched(it2.ravel(), 132)                                        # the H100's 132 SMs
+    assert 10 <= nc <= 20 and 10 <= ne <= 40 and 4 * nc + ne <= 124
+    assert makespan(c, nc, ne, 132) <= 0.75 * makespan(c, 0, 0, 132)
+    assert sched(it4.ravel(), 132)[:2] == (0, 0)
     rng = np.random.default_rng(0)
     for trial in range(20):                                                    # unseen profiles
         n = int(rng.integers(150, 3000))
@@ -555,13 +560,13 @@ def test_simulated_schedule_opt_in(monkeypatch):
     _, _, it4 = _golden_svc("c4_svc_rbf_16x16")
     nc, ne, c = sched(it2.ravel())
     assert 10 <= nc <= 20 and 10 <= ne <= 45 and 4 * nc + ne <= 140           # the 66-68k group on clusters, the 43-48k tier alone
-    assert makespan(c, nc, ne) <= 0.6 * makespan(c, 0, 0)                      # measured: 255 ms of solve vs 442 ms all shared
-    # measured on a B200 (B200GS_SMO_TIMELINE, 10 clusters + 35 exclusive): the tiers end at 242 / 255 / 237 ms
+    assert makespan(c, nc, ne) <= 0.6 * makespan(c, 0, 0)
+    # the simulator's calibration point (148 SMs, B200GS_SMO_TIMELINE, 10 clusters + 35 exclusive): the tiers end at 242 / 255 / 237 ms
     assert abs(makespan(c, 10, 35) * 1e-3 - 255.0) <= 0.05 * 255.0
     assert sched(it4.ravel())[:2] == (0, 0)                                    # 1280 problems: throughput-bound
-    assert makespan(np.sort(it4.ravel())[::-1].copy(), 0, 40) > makespan(np.sort(it4.ravel())[::-1].copy(), 0, 0)   # measured 676 vs 658 ms
+    assert makespan(np.sort(it4.ravel())[::-1].copy(), 0, 40) > makespan(np.sort(it4.ravel())[::-1].copy(), 0, 0)
     # a rank of the 8-GPU weak-scaling grid holds two classes of long problems (67k and 54k predicted iterations): both
-    # belong on clusters (the closed form used before left the second class on exclusive SMs: 292 instead of ~255 ms)
+    # belong on clusters (the closed form used before left the second class on exclusive SMs, which was slower where the simulator was calibrated)
     Cs, gs = np.logspace(-1, 2.5, 16), np.geomspace(1 / 4096, 1 / 256, 32)
     costs = np.array([L.gs_svc_predicted_iterations(1, float(C), float(g), 512) for C in Cs for g in gs])
     part = D.assign_candidates(len(costs), 8, costs)[0]

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Run one BASELINE workload through the C ABI on cuda:0, print the device profile, save the score
-arrays to gpurun_out/<name>_gpu.npz and compare with tests/golden/<name>.npz when it exists."""
+arrays to <name>_gpu.npz in the current directory and compare with tests/golden/<name>.npz when it exists."""
 import os
 import sys
 import time
@@ -50,8 +50,7 @@ def main(key, reps=2):
         print("%s rep%d: set_data %.1f ms, search %.1f ms wall -> %.1f fits/s | profile %s"
               % (key, rep, (t1 - t0) * 1e3, (t2 - t1) * 1e3, nfit / (t2 - t1),
                  {k: (round(v, 3) if isinstance(v, float) else v) for k, v in p.items()}), flush=True)
-    os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-    np.savez(os.path.join(ROOT, "gpurun_out", w["name"] + "_gpu.npz"), **{k: v for k, v in out.items() if v is not None})
+    np.savez(w["name"] + "_gpu.npz", **{k: v for k, v in out.items() if v is not None})
     gp = os.path.join(ROOT, "tests", "golden", w["name"] + ".npz")
     if os.path.exists(gp):
         g = np.load(gp)

@@ -1,7 +1,7 @@
 // Development micro-benchmark: latency of bringing one 40 KB kernel-matrix row to an SM, cold (HBM) and warm (L2):
 //   (a) one cp.async.bulk into shared memory   (b) N bulk copies of 1/N each   (c) coalesced LDG.128 by 1024 / 512 / 256 threads
 //   (d) bulk copy after cp.async.bulk.prefetch.L2 issued `lead` cycles earlier
-// build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o row_latency row_latency.cu
+// build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o row_latency row_latency.cu
 #include <cstdio>
 #include <cstdlib>
 #include <cuda_runtime.h>
@@ -79,7 +79,8 @@ int main()
     cudaMemcpy(d_l2, l2set.data(), nrows * 4, cudaMemcpyHostToDevice); cudaMemcpy(d_pg, l2page.data(), nrows * 4, cudaMemcpyHostToDevice);
     int *d_rows, *d_same; cudaMalloc(&d_rows, nrows * 4); cudaMalloc(&d_same, nrows * 4);
     cudaMemcpy(d_rows, rows.data(), nrows * 4, cudaMemcpyHostToDevice); cudaMemcpy(d_same, same.data(), nrows * 4, cudaMemcpyHostToDevice);
-    long long *out; cudaMallocManaged(&out, 148 * 8); float *sink; cudaMalloc(&sink, 4);
+    int sms = 0; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
+    long long *out; cudaMallocManaged(&out, (size_t)sms * 8); float *sink; cudaMalloc(&sink, 4);
     const int smem = 10016 * 4 + 256;
     cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     auto run = [&](const char *name, int grid, int nt, const int *r, int mode, int nsplit, int lead) {
