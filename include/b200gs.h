@@ -176,6 +176,26 @@ int gs_logreg(gs_handle *h, int32_t n_cand, const double *C, double tol, int32_t
 int gs_logreg_refit(gs_handle *h, double C, double tol, int32_t max_iter, int32_t fit_intercept,
                     double *coef_out, int32_t *n_iter);
 
+/*
+ * epsilon-SVR (replaces SVR.fit/score: sklearn libsvm svm.cpp solve_epsilon_svr on 2l variables, r2 base.py RegressorMixin).
+ * gs_set_targets_f64: the float64 targets y[n] in the caller's row order (scikit-learn fits SVR on float64 y; gs_set_data keeps
+ * float32 targets only).  Valid after a regression gs_set_data, which resets them.
+ * gs_svr: kernel[n_cand], C[n_cand], epsilon[n_cand]; gamma[n_cand*n_splits] resolved per split as for gs_svc.  tol / max_iter
+ * as SVR's; flags GS_RETURN_TRAIN, GS_NO_SHRINKING, GS_GRAM_TENSOR.  Splits: gs_set_data's fold ids or gs_set_splits masks; a
+ * fit's variables are its training rows in ascending original index (scikit-learn's X[train] for partition splitters).
+ * Scores: r2, or GS_SCORE_NEG_MSE / GS_SCORE_NEG_RMSE (gs_set_scoring).  Outputs as gs_svc's, n_iter per fit.
+ * At most 8192 training rows per fit, gs_svr_refit's all-row fit included (GS_ERR_UNSUPPORTED beyond); sample and class
+ * weights are rejected.  r2 of a split with fewer than two rows is NaN (scikit-learn: UndefinedMetricWarning).
+ * gs_svr_refit: all rows; coef[n] = dual coefficient (alpha+ - alpha-) by ORIGINAL row, *rho (prediction = sum coef k - rho),
+ * *n_iter.
+ */
+int gs_set_targets_f64(gs_handle *h, const double *y);
+int gs_svr(gs_handle *h, int32_t n_cand, const int32_t *kernel, const double *C, const double *epsilon, const double *gamma,
+           double tol, int32_t max_iter, uint32_t flags, double *test_scores, double *train_scores, int32_t *n_iter,
+           int32_t *n_sv, float *fit_ms, float *score_ms);
+int gs_svr_refit(gs_handle *h, int32_t kernel, double C, double epsilon, double gamma, double tol, int32_t max_iter,
+                 uint32_t flags, double *coef, double *rho, int32_t *n_iter);
+
 /* ---- test hooks (used by tests/ to localise a parity failure to one kernel) ---------------- */
 /* S_out [n][n] float64 Gram X X^T and xsq_out [n] (either may be NULL), in ORIGINAL row order.  */
 int gs_debug_gram(gs_handle *h, double *S_out, double *xsq_out);

@@ -99,6 +99,8 @@ class B200BaseSearchCV(BaseSearchCV):
                         p.set_scoring(self.scoring)           # raises for scorers without a fused CUDA path
                     if self.fit_params or hasattr(p, "set_fit_params"):
                         p.set_fit_params(self.fit_params)     # sample_weight; raises for anything without a CUDA path
+                    if self.refit and hasattr(p, "check_refit"):
+                        p.check_refit()                       # a refit the CUDA path cannot run fails before the search
                 parts = _dist.assign_for_plan(plans[0], n_param_candidates, len(devices))
                 locs = list(pool.map(lambda i: plans[i].evaluate(parts[i], return_train=self.return_train_score,
                                                                  error_score=self.error_score) if parts[i] else None,
@@ -115,6 +117,8 @@ class B200BaseSearchCV(BaseSearchCV):
                 plan.set_scoring(self.scoring)                # raises for scorers without a fused CUDA path
             if self.fit_params or hasattr(plan, "set_fit_params"):
                 plan.set_fit_params(self.fit_params)          # sample_weight; raises for anything without a CUDA path
+            if self.refit and hasattr(plan, "check_refit"):
+                plan.check_refit()                            # a refit the CUDA path cannot run fails before the search
             # candidates dealt to the GPUs by predicted cost (the reference leaves the placement of its tasks to Spark)
             parts = _dist.assign_for_plan(plan, n_param_candidates, world)
             my = parts[rank]

@@ -1,4 +1,4 @@
-// api.cu -- the C ABI of libb200gs.so (include/b200gs.h): lifecycle, dataset upload, SVC search/refit.
+// api.cu -- the C ABI of libb200gs.so (include/b200gs.h): lifecycle, dataset upload, SVC search/refit (SVR: svr.cu).
 // Host-side planning only; every floating-point operation of the hot path runs in the CUDA kernels
 // of gram.cu / smo.cu / score.cu.  There is no CPU fallback.
 #include "common.cuh"
@@ -73,31 +73,6 @@ __global__ void gather_rows_kernel(const T *__restrict__ src, const int *__restr
     }
 }
 
-struct EvTimer {       // accumulates elapsed ms between consecutive marks on one stream (events from the handle's pool)
-    cudaStream_t st;
-    EventPool &pool;
-    std::vector<cudaEvent_t> evs;
-    std::vector<int> tag;
-    EvTimer(cudaStream_t s, EventPool &p) : st(s), pool(p) {}
-    void mark(int t)
-    {
-        cudaEvent_t e = pool.get();
-        cudaEventRecord(e, st);
-        evs.push_back(e); tag.push_back(t);
-    }
-    // after a stream sync: add the time between mark k-1 and mark k to acc[tag[k]]
-    void collect(float *acc, int ntags)
-    {
-        for (size_t k = 1; k < evs.size(); k++) {
-            float ms = 0;
-            cudaEventElapsedTime(&ms, evs[k - 1], evs[k]);
-            if (tag[k] >= 0 && tag[k] < ntags) acc[tag[k]] += ms;
-        }
-        evs.clear(); tag.clear();
-    }
-};
-
-inline uint64_t dbits(double x) { uint64_t u; memcpy(&u, &x, 8); return u; }
 
 }  // namespace
 
@@ -203,7 +178,7 @@ void gs_destroy(gs_handle *h)
     cudaSetDevice(h->device);
     h->dX.release(); h->dY.release(); h->dFold.release(); h->dYt.release(); h->dTe.release(); h->dTr.release();
     h->dS.release(); h->dXsq.release(); h->dK.release(); h->dX64.release();
-    h->evp.release(); h->dScore.release(); h->dSw.release();
+    h->evp.release(); h->dScore.release(); h->dSw.release(); h->dZ64.release();
     for (auto &w : h->dWork) w.release();
     if (h->stream) cudaStreamDestroy(h->stream);
     if (h->stream_hi) cudaStreamDestroy(h->stream_hi);
@@ -227,6 +202,7 @@ int gs_set_data(gs_handle *h, const void *X, int32_t x_dtype, int64_t n, int64_t
     h->score_kind = GS_SCORE_DEFAULT; h->score_pos = 1;      // a new dataset starts from the estimator's own score and unit class weights
     h->class_w.clear(); h->class_w_sets = 0;
     h->sample_w.clear();
+    h->z64.clear();
     h->perm.resize(n);
     std::iota(h->perm.begin(), h->perm.end(), 0);
     h->n_classes = 0;

@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <cstring>
 #include <string>
 #include <vector>
 #include "../../include/b200gs.h"
@@ -68,6 +69,32 @@ struct TensorTimer {
     }
 };
 
+struct EvTimer {       // accumulates elapsed ms between consecutive marks on one stream (events from the handle's pool)
+    cudaStream_t st;
+    EventPool &pool;
+    std::vector<cudaEvent_t> evs;
+    std::vector<int> tag;
+    EvTimer(cudaStream_t s, EventPool &p) : st(s), pool(p) {}
+    void mark(int t)
+    {
+        cudaEvent_t e = pool.get();
+        cudaEventRecord(e, st);
+        evs.push_back(e); tag.push_back(t);
+    }
+    // after a stream sync: add the time between mark k-1 and mark k to acc[tag[k]]
+    void collect(float *acc, int ntags)
+    {
+        for (size_t k = 1; k < evs.size(); k++) {
+            float ms = 0;
+            cudaEventElapsedTime(&ms, evs[k - 1], evs[k]);
+            if (tag[k] >= 0 && tag[k] < ntags) acc[tag[k]] += ms;
+        }
+        evs.clear(); tag.clear();
+    }
+};
+
+inline uint64_t dbits(double x) { uint64_t u; memcpy(&u, &x, 8); return u; }   // bit pattern: map key of a gamma
+
 // Membership of every row in the training / test set of every CV split: two 64-bit words per row and kind (splits 0..127).
 // Replaces the per-task index arrays of the reference (base_search.py:81-82 islice(cv.split(...))): any splitter fits --
 // overlapping test sets (RepeatedKFold), rows in neither set (ShuffleSplit), rows that only ever train (PredefinedSplit -1).
@@ -118,6 +145,8 @@ struct gs_handle {
     int class_w_sets = 0;
     std::vector<float> sample_w;         // gs_set_sample_weight: [n] internal order; empty = all ones
     DevBuf dSw;                          // its device copy
+    std::vector<double> z64;             // gs_set_targets_f64: [n] float64 regression targets, internal order; empty = not set
+    DevBuf dZ64;                         // their device copy
     gs_profile prof;
     EventPool evp;                    // timing events of the current call
     TensorTimer tt;
@@ -163,6 +192,15 @@ struct SmoProblem {
 cudaError_t launch_smo(const SmoProblem *d_probs, const int *d_order, int n_prob, int lmax, bool fast, int rowcap,
                        cudaStream_t st, std::string *why);
 int smo_max_rows();   // largest sub-problem the resident-state kernel supports
+// epsilon-SVR data of one problem (parallel to SmoProblem; only the SVR instances read it)
+struct SvrData {
+    const double *z;      // [n] float64 targets by dataset row
+    double eps;           // SVR epsilon (libsvm's p)
+};
+// epsilon-SVR on the position-owned kernel: problem q has l = 2 x (training rows) positions, rows[] = the training rows
+// (ascending original index) twice, n_pos = l / 2; svr[q] holds its targets and epsilon.  coef gets alpha+ - alpha- by row.
+cudaError_t launch_smo_svr(const SmoProblem *d_probs, const SvrData *d_svr, const int *d_order, int n_prob, int lmax, bool fast,
+                           int rowcap, cudaStream_t st, std::string *why);
 // smo_lean.cu: the throughput instance (static slots = the problem's column runs, two or more sub-problems per SM).  Every
 // problem of the launch needs a slot layout: nseg > 0, nslots <= smo_lean_max_slots(), l < 16383; alpha and Gbar hold nslots doubles.
 int smo_lean_max_slots();
@@ -201,6 +239,12 @@ cudaError_t launch_auc_pairs_f32(const float *score, int64_t ld, int n, int n_a,
                                  const int *fold_of_task, int n_tasks, int sign, unsigned long long *out, cudaStream_t st);
 // score of one (task, split) from the class counts cnt[class][3] (float64, scikit-learn's formulas); NaN when undefined
 double gs_score_from_counts(int kind, int pos_class, int n_classes, const int *cnt);
+
+// ---- svr.cu ----
+// Residual sums of squares of regression tasks: rss[task][0 test, 1 train] = sum over the split's rows of
+// (z_r - (dec[first_col][r] - rho[first_col]))^2, float64, fixed-order block reduction (deterministic, no atomics).
+cudaError_t launch_rss(const double *dec, const double *rho, int n, const double *z, SplitMasks sm, const VoteTask *tasks,
+                       int n_tasks, double *rss, cudaStream_t st);
 
 // ---- gemm_tc.cu: wgmma + TMA contraction  C[M][N] = sum_k A[M][k] B[N][k]  (3xTF32 split, fp32 accumulate) ----
 struct alignas(64) TcMap { unsigned char bytes[128]; };            // CUtensorMap

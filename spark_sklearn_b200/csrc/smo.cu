@@ -1,4 +1,5 @@
-// smo.cu -- batched C-SVC dual solver: one CTA per (candidate, fold, class-pair) sub-problem.
+// smo.cu -- batched C-SVC dual solver: one CTA per (candidate, fold, class-pair) sub-problem; its epsilon-SVR instance
+// (smo_svr_kernel, driven by svr.cu) solves one (candidate, fold) SVR fit per CTA.
 //
 // Restates scikit-learn's libsvm Solver (svm.cpp:670-944 Solve, :946-1047 select_working_set,
 // :1049-1129 do_shrinking, :629-668 reconstruct_gradient, :1131-1168 calculate_rho) as a
@@ -46,9 +47,13 @@ using namespace smo;
 // (cp.async.bulk, mbarrier-signalled) and gathered from there.  A row gathered with per-thread LDGs is throttled by
 // the SM's outstanding-miss capacity (~64 lines x ~900 cycles of DRAM latency = ~18 GB/s per SM, 2.5 us per 32 KB row,
 // on the 148-SM GPU the kernels were first tuned on); the bulk copy streams the whole 40 KB row at the SM's full fill rate.  G_bar then lives in global memory.
-template <int NT, int KPT, bool SMEM_STATE, bool FAST, bool PROF, bool ROWBUF>
-__global__ void __launch_bounds__(NT, 1)
-smo_kernel(const SmoProblem *__restrict__ probs, const int *__restrict__ order, int rowcap)
+// SVR: epsilon-SVR (svm.cpp solve_epsilon_svr) on l = 2 x (training rows) positions: the first n_pos are the +1 copies of the
+// rows, the rest the -1 copies (rows[] lists every row twice).  Three differences from C-SVC, all compile-time: the linear
+// term p_t = eps -/+ z_row replaces -1 in the initial point and in reconstruct_gradient, and the coefficient of a row is
+// alpha(+1 copy) - alpha(-1 copy) (svm.cpp: alpha[i] = alpha2[i] - alpha2[i+l]).  svr[] is indexed like probs[].
+template <int NT, int KPT, bool SMEM_STATE, bool FAST, bool PROF, bool ROWBUF, bool SVR>
+__device__ __forceinline__ void
+smo_body(const SmoProblem *__restrict__ probs, const int *__restrict__ order, int rowcap, const SvrData *__restrict__ svr)
 {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     __shared__ Red red;
@@ -95,7 +100,11 @@ smo_kernel(const SmoProblem *__restrict__ probs, const int *__restrict__ order, 
         const int *__restrict__ rows = Pp->rows;
         for (int t = tid; t < l; t += NT) {
             const bool yp = t < n_pos;
-            mG[t] = yp ? 1.0 : -1.0;
+            if constexpr (SVR) {                                         // G = p: m = -fl(eps - z) (+1 copy), fl(eps + z) (-1 copy)
+                const SvrData sv = svr[order[blockIdx.x]];
+                const double zr = sv.z[rows[t]];
+                mG[t] = yp ? -__dsub_rn(sv.eps, zr) : __dadd_rn(sv.eps, zr);
+            } else mG[t] = yp ? 1.0 : -1.0;
             col[t] = (unsigned short)rows[t];
             fl[t] = (unsigned char)mkflags(yp, ST_LOWER);
             alpha[t] = 0.0;
@@ -217,7 +226,14 @@ smo_kernel(const SmoProblem *__restrict__ probs, const int *__restrict__ order, 
         for (int k = 0; k < KPT; k++) {
             const int t = k * NT + tid;
             const bool in = t >= active && t < l;
-            g[k] = in ? __dadd_rn(mGbar[t], (fl[t] & F_YPOS) ? 1.0 : -1.0) : 0.0;
+            if constexpr (SVR) {                                         // G = Gbar + p, p = eps -/+ z of the position
+                g[k] = 0.0;
+                if (in) {
+                    const SvrData sv = svr[order[blockIdx.x]];
+                    const double zr = sv.z[col[t]];
+                    g[k] = __dadd_rn(mGbar[t], (fl[t] & F_YPOS) ? -__dsub_rn(sv.eps, zr) : __dadd_rn(sv.eps, zr));
+                }
+            } else g[k] = in ? __dadd_rn(mGbar[t], (fl[t] & F_YPOS) ? 1.0 : -1.0) : 0.0;
             ck[k] = in ? (int)col[t] : -1;
         }
 #pragma unroll 2
@@ -597,6 +613,11 @@ smo_kernel(const SmoProblem *__restrict__ probs, const int *__restrict__ order, 
 
     // ---------------- calculate_rho (svm.cpp:1131-1168): sequential float64 sum in libsvm's order ----
     __syncthreads();
+    if constexpr (SVR) {
+        // a max_iter stop rebuilds the gradient of the shrunk positions first (svm.cpp:912-919: reconstruct_gradient,
+        // active_size = l), so rho is taken over all 2l positions
+        if (timed_out && active < l) { rebuild_gradient(); active = l; }
+    }
     const double C = Pp->C, Cng = Pp->Cn;
     if (tid == 0) {
         int nfree = 0;
@@ -621,6 +642,23 @@ smo_kernel(const SmoProblem *__restrict__ probs, const int *__restrict__ order, 
             nbsv += av >= ((fl[t] & F_YPOS) ? C : Cng);
         }
     }
+    if constexpr (SVR) {
+        // both copies of a row land on one coefficient, so the C-SVC scatter above is overwritten: the +1 copies store,
+        // then the -1 copies subtract (alpha+ - alpha-, one rounding); SV counts by row
+        double *__restrict__ coef = Pp->coef;
+        nsv = 0; nbsv = 0;
+        __syncthreads();
+        for (int t = tid; t < l; t += NT)
+            if (fl[t] & F_YPOS) coef[col[t]] = alpha[t];
+        __syncthreads();
+        for (int t = tid; t < l; t += NT)
+            if (!(fl[t] & F_YPOS)) {
+                const double cv = __dsub_rn(coef[col[t]], alpha[t]);
+                coef[col[t]] = cv;
+                nsv += cv != 0;
+                nbsv += fabs(cv) >= C;
+            }
+    }
 #pragma unroll
     for (int m = 16; m; m >>= 1) {
         nsv += __shfl_xor_sync(0xffffffffu, nsv, m);
@@ -643,31 +681,78 @@ smo_kernel(const SmoProblem *__restrict__ probs, const int *__restrict__ order, 
 }
 
 template <int NT, int KPT, bool SMEM_STATE, bool FAST, bool PROF, bool ROWBUF>
-cudaError_t launch_one(const SmoProblem *probs, const int *order, int n_prob, int rowcap, cudaStream_t st)
+__global__ void __launch_bounds__(NT, 1)
+smo_kernel(const SmoProblem *__restrict__ probs, const int *__restrict__ order, int rowcap)
+{
+    smo_body<NT, KPT, SMEM_STATE, FAST, PROF, ROWBUF, false>(probs, order, rowcap, nullptr);
+}
+
+template <int NT, int KPT, bool SMEM_STATE, bool FAST, bool PROF, bool ROWBUF>
+__global__ void __launch_bounds__(NT, 1)
+smo_svr_kernel(const SmoProblem *__restrict__ probs, const int *__restrict__ order, int rowcap, const SvrData *__restrict__ svr)
+{
+    smo_body<NT, KPT, SMEM_STATE, FAST, PROF, ROWBUF, true>(probs, order, rowcap, svr);
+}
+
+// svr == nullptr: the C-SVC kernel; otherwise the epsilon-SVR one
+template <int NT, int KPT, bool SMEM_STATE, bool FAST, bool PROF, bool ROWBUF, bool SVR>
+cudaError_t launch_one(const SmoProblem *probs, const int *order, int n_prob, int rowcap, const SvrData *svr, cudaStream_t st)
 {
     constexpr int LCAP = NT * KPT;
     const size_t smem = ROWBUF ? (size_t)LCAP * (8 + 8 + 2 + 1) + 128 + (size_t)rowcap * 4
                                : (size_t)LCAP * (SMEM_STATE ? (8 + 8 + 8 + 2 + 1) : (8 + 2 + 1));
-    auto kern = smo_kernel<NT, KPT, SMEM_STATE, FAST, PROF, ROWBUF>;
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    kern<<<n_prob, NT, smem, st>>>(probs, order, rowcap);
+    if constexpr (SVR) {
+        auto kern = smo_svr_kernel<NT, KPT, SMEM_STATE, FAST, PROF, ROWBUF>;
+        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) return e;
+        kern<<<n_prob, NT, smem, st>>>(probs, order, rowcap, svr);
+    } else {
+        auto kern = smo_kernel<NT, KPT, SMEM_STATE, FAST, PROF, ROWBUF>;
+        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) return e;
+        kern<<<n_prob, NT, smem, st>>>(probs, order, rowcap);
+    }
     return cudaGetLastError();
 }
 
-template <int NT, int KPT, bool SMEM_STATE, bool ROWBUF = false>
-cudaError_t launch_cfg(const SmoProblem *probs, const int *order, int n_prob, bool fast, bool prof, int rowcap, cudaStream_t st)
+template <int NT, int KPT, bool SMEM_STATE, bool ROWBUF = false, bool SVR = false>
+cudaError_t launch_cfg(const SmoProblem *probs, const int *order, int n_prob, bool fast, bool prof, int rowcap, const SvrData *svr,
+                       cudaStream_t st)
 {
-    if (prof) return fast ? launch_one<NT, KPT, SMEM_STATE, true, true, ROWBUF>(probs, order, n_prob, rowcap, st)
-                          : launch_one<NT, KPT, SMEM_STATE, false, true, ROWBUF>(probs, order, n_prob, rowcap, st);
-    return fast ? launch_one<NT, KPT, SMEM_STATE, true, false, ROWBUF>(probs, order, n_prob, rowcap, st)
-                : launch_one<NT, KPT, SMEM_STATE, false, false, ROWBUF>(probs, order, n_prob, rowcap, st);
+    if (prof) return fast ? launch_one<NT, KPT, SMEM_STATE, true, true, ROWBUF, SVR>(probs, order, n_prob, rowcap, svr, st)
+                          : launch_one<NT, KPT, SMEM_STATE, false, true, ROWBUF, SVR>(probs, order, n_prob, rowcap, svr, st);
+    return fast ? launch_one<NT, KPT, SMEM_STATE, true, false, ROWBUF, SVR>(probs, order, n_prob, rowcap, svr, st)
+                : launch_one<NT, KPT, SMEM_STATE, false, false, ROWBUF, SVR>(probs, order, n_prob, rowcap, svr, st);
 }
 
 int env_int(const char *name, int dflt)
 {
     const char *v = getenv(name);
     return v && *v ? atoi(v) : dflt;
+}
+
+// the tier choice of launch_smo / launch_smo_svr: lmax positions (C-SVC rows, or twice the SVR training rows)
+template <bool SVR>
+cudaError_t launch_tiers(const SmoProblem *d_probs, const int *d_order, int n_prob, int lmax, bool fast, int rowcap,
+                         const SvrData *svr, cudaStream_t st, std::string *why)
+{
+    if (n_prob <= 0) return cudaSuccess;
+    const bool prof = env_int("B200GS_SMO_PROF", 0) != 0;          // development switch: per-phase cycle counters
+    if (env_int("B200GS_SMO_NOFAST", 0)) fast = false;
+    if (lmax <= 512) return launch_cfg<128, 4, true, false, SVR>(d_probs, d_order, n_prob, fast, prof, 0, svr, st);
+    if (lmax <= 2048) return launch_cfg<256, 8, true, false, SVR>(d_probs, d_order, n_prob, fast, prof, 0, svr, st);
+    if (lmax <= 4096) return launch_cfg<512, 8, true, false, SVR>(d_probs, d_order, n_prob, fast, prof, 0, svr, st);
+    if (lmax <= 8192) {
+        // 8192 rows of state without G_bar = 152 KB; the row buffer may use what is left of the 227 KB
+        const bool rowbuf_fits = (size_t)8192 * 19 + 128 + (size_t)rowcap * 4 + 4096 <= 227 * 1024;
+        if (rowbuf_fits && env_int("B200GS_SMO_ROWBUF", 1))
+            return launch_cfg<1024, 8, true, true, SVR>(d_probs, d_order, n_prob, fast, prof, rowcap, svr, st);
+        return launch_cfg<1024, 8, true, false, SVR>(d_probs, d_order, n_prob, fast, prof, 0, svr, st);
+    }
+    if (lmax <= 16384) return launch_cfg<1024, 16, false, false, SVR>(d_probs, d_order, n_prob, fast, prof, 0, svr, st);
+    if (why) *why = SVR ? "SVR fit with more than 8192 training rows is not supported by the resident-state SMO kernel"
+                        : "SVC sub-problem larger than 16384 rows is not supported by the resident-state SMO kernel";
+    return cudaErrorInvalidValue;
 }
 
 }  // namespace
@@ -679,20 +764,11 @@ int smo_max_rows() { return 1024 * 16; }
 cudaError_t launch_smo(const SmoProblem *d_probs, const int *d_order, int n_prob, int lmax, bool fast, int rowcap, cudaStream_t st,
                        std::string *why)
 {
-    if (n_prob <= 0) return cudaSuccess;
-    const bool prof = env_int("B200GS_SMO_PROF", 0) != 0;          // development switch: per-phase cycle counters
-    if (env_int("B200GS_SMO_NOFAST", 0)) fast = false;
-    if (lmax <= 512) return launch_cfg<128, 4, true>(d_probs, d_order, n_prob, fast, prof, 0, st);
-    if (lmax <= 2048) return launch_cfg<256, 8, true>(d_probs, d_order, n_prob, fast, prof, 0, st);
-    if (lmax <= 4096) return launch_cfg<512, 8, true>(d_probs, d_order, n_prob, fast, prof, 0, st);
-    if (lmax <= 8192) {
-        // 8192 rows of state without G_bar = 152 KB; the row buffer may use what is left of the 227 KB
-        const bool rowbuf_fits = (size_t)8192 * 19 + 128 + (size_t)rowcap * 4 + 4096 <= 227 * 1024;
-        if (rowbuf_fits && env_int("B200GS_SMO_ROWBUF", 1))
-            return launch_cfg<1024, 8, true, true>(d_probs, d_order, n_prob, fast, prof, rowcap, st);
-        return launch_cfg<1024, 8, true>(d_probs, d_order, n_prob, fast, prof, 0, st);
-    }
-    if (lmax <= 16384) return launch_cfg<1024, 16, false>(d_probs, d_order, n_prob, fast, prof, 0, st);
-    if (why) *why = "SVC sub-problem larger than 16384 rows is not supported by the resident-state SMO kernel";
-    return cudaErrorInvalidValue;
+    return launch_tiers<false>(d_probs, d_order, n_prob, lmax, fast, rowcap, nullptr, st, why);
+}
+
+cudaError_t launch_smo_svr(const SmoProblem *d_probs, const SvrData *d_svr, const int *d_order, int n_prob, int lmax, bool fast,
+                           int rowcap, cudaStream_t st, std::string *why)
+{
+    return launch_tiers<true>(d_probs, d_order, n_prob, lmax, fast, rowcap, d_svr, st, why);
 }

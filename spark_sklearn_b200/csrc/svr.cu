@@ -1,0 +1,453 @@
+// svr.cu -- epsilon-SVR search and refit (gs_svr / gs_svr_refit) and the regression scorer over SVR decision values.
+//
+// An SVR fit on l training rows is libsvm's C-SVC Solver on 2l variables (svm.cpp solve_epsilon_svr): positions 0..l-1 are
+// the rows with y = +1 and linear term eps - z, positions l..2l-1 the same rows with y = -1 and linear term eps + z.  The
+// solve is the position-owned SMO kernel of smo.cu (its SVR instance), so the iterate sequence is libsvm's; everything
+// around it -- float64 Gram, float32 kernel matrices per (kernel, gamma), float64 decision values -- is the SVC pipeline.
+#include "common.cuh"
+#include <algorithm>
+#include <cmath>
+#include <cstring>
+#include <cstdlib>
+#include <map>
+#include <numeric>
+
+namespace {
+
+// rss[task][0 / 1] = sum over test / training rows of the split of (z - (dec - rho))^2.  One block per task; every thread
+// sums a fixed row stride, then a fixed shared-memory tree: the same bits every run.
+constexpr int RSS_NT = 256;
+
+__global__ void __launch_bounds__(RSS_NT)
+rss_kernel(const double *__restrict__ dec, const double *__restrict__ rho, int n, const double *__restrict__ z, SplitMasks sm,
+           const VoteTask *__restrict__ tasks, double *__restrict__ rss)
+{
+    __shared__ double red[2][RSS_NT];
+    const VoteTask T = tasks[blockIdx.x];
+    const double *__restrict__ dv = dec + (size_t)T.first_col * n;
+    const double b = rho[T.first_col];
+    double s_te = 0.0, s_tr = 0.0;
+    for (int r = threadIdx.x; r < n; r += RSS_NT) {
+        const bool te = split_test(sm, r, T.fold), tr = !te && split_train(sm, r, T.fold);
+        if (te || tr) {
+            const double e = __dsub_rn(z[r], __dsub_rn(dv[r], b));
+            const double e2 = __dmul_rn(e, e);
+            if (te) s_te = __dadd_rn(s_te, e2); else s_tr = __dadd_rn(s_tr, e2);
+        }
+    }
+    red[0][threadIdx.x] = s_te; red[1][threadIdx.x] = s_tr;
+    __syncthreads();
+    for (int w = RSS_NT / 2; w > 0; w >>= 1) {
+        if ((int)threadIdx.x < w) {
+            red[0][threadIdx.x] = __dadd_rn(red[0][threadIdx.x], red[0][threadIdx.x + w]);
+            red[1][threadIdx.x] = __dadd_rn(red[1][threadIdx.x], red[1][threadIdx.x + w]);
+        }
+        __syncthreads();
+    }
+    if (threadIdx.x < 2) rss[(size_t)blockIdx.x * 2 + threadIdx.x] = red[threadIdx.x][0];
+}
+
+// scikit-learn r2_score (metrics/_regression.py, force_finite=True) from the residual and total sums of squares of m rows;
+// NaN for fewer than two rows (scikit-learn: UndefinedMetricWarning)
+double r2_from(double rss, double tss, double m)
+{
+    if (m < 2) return NAN;
+    if (tss != 0) return 1.0 - rss / tss;
+    return rss == 0 ? 1.0 : 0.0;
+}
+
+}  // namespace
+
+cudaError_t launch_rss(const double *dec, const double *rho, int n, const double *z, SplitMasks sm, const VoteTask *tasks,
+                       int n_tasks, double *rss, cudaStream_t st)
+{
+    if (n_tasks <= 0) return cudaSuccess;
+    rss_kernel<<<n_tasks, RSS_NT, 0, st>>>(dec, rho, n, z, sm, tasks, rss);
+    return cudaGetLastError();
+}
+
+static int svr_run(gs_handle *h, int n_cand, const int32_t *kernel, const double *Cv, const double *epsv, const double *gamma,
+                   double tol, int max_iter, uint32_t flags, bool refit,
+                   double *test_scores, double *train_scores, int32_t *n_iter, int32_t *n_sv, float *fit_ms, float *score_ms,
+                   double *coef_out, double *rho_out)
+{
+    if (!h) return GS_ERR_ARG;
+    if (h->n == 0) { gs_set_error(h, "gs_svr: no dataset (call gs_set_data first)"); return GS_ERR_NO_DATA; }
+    if (h->classification) { gs_set_error(h, "gs_svr: the dataset has class labels (SVR needs a regression gs_set_data)"); return GS_ERR_ARG; }
+    if (h->z64.empty()) { gs_set_error(h, "gs_svr: no float64 targets (call gs_set_targets_f64 after gs_set_data)"); return GS_ERR_NO_DATA; }
+    if (n_cand <= 0 || !kernel || !Cv || !epsv || !gamma) { gs_set_error(h, "gs_svr: bad arguments"); return GS_ERR_ARG; }
+    if (!h->sample_w.empty()) { gs_set_error(h, "gs_svr: sample weights are not supported by the SVR kernels"); return GS_ERR_UNSUPPORTED; }
+    if (h->class_w_sets > 0) { gs_set_error(h, "gs_svr: class weights do not apply to a regressor"); return GS_ERR_ARG; }
+    const int kind = refit ? GS_SCORE_DEFAULT : h->score_kind;
+    if (kind != GS_SCORE_DEFAULT && kind != GS_SCORE_NEG_MSE && kind != GS_SCORE_NEG_RMSE) {
+        gs_set_error(h, "gs_svr: classification scorer on a regressor"); return GS_ERR_ARG;
+    }
+    for (int c = 0; c < n_cand; c++) {
+        if (kernel[c] != GS_KERNEL_LINEAR && kernel[c] != GS_KERNEL_RBF) { gs_set_error(h, "gs_svr: unsupported kernel id"); return GS_ERR_UNSUPPORTED; }
+        if (!(Cv[c] > 0) || !std::isfinite(Cv[c])) { gs_set_error(h, "gs_svr: C must be > 0"); return GS_ERR_ARG; }
+        if (!(epsv[c] >= 0) || !std::isfinite(epsv[c])) { gs_set_error(h, "gs_svr: epsilon must be >= 0"); return GS_ERR_ARG; }
+    }
+    GS_CUDA(cudaSetDevice(h->device));
+    cudaStream_t st = h->stream;
+    const int n = (int)h->n, d = (int)h->d;
+    const int n_splits = refit ? 1 : h->n_splits;
+    const int n_tasks = n_cand * n_splits;
+    const int64_t ldk = ((int64_t)n + 31) & ~31LL;
+
+    // ---- training rows of every split, ascending ORIGINAL index (scikit-learn fits X[train]), validated before any launch ----
+    std::vector<int> by_orig(n);
+    for (int r = 0; r < n; r++) by_orig[h->perm[r]] = r;
+    std::vector<int> rows_all;
+    std::vector<int> sp_off(n_splits + 1, 0);
+    int lmax = 0;
+    for (int k = 0; k < n_splits; k++) {
+        sp_off[k] = (int)rows_all.size();
+        std::vector<int> rs;
+        for (int o = 0; o < n; o++) {
+            const int r = by_orig[o];
+            if (refit || h->is_train(r, k)) rs.push_back(r);
+        }
+        const int l = (int)rs.size();
+        if (l == 0) { gs_set_error(h, "gs_svr: a split has no training rows"); return GS_ERR_ARG; }
+        if (2 * l > smo_max_rows()) {
+            gs_set_error(h, "gs_svr: a fit on " + std::to_string(l) + " training rows exceeds the SVR kernel limit of " +
+                                std::to_string(smo_max_rows() / 2));
+            return GS_ERR_UNSUPPORTED;
+        }
+        rows_all.insert(rows_all.end(), rs.begin(), rs.end());                // +1 copies
+        rows_all.insert(rows_all.end(), rs.begin(), rs.end());                // -1 copies
+        lmax = std::max(lmax, 2 * l);
+    }
+    sp_off[n_splits] = (int)rows_all.size();
+
+    // ---- groups by kernel matrix (kernel, gamma) ----
+    std::map<std::pair<int, uint64_t>, int> gmap;
+    std::vector<std::pair<int, double>> groups;
+    std::vector<int> task_group(n_tasks);
+    for (int c = 0; c < n_cand; c++)
+        for (int k = 0; k < n_splits; k++) {
+            const double g = kernel[c] == GS_KERNEL_RBF ? gamma[(size_t)c * n_splits + k] : 0.0;
+            if (kernel[c] == GS_KERNEL_RBF && !(g > 0 && std::isfinite(g))) { gs_set_error(h, "gs_svr: gamma must be > 0"); return GS_ERR_ARG; }
+            auto key = std::make_pair((int)kernel[c], dbits(g));
+            auto it = gmap.find(key);
+            if (it == gmap.end()) { it = gmap.emplace(key, (int)groups.size()).first; groups.emplace_back(kernel[c], g); }
+            task_group[(size_t)c * n_splits + k] = it->second;
+        }
+    const int n_groups = (int)groups.size();
+    std::vector<std::vector<int>> group_tasks(n_groups);
+    for (int t = 0; t < n_tasks; t++) group_tasks[task_group[t]].push_back(t);
+
+    // ---- per-split sizes and r2 denominators (they depend on the split only) ----
+    std::vector<double> tss((size_t)n_splits * 2, 0.0), cnt((size_t)n_splits * 2, 0.0);
+    if (!refit) {
+        for (int k = 0; k < n_splits; k++)
+            for (int sp = 0; sp < 2; sp++) {
+                // np.average then sum of squared deviations, ascending original row order as scikit-learn's y[test] / y[train]
+                double sum = 0, m = 0;
+                for (int o = 0; o < n; o++) {
+                    const int r = by_orig[o];
+                    if (sp == 0 ? h->is_test(r, k) : (!h->is_test(r, k) && h->is_train(r, k))) { sum += h->z64[r]; m += 1; }
+                }
+                const double mean = m > 0 ? sum / m : 0.0;
+                double s = 0;
+                for (int o = 0; o < n; o++) {
+                    const int r = by_orig[o];
+                    if (sp == 0 ? h->is_test(r, k) : (!h->is_test(r, k) && h->is_train(r, k))) { const double e = h->z64[r] - mean; s += e * e; }
+                }
+                tss[(size_t)k * 2 + sp] = s; cnt[(size_t)k * 2 + sp] = m;
+            }
+    }
+
+    gs_profile &pf = h->prof;
+    const float keep_h2d = pf.ms_h2d; const int64_t keep_h2d_bytes = pf.h2d_bytes;
+    memset(&pf, 0, sizeof pf);
+    pf.ms_h2d = keep_h2d; pf.h2d_bytes = keep_h2d_bytes;
+    float acc[5] = {0, 0, 0, 0, 0};   // 0 gram, 1 kernel matrix, 2 solve, 3 score, 4 other
+    h->evp.reset(); h->tt.reset();
+    EvTimer tm(st, h->evp);
+    cudaEvent_t ev_begin = h->evp.get(), ev_end = h->evp.get();
+    cudaEventRecord(ev_begin, st);
+    tm.mark(-1);
+
+    // ---- 1. Gram X X^T in float64 (GS_GRAM_TENSOR: the fp32-faithful tensor-core Gram, opt-in) ----
+    GS_CUDA(h->dS.reserve((size_t)n * n * 8));
+    GS_CUDA(h->dXsq.reserve((size_t)n * 8));
+    if (flags & GS_GRAM_TENSOR) {
+        const int dpad = (d + 31) & ~31;
+        const int64_t ld32 = ((int64_t)n + 3) & ~3LL;
+        DevBuf &bx = h->dWork[1], &bs = h->dWork[2], &bb = h->dWork[6];
+        GS_CUDA(bx.reserve((size_t)n * dpad * 4 * 3));
+        GS_CUDA(bs.reserve((size_t)n * ld32 * 4));
+        GS_CUDA(bb.reserve(sizeof(TcBatch) + 64));
+        float *xp = bx.as<float>(), *xh = xp + (size_t)n * dpad, *xl = xh + (size_t)n * dpad;
+        GS_CUDA(cudaMemsetAsync(xp, 0, (size_t)n * dpad * 4, st));
+        GS_CUDA(cudaMemcpy2DAsync(xp, (size_t)dpad * 4, h->dX.p, (size_t)d * 4, (size_t)d * 4, n, cudaMemcpyDeviceToDevice, st));
+        GS_CUDA(launch_split_tf32(xp, xh, xl, (size_t)n * dpad, st));
+        TcMap mh, ml;
+        GS_CUDA(tc_make_map(&mh, xh, n, dpad, dpad));
+        GS_CUDA(tc_make_map(&ml, xl, n, dpad, dpad));
+        TcBatch hb{0, 0, 0, dpad, bs.as<float>(), ld32};
+        GS_CUDA(cudaMemcpyAsync(bb.p, &hb, sizeof hb, cudaMemcpyHostToDevice, st));
+        h->tt.begin(h->evp, st);
+        GS_CUDA(launch_gemm_nt_tf32x3(mh, ml, mh, ml, bb.as<TcBatch>(), 1, n, n, 1.0f, false, st, true));
+        h->tt.end(h->evp, st, 3.0 * 2.0 * n * (double)n * dpad);
+        GS_CUDA(launch_widen_gram(bs.as<float>(), n, ld32, h->dS.as<double>(), h->dXsq.as<double>(), st));
+        pf.launches += 3;
+    } else {
+        GS_CUDA(launch_gram_f64(h->x_dtype == GS_F64 ? h->dX64.p : h->dX.p, h->x_dtype, n, d, h->dS.as<double>(), h->dXsq.as<double>(), st));
+        pf.launches++;
+    }
+    pf.gram_flops = 2.0 * n * (double)n * d;
+    pf.gram_bytes = (double)n * d * 4 + (double)n * n * ((flags & GS_GRAM_TENSOR) ? 4 : 8);
+    tm.mark(0);
+
+    // ---- 2. kernel matrices in batches that fit in free HBM (the rule of gs_svc) ----
+    const size_t kbytes = (size_t)n * ldk * 4;
+    int gpb = n_groups;
+    if (h->dK.cap < kbytes * (size_t)n_groups) {
+        size_t free_b = 0, total_b = 0;
+        GS_CUDA(cudaMemGetInfo(&free_b, &total_b));
+        free_b += h->dK.cap;
+        const size_t budget = (size_t)(free_b * 0.6);
+        gpb = (int)std::max<size_t>(1, std::min<size_t>(n_groups, budget / std::max<size_t>(kbytes, 1)));
+        GS_CUDA(h->dK.reserve(kbytes * gpb));
+    }
+    GS_CUDA(h->dWork[0].reserve(rows_all.size() * 4));
+    GS_CUDA(cudaMemcpyAsync(h->dWork[0].p, rows_all.data(), rows_all.size() * 4, cudaMemcpyHostToDevice, st));
+    pf.h2d_bytes += rows_all.size() * 4;
+    const int *d_rows = h->dWork[0].as<int>();
+
+    std::vector<int> task_iter(n_tasks, 0), task_sv(n_tasks, 0);
+    std::vector<double> task_fit_ms(n_tasks, 0.0), task_rss((size_t)n_tasks * 2, 0.0);
+    std::vector<char> task_bad(n_tasks, 0);
+    int64_t total_iter = 0;
+    double solve_bytes = 0;
+
+    for (int g0 = 0; g0 < n_groups; g0 += gpb) {
+        const int g1 = std::min(n_groups, g0 + gpb);
+        GS_CUDA(h->dWork[7].reserve(64));
+        GS_CUDA(cudaMemsetAsync(h->dWork[7].p, 0, 4, st));
+        bool fast = true;
+        for (int g = g0; g < g1; g++) {
+            GS_CUDA(launch_kernel_matrix(h->dS.as<double>(), h->dXsq.as<double>(), n, groups[g].first, groups[g].second,
+                                         h->dK.as<float>() + (size_t)(g - g0) * n * ldk, ldk, h->dWork[7].as<int>(), st));
+            pf.launches++;
+            fast = fast && groups[g].first == GS_KERNEL_RBF;
+        }
+        // the branch-free instance and its device guard, as in gs_svc (SmoProblem::guard)
+        if (getenv("B200GS_SMO_NOFAST") && atoi(getenv("B200GS_SMO_NOFAST"))) fast = false;
+        const int *d_guard = fast ? h->dWork[7].as<int>() : nullptr;
+        tm.mark(1);
+
+        // ---- 3. one problem per (candidate, split), ordered by group: column index == problem index ----
+        std::vector<SmoProblem> probs;
+        std::vector<SvrData> svr;
+        std::vector<int> prob_task, group_first(g1 - g0 + 1, 0);
+        std::vector<VoteTask> vtasks;
+        size_t wl = 0, ws = 0;
+        for (int g = g0; g < g1; g++) {
+            group_first[g - g0] = (int)probs.size();
+            for (int t : group_tasks[g]) {
+                const int c = t / n_splits, k = t % n_splits;
+                vtasks.push_back(VoteTask{(int)probs.size(), refit ? -100 : k});
+                SmoProblem P;
+                memset(&P, 0, sizeof P);
+                P.K = h->dK.as<float>() + (size_t)(g - g0) * n * ldk;
+                P.qd = groups[g].first == GS_KERNEL_LINEAR ? h->dXsq.as<double>() : nullptr;
+                P.rows = d_rows + sp_off[k];
+                P.l = sp_off[k + 1] - sp_off[k];
+                P.n_pos = P.l / 2;
+                P.nseg = 0;                                   // bulk row copies take the whole row
+                P.ldk = ldk; P.C = Cv[c]; P.Cn = Cv[c]; P.eps = tol; P.max_iter = max_iter;
+                P.shrinking = (flags & GS_NO_SHRINKING) ? 0 : 1;
+                P.guard = d_guard;
+                const size_t wlen = ((size_t)P.l + 3) & ~(size_t)3;
+                P.alpha = (double *)wl; wl += wlen;           // offsets now, pointers below
+                P.Gbar = (double *)wl; wl += wlen;
+                P.scratch = (int *)ws; ws += 2 * (size_t)P.l + 64;
+                probs.push_back(P);
+                svr.push_back(SvrData{nullptr, epsv[c]});
+                prob_task.push_back(t);
+            }
+        }
+        group_first[g1 - g0] = (int)probs.size();
+        const int np = (int)probs.size();
+        GS_CUDA(h->dWork[1].reserve(wl * 8));
+        GS_CUDA(h->dWork[2].reserve(ws * 4));
+        GS_CUDA(h->dWork[3].reserve((size_t)np * n * 8));                 // coef columns
+        GS_CUDA(h->dWork[4].reserve((size_t)np * n * 8));                 // decision columns
+        GS_CUDA(h->dWork[5].reserve((size_t)np * (8 + 16 + 96 + 16) + 64)); // rho, info[4], ns[12], rss[2]
+        const size_t meta_bytes = (size_t)np * (sizeof(SmoProblem) + sizeof(SvrData) + 4) + vtasks.size() * sizeof(VoteTask) + 256;
+        GS_CUDA(h->dWork[6].reserve(meta_bytes));
+        double *d_rho = h->dWork[5].as<double>();
+        double *d_rss = d_rho + np;
+        int *d_info = (int *)(d_rss + 2 * (size_t)np);
+        unsigned long long *d_ns = (unsigned long long *)(d_info + 4 * (size_t)np);
+        GS_CUDA(cudaMemsetAsync(d_ns, 0, (size_t)np * 12 * 8, st));
+        for (int q = 0; q < np; q++) {
+            SmoProblem &P = probs[q];
+            P.alpha = h->dWork[1].as<double>() + (size_t)P.alpha;
+            P.Gbar = h->dWork[1].as<double>() + (size_t)P.Gbar;
+            P.scratch = h->dWork[2].as<int>() + (size_t)P.scratch;
+            P.coef = h->dWork[3].as<double>() + (size_t)q * n;
+            P.out_rho = d_rho + q; P.out_info = d_info + 4 * (size_t)q; P.out_ns = d_ns + 12 * (size_t)q;
+            svr[q].z = h->dZ64.as<double>();
+        }
+        // ---- 4. launch order: longest predicted first.  There is no iteration model for SVR yet; C x l orders the
+        // problems (larger C and more rows mean more iterations in the measured searches) until one is calibrated.
+        std::vector<double> cost(np);
+        for (int q = 0; q < np; q++) cost[q] = Cv[prob_task[q] / n_splits] * (double)probs[q].l;
+        std::vector<int> order(np);
+        std::iota(order.begin(), order.end(), 0);
+        std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return cost[a] > cost[b]; });
+        unsigned char *dmeta = h->dWork[6].as<unsigned char>();
+        SmoProblem *d_probs = (SmoProblem *)dmeta;
+        size_t off = (size_t)np * sizeof(SmoProblem);
+        SvrData *d_svr = (SvrData *)(dmeta + off);
+        off += (size_t)np * sizeof(SvrData);
+        int *d_order = (int *)(dmeta + off);
+        off = (off + (size_t)np * 4 + 15) & ~(size_t)15;
+        VoteTask *d_vt = (VoteTask *)(dmeta + off);
+        GS_CUDA(cudaMemcpyAsync(d_probs, probs.data(), (size_t)np * sizeof(SmoProblem), cudaMemcpyHostToDevice, st));
+        GS_CUDA(cudaMemcpyAsync(d_svr, svr.data(), (size_t)np * sizeof(SvrData), cudaMemcpyHostToDevice, st));
+        GS_CUDA(cudaMemcpyAsync(d_order, order.data(), (size_t)np * 4, cudaMemcpyHostToDevice, st));
+        GS_CUDA(cudaMemcpyAsync(d_vt, vtasks.data(), vtasks.size() * sizeof(VoteTask), cudaMemcpyHostToDevice, st));
+        GS_CUDA(cudaMemsetAsync(h->dWork[3].p, 0, (size_t)np * n * 8, st));
+        pf.h2d_bytes += (size_t)np * (sizeof(SmoProblem) + sizeof(SvrData) + 4) + vtasks.size() * sizeof(VoteTask);
+        tm.mark(4);
+        // ---- 5. solve: one launch per instance (branch-free first, then the guarded general one) ----
+        for (int inst = fast ? 1 : 0; inst >= 0; inst--) {
+            std::string why;
+            const cudaError_t ce = launch_smo_svr(d_probs, d_svr, d_order, np, lmax, inst == 1, (int)ldk, st, &why);
+            if (ce != cudaSuccess) {
+                gs_set_error(h, why.empty() ? std::string("launch_smo_svr: ") + cudaGetErrorString(ce) : why);
+                return why.empty() ? GS_ERR_CUDA : GS_ERR_UNSUPPORTED;
+            }
+            pf.launches++;
+        }
+        tm.mark(2);
+        // ---- 6. decision values (float64 kernel, every row) and residual sums of squares ----
+        if (!refit) {
+            size_t part_doubles = 0;
+            std::vector<int> jch(g1 - g0, 1);
+            for (int g = g0; g < g1; g++) {
+                const int cols = group_first[g - g0 + 1] - group_first[g - g0];
+                jch[g - g0] = decision_chunks(n, cols, h->sm_count);
+                if (jch[g - g0] > 1) part_doubles = std::max(part_doubles, (size_t)jch[g - g0] * cols * n);
+            }
+            if (part_doubles) GS_CUDA(h->dWork[8].reserve(part_doubles * 8));
+            for (int g = g0; g < g1; g++) {
+                const int c0 = group_first[g - g0], c1 = group_first[g - g0 + 1], jc = jch[g - g0];
+                GS_CUDA(launch_decision(h->dS.as<double>(), h->dXsq.as<double>(), n, groups[g].first, groups[g].second,
+                                        h->dWork[3].as<double>() + (size_t)c0 * n, c1 - c0,
+                                        h->dWork[4].as<double>() + (size_t)c0 * n, jc > 1 ? h->dWork[8].as<double>() : nullptr, jc, st));
+                pf.launches += jc > 1 ? 2 : 1;
+            }
+            GS_CUDA(launch_rss(h->dWork[4].as<double>(), d_rho, n, h->dZ64.as<double>(), h->masks(), d_vt, (int)vtasks.size(), d_rss, st));
+            pf.launches++;
+        }
+        tm.mark(3);
+        // ---- results of this batch ----
+        std::vector<int> info((size_t)np * 4);
+        std::vector<unsigned long long> ns((size_t)np * 12);
+        std::vector<double> rho(np), rss((size_t)np * 2, 0.0), coef_host;
+        GS_CUDA(cudaMemcpyAsync(info.data(), d_info, info.size() * 4, cudaMemcpyDeviceToHost, st));
+        GS_CUDA(cudaMemcpyAsync(ns.data(), d_ns, ns.size() * 8, cudaMemcpyDeviceToHost, st));
+        GS_CUDA(cudaMemcpyAsync(rho.data(), d_rho, rho.size() * 8, cudaMemcpyDeviceToHost, st));
+        if (!refit) GS_CUDA(cudaMemcpyAsync(rss.data(), d_rss, rss.size() * 8, cudaMemcpyDeviceToHost, st));
+        if (refit && coef_out) {
+            coef_host.resize((size_t)np * n);
+            GS_CUDA(cudaMemcpyAsync(coef_host.data(), h->dWork[3].p, coef_host.size() * 8, cudaMemcpyDeviceToHost, st));
+        }
+        GS_CUDA(cudaStreamSynchronize(st));
+        pf.d2h_bytes += info.size() * 4 + ns.size() * 8 + rho.size() * 8 + (refit ? 0 : rss.size() * 8) + coef_host.size() * 8;
+        tm.collect(acc, 5);
+        tm.mark(-1);
+        for (int q = 0; q < np; q++) {
+            const int t = prob_task[q];
+            task_iter[t] = info[(size_t)q * 4]; task_sv[t] = info[(size_t)q * 4 + 2];
+            task_fit_ms[t] = (double)(ns[(size_t)q * 12 + 1] - ns[(size_t)q * 12]) * 1e-6;
+            task_rss[(size_t)t * 2] = rss[(size_t)q * 2]; task_rss[(size_t)t * 2 + 1] = rss[(size_t)q * 2 + 1];
+            total_iter += info[(size_t)q * 4];
+            // two gathered K rows per iteration, over the problem's l / 2 distinct columns
+            solve_bytes += (double)info[(size_t)q * 4] * 2.0 * (probs[q].l / 2) * 4.0;
+            if (!std::isfinite(rho[q])) { if (refit) { gs_set_error(h, "gs_svr_refit: non-finite intercept"); return GS_ERR_NUMERIC; } task_bad[t] = 1; }
+        }
+        if (refit) {
+            if (rho_out) *rho_out = rho[0];
+            if (n_iter) *n_iter = info[0];
+            if (coef_out)
+                for (int r = 0; r < n; r++) coef_out[h->perm[r]] = coef_host[r];
+        }
+    }
+    cudaEventRecord(ev_end, st);
+    GS_CUDA(cudaStreamSynchronize(st));
+    tm.collect(acc, 5);
+    cudaEventElapsedTime(&pf.ms_total, ev_begin, ev_end);
+    pf.ms_tensor = h->tt.collect(); pf.tensor_flops = h->tt.flops;
+    pf.ms_gram = acc[0]; pf.ms_kernel_matrix = acc[1]; pf.ms_solve = acc[2]; pf.ms_score = acc[3];
+    pf.smo_iterations = total_iter;
+    pf.solve_bytes = solve_bytes;
+
+    if (!refit) {
+        for (int t = 0; t < n_tasks; t++) {
+            const int k = t % n_splits;
+            double sc[2];
+            for (int sp = 0; sp < 2; sp++) {
+                const double r = task_rss[(size_t)t * 2 + sp], m = cnt[(size_t)k * 2 + sp];
+                if (!(m > 0)) { sc[sp] = NAN; continue; }
+                if (kind == GS_SCORE_NEG_MSE) sc[sp] = -(r / m);                         // mean_squared_error
+                else if (kind == GS_SCORE_NEG_RMSE) sc[sp] = -std::sqrt(r / m);          // root_mean_squared_error
+                else sc[sp] = r2_from(r, tss[(size_t)k * 2 + sp], m);
+            }
+            test_scores[t] = task_bad[t] ? NAN : sc[0];
+            if (train_scores) train_scores[t] = task_bad[t] ? NAN : sc[1];
+            if (n_iter) n_iter[t] = task_iter[t];
+            if (n_sv) n_sv[t] = task_sv[t];
+            if (fit_ms) fit_ms[t] = (float)task_fit_ms[t];
+            if (score_ms) score_ms[t] = pf.ms_score / (float)n_tasks;
+        }
+    }
+    return GS_OK;
+}
+
+extern "C" {
+
+int gs_set_targets_f64(gs_handle *h, const double *y)
+{
+    if (!h) return GS_ERR_ARG;
+    if (h->n == 0 || h->classification) { gs_set_error(h, "gs_set_targets_f64: no regression dataset (call gs_set_data first)"); return GS_ERR_NO_DATA; }
+    if (!y) { gs_set_error(h, "gs_set_targets_f64: y is NULL"); return GS_ERR_ARG; }
+    const int64_t n = h->n;
+    std::vector<double> z((size_t)n);
+    for (int64_t i = 0; i < n; i++) {
+        z[i] = y[h->perm[i]];
+        if (!std::isfinite(z[i])) { gs_set_error(h, "gs_set_targets_f64: targets must be finite"); return GS_ERR_ARG; }
+    }
+    GS_CUDA(cudaSetDevice(h->device));
+    GS_CUDA(h->dZ64.reserve((size_t)n * 8));
+    GS_CUDA(cudaMemcpyAsync(h->dZ64.p, z.data(), (size_t)n * 8, cudaMemcpyHostToDevice, h->stream));
+    GS_CUDA(cudaStreamSynchronize(h->stream));
+    h->z64.swap(z);
+    h->prof.h2d_bytes += n * 8;
+    return GS_OK;
+}
+
+int gs_svr(gs_handle *h, int32_t n_cand, const int32_t *kernel, const double *C, const double *epsilon, const double *gamma,
+           double tol, int32_t max_iter, uint32_t flags, double *test_scores, double *train_scores, int32_t *n_iter,
+           int32_t *n_sv, float *fit_ms, float *score_ms)
+{
+    if (h && !test_scores) { gs_set_error(h, "gs_svr: test_scores is NULL"); return GS_ERR_ARG; }
+    return svr_run(h, n_cand, kernel, C, epsilon, gamma, tol, max_iter, flags, false, test_scores,
+                   (flags & GS_RETURN_TRAIN) ? train_scores : nullptr, n_iter, n_sv, fit_ms, score_ms, nullptr, nullptr);
+}
+
+int gs_svr_refit(gs_handle *h, int32_t kernel, double C, double epsilon, double gamma, double tol, int32_t max_iter,
+                 uint32_t flags, double *coef, double *rho, int32_t *n_iter)
+{
+    const int32_t k = kernel;
+    return svr_run(h, 1, &k, &C, &epsilon, &gamma, tol, max_iter, flags, true, nullptr, nullptr, n_iter, nullptr, nullptr,
+                   nullptr, coef, rho);
+}
+
+}  // extern "C"

@@ -66,6 +66,9 @@ def load_library():
     L.gs_ridge_refit.argtypes = [vp, dbl, i32, vp]
     L.gs_enet.argtypes = [vp, i32, vp, vp, i32, dbl, i32, u32, vp, vp, vp, vp, vp]
     L.gs_enet_refit.argtypes = [vp, dbl, dbl, i32, dbl, i32, vp, vp, vp]
+    L.gs_set_targets_f64.argtypes = [vp, vp]
+    L.gs_svr.argtypes = [vp, i32, vp, vp, vp, vp, dbl, i32, u32, vp, vp, vp, vp, vp, vp]
+    L.gs_svr_refit.argtypes = [vp, i32, dbl, dbl, dbl, dbl, i32, u32, vp, vp, vp]
     L.gs_logreg.argtypes = [vp, i32, vp, dbl, i32, i32, u32, vp, vp, vp, vp, vp]
     L.gs_logreg_refit.argtypes = [vp, dbl, dbl, i32, i32, vp, vp]
     L.gs_get_profile.argtypes = [vp, c.POINTER(GsProfile)]
@@ -80,7 +83,8 @@ def load_library():
     L.gs_svc_schedule.restype = None
     L.gs_svc_simulate.argtypes = [vp, i32, i32, i32, i32]
     L.gs_svc_simulate.restype = dbl
-    for f in ("gs_create", "gs_set_data", "gs_svc", "gs_svc_refit", "gs_ridge", "gs_ridge_refit", "gs_enet", "gs_enet_refit", "gs_logreg",
+    for f in ("gs_create", "gs_set_data", "gs_svc", "gs_svc_refit", "gs_ridge", "gs_ridge_refit", "gs_enet", "gs_enet_refit", "gs_set_targets_f64",
+              "gs_svr", "gs_svr_refit", "gs_logreg",
               "gs_logreg_refit", "gs_get_profile", "gs_debug_gram", "gs_debug_kernel_matrix", "gs_debug_gemm_nt"):
         getattr(L, f).restype = c.c_int
     _lib = L
@@ -198,6 +202,44 @@ class Engine:
         self._check(self._L.gs_svc_refit(self._h, k, float(C), float(gamma), float(tol), int(max_iter),
                                          0 if shrinking else GS_NO_SHRINKING, _ptr(coef), _ptr(rho), _ptr(it)))
         return coef, rho, it
+
+    def set_targets_f64(self, y):
+        """float64 regression targets [n] (caller's row order) of the following svr / svr_refit calls, after set_data"""
+        y = np.ascontiguousarray(y, np.float64)
+        if y.shape != (self.n,):
+            raise ValueError("y has shape %r; expected (%d,)" % (y.shape, self.n))
+        self._check(self._L.gs_set_targets_f64(self._h, _ptr(y)))
+
+    # -- map(fun).collect() for epsilon-SVR --
+    def svr(self, kernel, C, epsilon, gamma, tol=1e-3, max_iter=-1, shrinking=True, return_train=True, flags=0):
+        kernel = np.ascontiguousarray([KERNEL_ID[k] if isinstance(k, str) else int(k) for k in kernel], np.int32)
+        C = np.ascontiguousarray(C, np.float64)
+        n_cand = len(C)
+        epsilon = np.ascontiguousarray(np.broadcast_to(np.asarray(epsilon, np.float64), (n_cand,)))
+        gamma = np.ascontiguousarray(np.broadcast_to(np.asarray(gamma, np.float64).reshape(n_cand, -1),
+                                                     (n_cand, self.n_splits)))
+        shape = (n_cand, self.n_splits)
+        out = dict(test=np.zeros(shape), train=np.zeros(shape), n_iter=np.zeros(shape, np.int32),
+                   n_sv=np.zeros(shape, np.int32), fit_ms=np.zeros(shape, np.float32),
+                   score_ms=np.zeros(shape, np.float32))
+        fl = int(flags) | (GS_RETURN_TRAIN if return_train else 0) | (0 if shrinking else GS_NO_SHRINKING)
+        self._check(self._L.gs_svr(self._h, n_cand, _ptr(kernel), _ptr(C), _ptr(epsilon), _ptr(gamma), float(tol),
+                                   int(max_iter), fl, _ptr(out["test"]), _ptr(out["train"]), _ptr(out["n_iter"]),
+                                   _ptr(out["n_sv"]), _ptr(out["fit_ms"]), _ptr(out["score_ms"])))
+        if not return_train:
+            out["train"] = None
+        return out
+
+    def svr_refit(self, kernel, C, epsilon, gamma, tol=1e-3, max_iter=-1, shrinking=True, flags=0):
+        """-> (coef [n] by row: alpha+ - alpha-, rho, n_iter); prediction = sum coef k(x, x_row) - rho"""
+        coef = np.zeros(self.n)
+        rho = np.zeros(1)
+        it = np.zeros(1, np.int32)
+        k = KERNEL_ID[kernel] if isinstance(kernel, str) else int(kernel)
+        fl = int(flags) | (0 if shrinking else GS_NO_SHRINKING)
+        self._check(self._L.gs_svr_refit(self._h, k, float(C), float(epsilon), float(gamma), float(tol), int(max_iter),
+                                         fl, _ptr(coef), _ptr(rho), _ptr(it)))
+        return coef, float(rho[0]), int(it[0])
 
     def ridge(self, alpha, fit_intercept=True, return_train=True):
         alpha = np.ascontiguousarray(alpha, np.float64)

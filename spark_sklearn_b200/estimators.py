@@ -2,7 +2,7 @@
 and turn refit buffers back into genuine fitted scikit-learn estimators for ``best_estimator_``
 (reference base_search.py:165-174 delegates ``predict`` & co. to it).
 
-Only estimators with a CUDA path are accepted (SVC rbf/linear, Ridge, LogisticRegression -- the
+Only estimators with a CUDA path are accepted (SVC and SVR rbf/linear, Ridge, LogisticRegression -- the
 families the reference ships examples for); anything else raises: no CPU fallback.
 """
 import numbers
@@ -94,10 +94,12 @@ class Folds:
 def adapter_for(estimator):
     from sklearn.linear_model import ElasticNet, Lasso, LogisticRegression, Ridge
     from sklearn.pipeline import Pipeline
-    from sklearn.svm import SVC
+    from sklearn.svm import SVC, SVR
     t = type(estimator)
     if t is SVC:
         return SVCAdapter
+    if t is SVR:
+        return SVRAdapter
     if t is Ridge:
         return RidgeAdapter
     if t is LogisticRegression:
@@ -109,7 +111,7 @@ def adapter_for(estimator):
         # (python/spark_sklearn/tests/test_search_2.py:69-93): the step's adapter runs, the names are translated
         return PipelineAdapter(estimator.steps[0][0], adapter_for(estimator.steps[0][1]))
     raise NotImplementedError(
-        "spark_sklearn_b200 has CUDA paths for SVC, Ridge, Lasso, ElasticNet and LogisticRegression (bare or as the only "
+        "spark_sklearn_b200 has CUDA paths for SVC, SVR, Ridge, Lasso, ElasticNet and LogisticRegression (bare or as the only "
         "step of a Pipeline); got %s (no CPU fallback)" % t.__name__)
 
 
@@ -270,7 +272,27 @@ class SVCAdapter:
         return SVCPlan(estimator, cands, X, y, fold_id, n_splits, device)
 
 
-class SVCPlan(_Plan):
+class _KernelGamma:
+    """gamma of one libsvm fit: sklearn svm/_base.py:278-286, shared by the SVC and SVR plans."""
+
+    def _gamma(self, g, k):
+        """'scale' uses the variance of the TRAINING fold (float64); k < 0: all rows."""
+        if isinstance(g, str):
+            if g == "auto":
+                return 1.0 / self.X.shape[1]
+            if g == "scale":
+                cache = self.__dict__.setdefault("_var_cache", {})
+                if k not in cache:
+                    cache[k] = np.asarray(self.X[self._train_rows(k)], np.float64).var()
+                v = cache[k]
+                return 1.0 / (self.X.shape[1] * v) if v != 0 else 1.0
+            raise ValueError("gamma=%r" % (g,))
+        if not (isinstance(g, numbers.Real) and g >= 0):
+            raise ValueError("gamma must be >= 0 or 'scale'/'auto'; got %r" % (g,))
+        return float(g)
+
+
+class SVCPlan(_KernelGamma, _Plan):
     """sklearn.svm.SVC (C-SVC).  Scalars per candidate: kernel, C, gamma (resolved per fold)."""
     scorers = CLASSIFICATION_SCORERS
     # what one more (kernel, gamma) group costs a GPU, in the units of costs() (thousands of SMO iterations of one candidate's
@@ -296,21 +318,6 @@ class SVCPlan(_Plan):
             raise NotImplementedError("SVC break_ties=True is not supported by the CUDA path")
         if not (isinstance(p["C"], numbers.Real) and p["C"] > 0):
             raise ValueError("C must be a positive number; got %r" % (p["C"],))
-
-    def _gamma(self, g, k):
-        """sklearn svm/_base.py:278-286; 'scale' uses the variance of the TRAINING fold (float64)."""
-        if isinstance(g, str):
-            if g == "auto":
-                return 1.0 / self.X.shape[1]
-            if g == "scale":
-                if k not in self._var_cache:
-                    self._var_cache[k] = np.asarray(self.X[self._train_rows(k)], np.float64).var()
-                v = self._var_cache[k]
-                return 1.0 / (self.X.shape[1] * v) if v != 0 else 1.0
-            raise ValueError("gamma=%r" % (g,))
-        if not (isinstance(g, numbers.Real) and g >= 0):
-            raise ValueError("gamma must be >= 0 or 'scale'/'auto'; got %r" % (g,))
-        return float(g)
 
     def costs(self):
         """Predicted SMO iterations per candidate from the library's own model (gs_svc_predicted_iterations: the one
@@ -430,6 +437,151 @@ def materialize_svc(est, X, y_class, classes, pair_coef, rho, n_iter, gamma):
     est.fit_status_ = 0
     est._num_iter = np.asarray(n_iter, np.int32)
     est.n_iter_ = est._num_iter
+    est.shape_fit_ = X.shape
+    est.n_features_in_ = X.shape[1]
+    return est
+
+
+# ------------------------------------------------------------------ SVR -----------------------
+class SVRAdapter:
+    multi_device = True        # plan(..., device=d): one plan per GPU of the in-process scheduler
+    scorers = REGRESSION_SCORERS
+
+    @staticmethod
+    def plan(estimator, cands, X, y, fold_id, n_splits, device=None):
+        return SVRPlan(estimator, cands, X, y, fold_id, n_splits, device)
+
+
+class SVRPlan(_KernelGamma, _Plan):
+    """sklearn.svm.SVR (epsilon-SVR).  Scalars per candidate: kernel, C, epsilon, gamma (resolved per fold).  Each fit runs
+    libsvm's solver on its training rows in ascending row order, as scikit-learn's X[train] does for KFold-like splitters."""
+    scorers = REGRESSION_SCORERS
+
+    def __init__(self, estimator, cands, X, y, fold_id, n_splits, device=None):
+        super().__init__(estimator, cands, X, y, fold_id, n_splits, device)
+        if y is None:
+            raise ValueError("SVR needs y")
+        y = np.asarray(y)
+        if y.ndim == 2 and y.shape[1] == 1:               # scikit-learn: column_or_1d(y, warn=True)
+            from sklearn.exceptions import DataConversionWarning
+            warnings.warn("A column-vector y was passed when a 1d array was expected. Please change the shape of y to "
+                          "(n_samples, ), for example using ravel().", DataConversionWarning, stacklevel=2)
+            y = y[:, 0]
+        if y.ndim != 1:
+            raise ValueError("SVR needs a 1d target; got y of shape %r" % (y.shape,))
+        self.y = y.astype(np.float64)                     # scikit-learn fits SVR on float64 y
+        self._set_data(self.X, y_target=self.y.astype(np.float32))
+        self.engine.set_targets_f64(self.y)
+
+    def _check(self, p):
+        if p["kernel"] not in ("rbf", "linear"):
+            raise NotImplementedError("SVR kernel=%r has no CUDA path (rbf and linear do)" % (p["kernel"],))
+        if not (isinstance(p["C"], numbers.Real) and p["C"] > 0):
+            raise ValueError("C must be a positive number; got %r" % (p["C"],))
+        if not (isinstance(p["epsilon"], numbers.Real) and p["epsilon"] >= 0):
+            raise ValueError("epsilon must be a non-negative number; got %r" % (p["epsilon"],))
+
+    def affinity(self):
+        """Candidates with the same (kernel, gamma) share a kernel matrix and a decision-value pass."""
+        try:
+            out = []
+            for cand in self.cands:
+                p = self._base_params(cand)
+                out.append((p["kernel"], self._gamma(p["gamma"], -1) if p["kernel"] == "rbf" else 0.0))
+            return out
+        except Exception:
+            return None
+
+    def _flags(self):
+        import os
+        # B200GS_GRAM=tensor: opt-in wgmma Gram (fp32-faithful; scores match to solver tolerance, not bit for bit)
+        return 2 if os.environ.get("B200GS_GRAM", "exact") == "tensor" else 0
+
+    max_rows = 8192        # training rows of one fit: 2 x 8192 solver variables, the largest resident-state SMO instance
+
+    def _check_rows(self, k):
+        m = int(np.count_nonzero(self._train_rows(k)))
+        if m > self.max_rows:
+            raise NotImplementedError("SVR fit on %d training rows: the CUDA solver handles up to %d" % (m, self.max_rows))
+
+    def check_refit(self):
+        """the refit trains on every row: raise before the search when that fit is too large"""
+        self._check_rows(-1)
+
+    def evaluate(self, my, return_train=True, error_score='raise'):
+        ns = self.n_splits
+        shape = (len(my), ns)
+        res = dict(test=np.zeros(shape), train=np.zeros(shape), fit_ms=np.zeros(shape), score_ms=np.zeros(shape),
+                   n_iter=np.zeros(shape, np.int64))
+        for k in range(ns):
+            self._check_rows(k)
+        groups = {}
+        params = []
+        for j, ci in enumerate(my):
+            p = self._base_params(self.cands[ci])
+            self._check(p)
+            params.append(p)
+            groups.setdefault((float(p["tol"]), int(p["max_iter"]), bool(p["shrinking"])), []).append(j)
+        prof = {}
+        for (tol, max_iter, shrinking), idx in groups.items():
+            kern = [params[j]["kernel"] for j in idx]
+            C = [float(params[j]["C"]) for j in idx]
+            eps = [float(params[j]["epsilon"]) for j in idx]
+            gam = np.array([[self._gamma(params[j]["gamma"], k) if params[j]["kernel"] == "rbf" else 0.0
+                             for k in range(ns)] for j in idx])
+            self.engine.set_scoring(self.score_kind, self.score_pos)
+            r = self.engine.svr(kern, C, eps, gam, tol=tol, max_iter=max_iter, shrinking=shrinking,
+                                return_train=return_train, flags=self._flags())
+            for key in ("test", "fit_ms", "score_ms", "n_iter"):
+                res[key][idx] = r[key]
+            if return_train:
+                res["train"][idx] = r["train"]
+            for k, v in self.engine.profile().items():
+                prof[k] = prof.get(k, 0) + v
+        self._prof = prof
+        self.n_iter_ = res["n_iter"]
+        return self._finish(res, return_train, error_score, len(my))
+
+    def refit(self, best_params):
+        p = self._base_params(best_params)
+        self._check(p)
+        self._check_rows(-1)
+        gamma = self._gamma(p["gamma"], -1)          # all rows train (svm/_base.py:278-286)
+        coef, rho, n_iter = self.engine.svr_refit(p["kernel"], p["C"], p["epsilon"], gamma if p["kernel"] == "rbf" else 0.0,
+                                                  tol=p["tol"], max_iter=p["max_iter"], shrinking=p["shrinking"],
+                                                  flags=self._flags())
+        est = clone(self.estimator).set_params(**best_params)
+        est = materialize_svr(est, self.X, coef, rho, n_iter, gamma)
+        if p["max_iter"] != -1 and n_iter >= p["max_iter"]:        # svm/_base.py: fit_status_ 1 and its warning
+            from sklearn.exceptions import ConvergenceWarning
+            est.fit_status_ = 1
+            warnings.warn("Solver terminated early (max_iter=%i).  Consider pre-processing your data with StandardScaler "
+                          "or MinMaxScaler." % p["max_iter"], ConvergenceWarning)
+        return est
+
+
+def materialize_svr(est, X, coef, rho, n_iter, gamma):
+    """Fill a (cloned, parametrised) sklearn.svm.SVR with the fitted state libsvm would have produced for epsilon-SVR
+    (svm.cpp svm_train: support vectors = rows with a non-zero coefficient, ascending; sklearn _libsvm.pyx fit: _n_support
+    = [n_SV, n_SV] for regression; svm/_base.py fit: intercept_ = -rho, n_iter_ a plain int)."""
+    X64 = np.ascontiguousarray(X, np.float64)
+    coef = np.asarray(coef, np.float64)
+    sv = np.flatnonzero(coef != 0)
+    est._sparse = False
+    est._gamma = np.float64(gamma)
+    est.support_ = sv.astype(np.int32)
+    est.support_vectors_ = X64[sv]
+    est._n_support = np.array([len(sv), len(sv)], np.int32)
+    est._dual_coef_ = coef[sv].reshape(1, -1)
+    est._intercept_ = np.array([-float(rho)])
+    est.dual_coef_ = est._dual_coef_.copy()
+    est.intercept_ = est._intercept_.copy()
+    est._probA = np.empty(0)
+    est._probB = np.empty(0)
+    est._effective_probability = False
+    est.fit_status_ = 0
+    est._num_iter = np.array([n_iter], np.int32)
+    est.n_iter_ = int(n_iter)
     est.shape_fit_ = X.shape
     est.n_features_in_ = X.shape[1]
     return est

@@ -71,6 +71,19 @@ def _lasso(n=20000, d=1024, n_alpha=32, cv=10, name="lasso_1024", enet=False):
     return w
 
 
+def _svr(n=1000, d=32, grid=None, cv=5, name="svr_small"):
+    """epsilon-SVR: make_regression, X standardised then fp32, y standardised in float64 (SVR's epsilon is in y units)."""
+    from sklearn.datasets import make_regression
+    from sklearn.preprocessing import StandardScaler
+    X, y = make_regression(n_samples=n, n_features=d, n_informative=8, noise=10.0, random_state=0)
+    X = np.ascontiguousarray(StandardScaler().fit_transform(X).astype(np.float32))
+    y = (y - y.mean()) / y.std()
+    if grid is None:
+        grid = {"C": [0.1, 1.0, 10.0, 100.0], "gamma": [1.0 / 256, 1.0 / 32, "scale"], "epsilon": [0.05, 0.2]}
+    return dict(name=name, X=X, y=y.astype(np.float64), estimator="SVR", est_params={"kernel": "rbf"},
+                param_grid=grid, cv=cv, search="grid")
+
+
 WORKLOADS = {
     "c1": _c1, "c2": _c2, "c3": _c3, "c4": _c4, "c5": _c5,
     # reduced-size variants: same recipes, sizes the CPU oracle finishes in seconds
@@ -82,6 +95,12 @@ WORKLOADS = {
     "lasso_1024": _lasso,
     "lasso_small": lambda: _lasso(n=2000, d=64, n_alpha=16, cv=5, name="lasso_small"),
     "enet_small": lambda: _lasso(n=1500, d=200, n_alpha=6, cv=4, name="enet_small", enet=True),
+    # epsilon-SVR (SURVEY.md 8f-2): svr_c6 is the measurement config (8 x 8 C x gamma, 8000 training rows per fit)
+    "svr_small": _svr,
+    "svr_mid": lambda: _svr(n=5000, d=128, grid={"C": [0.3, 3.0, 30.0], "gamma": [1.0 / 1024, 1.0 / 128, "scale"],
+                                                 "epsilon": [0.1]}, name="svr_mid"),
+    "svr_c6": lambda: _svr(n=10000, d=512, grid={"C": np.logspace(-1, 2.5, 8), "gamma": np.geomspace(1.0 / 4096, 1.0 / 256, 8),
+                                                 "epsilon": [0.1]}, name="svr_c6"),
 }
 
 
@@ -100,6 +119,9 @@ def make_estimator(w):
     if w["estimator"] == "Ridge":
         from sklearn.linear_model import Ridge
         return Ridge(**w["est_params"])
+    if w["estimator"] == "SVR":
+        from sklearn.svm import SVR
+        return SVR(**w["est_params"])
     if w["estimator"] in ("Lasso", "ElasticNet"):
         import sklearn.linear_model as lm
         return getattr(lm, w["estimator"])(**w["est_params"])
