@@ -529,49 +529,12 @@ static int svc_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
     }
 
     gs_profile &pf = h->prof;
-    const float keep_h2d = pf.ms_h2d; const int64_t keep_h2d_bytes = pf.h2d_bytes;
-    memset(&pf, 0, sizeof pf);
-    pf.ms_h2d = keep_h2d; pf.h2d_bytes = keep_h2d_bytes;
-    float acc[5] = {0, 0, 0, 0, 0};   // 0 gram, 1 kernel matrix, 2 solve, 3 score, 4 other
-    h->evp.reset(); h->tt.reset();
-    EvTimer tm(st, h->evp);
-    cudaEvent_t ev_begin = h->evp.get(), ev_end = h->evp.get();
-    cudaEventRecord(ev_begin, st);
-    tm.mark(-1);
+    SvmSearch search(h, st);
+    search.begin();
 
-    // ---- 1. Gram X X^T (shared by every candidate, fold and pair) ----
-    // default: float64 on the FP64 pipe (libsvm-faithful, gram.cu).  GS_GRAM_TENSOR: wgmma tensor cores, 3xTF32 split,
-    // TMA-fed (gemm_tc.cu) -- fp32-faithful, so scores agree with scikit-learn to solver tolerance, not bit for bit.
-    GS_CUDA(h->dS.reserve((size_t)n * n * 8));
-    GS_CUDA(h->dXsq.reserve((size_t)n * 8));
-    if (flags & GS_GRAM_TENSOR) {
-        const int dpad = (d + 31) & ~31;
-        const int64_t ld32 = ((int64_t)n + 3) & ~3LL;
-        DevBuf &bx = h->dWork[1], &bs = h->dWork[2], &bb = h->dWork[6];
-        GS_CUDA(bx.reserve((size_t)n * dpad * 4 * 3));
-        GS_CUDA(bs.reserve((size_t)n * ld32 * 4));
-        GS_CUDA(bb.reserve(sizeof(TcBatch) + 64));
-        float *xp = bx.as<float>(), *xh = xp + (size_t)n * dpad, *xl = xh + (size_t)n * dpad;
-        GS_CUDA(cudaMemsetAsync(xp, 0, (size_t)n * dpad * 4, st));
-        GS_CUDA(cudaMemcpy2DAsync(xp, (size_t)dpad * 4, h->dX.p, (size_t)d * 4, (size_t)d * 4, n, cudaMemcpyDeviceToDevice, st));
-        GS_CUDA(launch_split_tf32(xp, xh, xl, (size_t)n * dpad, st));
-        TcMap mh, ml;
-        GS_CUDA(tc_make_map(&mh, xh, n, dpad, dpad));
-        GS_CUDA(tc_make_map(&ml, xl, n, dpad, dpad));
-        TcBatch hb{0, 0, 0, dpad, bs.as<float>(), ld32};
-        GS_CUDA(cudaMemcpyAsync(bb.p, &hb, sizeof hb, cudaMemcpyHostToDevice, st));
-        h->tt.begin(h->evp, st);
-        GS_CUDA(launch_gemm_nt_tf32x3(mh, ml, mh, ml, bb.as<TcBatch>(), 1, n, n, 1.0f, false, st, true));
-        h->tt.end(h->evp, st, 3.0 * 2.0 * n * (double)n * dpad);
-        GS_CUDA(launch_widen_gram(bs.as<float>(), n, ld32, h->dS.as<double>(), h->dXsq.as<double>(), st));
-        pf.launches += 3;
-    } else {
-        GS_CUDA(launch_gram_f64(h->x_dtype == GS_F64 ? h->dX64.p : h->dX.p, h->x_dtype, n, d, h->dS.as<double>(), h->dXsq.as<double>(), st));
-        pf.launches++;
-    }
-    pf.gram_flops = 2.0 * n * (double)n * d;
-    pf.gram_bytes = (double)n * d * 4 + (double)n * n * ((flags & GS_GRAM_TENSOR) ? 4 : 8);
-    tm.mark(0);
+    // ---- 1. Gram X X^T, enqueued first: the host prepares the sub-problems below while it runs ----
+    if (const int rc = build_gram(h, flags, st)) return rc;
+    search.tm.mark(0);
 
     // ---- 2. sub-problem row lists per (fold, pair): class a rows then class b rows, train rows only ----
     std::vector<int> rows_all;
@@ -621,44 +584,16 @@ static int svc_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
         return GS_ERR_UNSUPPORTED;
     }
 
-    // ---- 3. group tasks by kernel matrix (kernel, gamma) ----
-    std::map<std::pair<int, uint64_t>, int> gmap;
-    std::vector<std::pair<int, double>> groups;         // (kernel, gamma)
-    std::vector<int> task_group(n_tasks);
-    for (int c = 0; c < n_cand; c++)
-        for (int k = 0; k < n_splits; k++) {
-            const double g = kernel[c] == GS_KERNEL_RBF ? gamma[(size_t)c * n_splits + k] : 0.0;
-            if (kernel[c] == GS_KERNEL_RBF && !(g > 0) ) { gs_set_error(h, "gs_svc: gamma must be > 0"); return GS_ERR_ARG; }
-            auto key = std::make_pair((int)kernel[c], dbits(g));
-            auto it = gmap.find(key);
-            if (it == gmap.end()) { it = gmap.emplace(key, (int)groups.size()).first; groups.emplace_back(kernel[c], g); }
-            task_group[(size_t)c * n_splits + k] = it->second;
-        }
-    const int n_groups = (int)groups.size();
-    std::vector<std::vector<int>> group_tasks(n_groups);
-    for (int t = 0; t < n_tasks; t++) group_tasks[task_group[t]].push_back(t);
-
-    // ---- 4. memory plan: kernel matrices are processed in batches that fit in free HBM ----
-    const size_t kbytes = (size_t)n * ldk * 4;
-    int gpb = n_groups;
-    if (h->dK.cap < kbytes * (size_t)n_groups) {
-        // Ask the driver only when the buffer has to grow: cudaMemGetInfo takes anything from 0.1 to 100+ ms on a busy box
-        // (it showed as outliers of this phase with the Gram already in flight), and a repeated search of the same
-        // shape needs no new plan.
-        size_t free_b = 0, total_b = 0;
-        GS_CUDA(cudaMemGetInfo(&free_b, &total_b));
-        free_b += h->dK.cap;
-        const size_t budget = (size_t)(free_b * 0.6);
-        gpb = (int)std::max<size_t>(1, std::min<size_t>(n_groups, budget / std::max<size_t>(kbytes, 1)));
-        GS_CUDA(h->dK.reserve(kbytes * gpb));
-    }
+    // ---- 3. group tasks by kernel matrix (kernel, gamma); 4. memory plan: batches of kernel matrices that fit in free HBM ----
+    if (const int rc = search.group("gs_svc", n_cand, n_splits, kernel, gamma)) return rc;
+    if (const int rc = search.plan_batches()) return rc;
+    const int n_groups = (int)search.groups.size(), gpb = search.per_batch;
 
     GS_CUDA(h->dWork[0].reserve(rows_all.size() * 4));
     GS_CUDA(cudaMemcpyAsync(h->dWork[0].p, rows_all.data(), rows_all.size() * 4, cudaMemcpyHostToDevice, st));
     pf.h2d_bytes += rows_all.size() * 4;
     const int *d_rows = h->dWork[0].as<int>();
 
-    std::vector<int> cnt_host;            // per task: 4 counters
     std::vector<int> task_iter(n_tasks, 0), task_sv(n_tasks, 0);
     std::vector<double> task_fit_ms(n_tasks, 0.0);
     std::vector<int> all_counts((size_t)n_tasks * 4, 0);
@@ -680,31 +615,15 @@ static int svc_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
     for (int g0 = 0; g0 < n_groups; g0 += gpb) {
         const int g1 = std::min(n_groups, g0 + gpb);
         // -- kernel matrices of this batch --
-        GS_CUDA(h->dWork[7].reserve(64));
-        GS_CUDA(cudaMemsetAsync(h->dWork[7].p, 0, 4, st));
-        bool fast = true;
-        for (int g = g0; g < g1; g++) {
-            GS_CUDA(launch_kernel_matrix(h->dS.as<double>(), h->dXsq.as<double>(), n, groups[g].first, groups[g].second,
-                                         h->dK.as<float>() + (size_t)(g - g0) * n * ldk, ldk, h->dWork[7].as<int>(), st));
-            pf.launches++;
-            fast = fast && groups[g].first == GS_KERNEL_RBF;
-        }
-        // The branch-free SMO instance needs rbf (QD == 1) and only positive normal floats in K.  The second condition is a
-        // device flag the kernel-matrix kernels raise: both instances are enqueued and the wrong one returns at once
-        // (SmoProblem::guard), so the host never waits in the middle of a search and everything it prepares below overlaps
-        // the Gram and kernel-matrix kernels already in flight.
-        if (getenv("B200GS_SMO_NOFAST") && atoi(getenv("B200GS_SMO_NOFAST"))) fast = false;   // development switch: general instance only, unguarded
-        const int *d_guard = fast ? h->dWork[7].as<int>() : nullptr;
-        tm.mark(1);
+        if (const int rc = search.kernel_matrices(g0, g1)) return rc;
         // -- problems: ordered by (group, task, pair); column index == problem index --
         std::vector<SmoProblem> probs;
         std::vector<int> prob_task, group_first(g1 - g0 + 1, 0);
         std::vector<VoteTask> vtasks;
         std::vector<int> vtask_id;
-        size_t wl = 0, ws = 0;            // workspace doubles / ints
         for (int g = g0; g < g1; g++) {
             group_first[g - g0] = (int)probs.size();
-            for (int t : group_tasks[g]) {
+            for (int t : search.group_tasks[g]) {
                 const int c = t / n_splits, k = t % n_splits;
                 vtasks.push_back(VoteTask{(int)probs.size(), refit ? -100 : k});
                 vtask_id.push_back(t);
@@ -713,7 +632,7 @@ static int svc_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
                     SmoProblem P;
                     memset(&P, 0, sizeof P);
                     P.K = h->dK.as<float>() + (size_t)(g - g0) * n * ldk;
-                    P.qd = groups[g].first == GS_KERNEL_LINEAR ? h->dXsq.as<double>() : nullptr;
+                    P.qd = search.groups[g].first == GS_KERNEL_LINEAR ? h->dXsq.as<double>() : nullptr;
                     P.rows = d_rows + sp_off[s];
                     P.l = sp_off[s + 1] - sp_off[s];
                     P.nseg = sp_nseg[s];
@@ -727,13 +646,9 @@ static int svc_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
                         P.C = Cv[c] * cw[a_]; P.Cn = Cv[c] * cw[b_];
                     }
                     P.shrinking = (flags & GS_NO_SHRINKING) ? 0 : 1;
-                    P.guard = d_guard;
+                    P.guard = search.d_guard;
                     P.nslots = 0;
                     for (int e = 0; e < P.nseg; e++) P.nslots += P.seg_len[e];
-                    const size_t wlen = ((size_t)std::max(P.l, P.nslots) + 3) & ~(size_t)3;   // by position or by slot, 32-byte multiples
-                    P.alpha = (double *)wl; wl += wlen;         // offsets now, pointers below
-                    P.Gbar = (double *)wl; wl += wlen;
-                    P.scratch = (int *)ws; ws += 2 * (size_t)P.l + 64;
                     probs.push_back(P);
                     prob_task.push_back(t);
                 }
@@ -741,31 +656,14 @@ static int svc_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
         }
         group_first[g1 - g0] = (int)probs.size();
         const int np = (int)probs.size();
-        // workspaces
-        GS_CUDA(h->dWork[1].reserve(wl * 8));
-        GS_CUDA(h->dWork[2].reserve(ws * 4));
-        GS_CUDA(h->dWork[3].reserve((size_t)np * n * 8));                 // coef columns
-        GS_CUDA(h->dWork[4].reserve((size_t)np * n * 8));                 // decision columns
-        GS_CUDA(h->dWork[5].reserve((size_t)np * (8 + 16 + 96) + 64));    // rho, info[4], ns[12]
+        if (const int rc = search.workspaces(probs)) return rc;
         GS_CUDA(h->dWork[6].reserve((size_t)np * sizeof(SmoProblem) + (size_t)np * 4 + vtasks.size() * (sizeof(VoteTask) + 16) + 256));
-        double *d_rho = h->dWork[5].as<double>();
-        int *d_info = (int *)(d_rho + np);
-        unsigned long long *d_ns = (unsigned long long *)(d_info + 4 * (size_t)np);
-        GS_CUDA(cudaMemsetAsync(d_ns, 0, (size_t)np * 12 * 8, st));
-        for (int q = 0; q < np; q++) {
-            SmoProblem &P = probs[q];
-            P.alpha = h->dWork[1].as<double>() + (size_t)P.alpha;
-            P.Gbar = h->dWork[1].as<double>() + (size_t)P.Gbar;
-            P.scratch = h->dWork[2].as<int>() + (size_t)P.scratch;
-            P.coef = h->dWork[3].as<double>() + (size_t)q * n;
-            P.out_rho = d_rho + q; P.out_info = d_info + 4 * (size_t)q; P.out_ns = d_ns + 12 * (size_t)q;
-        }
         // Predicted cost = rows x predicted SMO iterations (gs_svc_predicted_iterations): the predicted-longest problems lead
         // the launch order and the cluster policy below works on cost ratios.
         std::vector<double> cost(np);
         for (int q = 0; q < np; q++) {
             const int t = prob_task[q];
-            const auto &grp = groups[task_group[t]];
+            const auto &grp = search.groups[search.task_group[t]];
             cost[q] = gs_svc_predicted_iterations(grp.first, Cv[t / n_splits], grp.second, (int32_t)d) * (double)probs[q].l;
         }
         std::vector<int> order(np);
@@ -786,7 +684,7 @@ static int svc_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
         GS_CUDA(cudaMemsetAsync(d_counts, 0, vtasks.size() * 16, st));
         GS_CUDA(cudaMemsetAsync(h->dWork[3].p, 0, (size_t)np * n * 8, st));
         pf.h2d_bytes += (size_t)np * sizeof(SmoProblem) + (size_t)np * 4 + vtasks.size() * sizeof(VoteTask);
-        tm.mark(4);
+        search.tm.mark(4);
         // -- solve --
         // Policy: a 4-CTA cluster solves one problem in about half the time per iteration of the single-CTA kernel, but costs
         // twice the SM-time per iteration.  So clusters are for the critical path only:
@@ -804,7 +702,7 @@ static int svc_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
             max_slots = std::max(max_slots, probs[q].nslots);
         }
         auto launch_single = [&](const int *ord, int cnt, cudaStream_t s_, bool exclusive) -> cudaError_t {
-            for (int inst = fast ? 1 : 0; inst >= 0; inst--) {              // branch-free instance, then the general one (guarded)
+            for (int inst = search.fast ? 1 : 0; inst >= 0; inst--) {              // branch-free instance, then the general one (guarded)
                 const cudaError_t e = lean_ok ? launch_smo_lean(d_probs, ord, cnt, max_slots, inst == 1, exclusive, s_)
                                               : launch_smo(d_probs, ord, cnt, lmax, inst == 1, (int)ldk, s_, &why);
                 if (e != cudaSuccess) return e;
@@ -846,7 +744,7 @@ static int svc_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
             cudaEventRecord(ready, st);
             cudaError_t ce = cudaSuccess;
             if (n_cl > 0) {
-                for (int inst = fast ? 1 : 0; inst >= 0 && ce == cudaSuccess; inst--) {
+                for (int inst = search.fast ? 1 : 0; inst >= 0 && ce == cudaSuccess; inst--) {
                     ce = launch_smo_colown(d_probs, d_order, n_cl, lmax, cl, inst == 1, st);
                     pf.launches++;
                 }
@@ -877,27 +775,13 @@ static int svc_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
             cudaError_t ce = launch_single(d_order, np, st, false);
             if (ce != cudaSuccess) { gs_set_error(h, why.empty() ? std::string("launch_smo: ") + cudaGetErrorString(ce) : why); return why.empty() ? GS_ERR_CUDA : GS_ERR_UNSUPPORTED; }
         }
-        tm.mark(2);
+        search.tm.mark(2);
         // -- score (skipped for refit) --
         if (!refit) {
-            size_t part_doubles = 0;                                              // partial sums of the j-slabs
-            std::vector<int> jch(g1 - g0, 1);
-            for (int g = g0; g < g1; g++) {
-                const int cols = group_first[g - g0 + 1] - group_first[g - g0];
-                jch[g - g0] = decision_chunks(n, cols, h->sm_count);
-                if (jch[g - g0] > 1) part_doubles = std::max(part_doubles, (size_t)jch[g - g0] * cols * n);
-            }
-            if (part_doubles) GS_CUDA(h->dWork[8].reserve(part_doubles * 8));
-            for (int g = g0; g < g1; g++) {
-                const int c0 = group_first[g - g0], c1 = group_first[g - g0 + 1], jc = jch[g - g0];
-                GS_CUDA(launch_decision(h->dS.as<double>(), h->dXsq.as<double>(), n, groups[g].first, groups[g].second,
-                                        h->dWork[3].as<double>() + (size_t)c0 * n, c1 - c0,
-                                        h->dWork[4].as<double>() + (size_t)c0 * n, jc > 1 ? h->dWork[8].as<double>() : nullptr, jc, st));
-                pf.launches += jc > 1 ? 2 : 1;
-            }
+            if (const int rc = search.decisions(g0, g1, group_first)) return rc;
             const int kind = h->score_kind, nvt = (int)vtasks.size();
             if (kind == GS_SCORE_DEFAULT) {
-                GS_CUDA(launch_vote(h->dWork[4].as<double>(), d_rho, n, nc, h->dY.as<int>(), h->masks(),
+                GS_CUDA(launch_vote(h->dWork[4].as<double>(), search.d_rho, n, nc, h->dY.as<int>(), h->masks(),
                                     d_vt, nvt, d_counts, st));
             } else if (kind == GS_SCORE_ROC_AUC) {
                 // rank statistic of the decision values already in HBM (scikit-learn: roc_auc_score(y, decision_function(X)))
@@ -915,31 +799,20 @@ static int svc_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
             } else {
                 GS_CUDA(h->dScore.reserve((size_t)nvt * 2 * nc * 3 * 4));
                 GS_CUDA(cudaMemsetAsync(h->dScore.p, 0, (size_t)nvt * 2 * nc * 3 * 4, st));
-                GS_CUDA(launch_vote_classes(h->dWork[4].as<double>(), d_rho, n, nc, h->dY.as<int>(), h->masks(),
+                GS_CUDA(launch_vote_classes(h->dWork[4].as<double>(), search.d_rho, n, nc, h->dY.as<int>(), h->masks(),
                                             d_vt, nvt, h->dScore.as<int>(), st));
                 class_counts.resize((size_t)nvt * 2 * nc * 3);
                 GS_CUDA(cudaMemcpyAsync(class_counts.data(), h->dScore.p, class_counts.size() * 4, cudaMemcpyDeviceToHost, st));
             }
             pf.launches++;
         }
-        tm.mark(3);
+        search.tm.mark(3);
         // -- results of this batch --
-        std::vector<int> info((size_t)np * 4), counts(vtasks.size() * 4);
-        std::vector<unsigned long long> ns((size_t)np * 12);
-        std::vector<double> rho(np);
-        GS_CUDA(cudaMemcpyAsync(info.data(), d_info, info.size() * 4, cudaMemcpyDeviceToHost, st));
-        GS_CUDA(cudaMemcpyAsync(ns.data(), d_ns, ns.size() * 8, cudaMemcpyDeviceToHost, st));
-        GS_CUDA(cudaMemcpyAsync(rho.data(), d_rho, rho.size() * 8, cudaMemcpyDeviceToHost, st));
+        std::vector<int> counts(vtasks.size() * 4);
         GS_CUDA(cudaMemcpyAsync(counts.data(), d_counts, counts.size() * 4, cudaMemcpyDeviceToHost, st));
-        std::vector<double> coef_host;
-        if (refit && pair_coef) {
-            coef_host.resize((size_t)np * n);
-            GS_CUDA(cudaMemcpyAsync(coef_host.data(), h->dWork[3].p, coef_host.size() * 8, cudaMemcpyDeviceToHost, st));
-        }
-        GS_CUDA(cudaStreamSynchronize(st));
-        pf.d2h_bytes += info.size() * 4 + ns.size() * 8 + rho.size() * 8 + counts.size() * 4 + coef_host.size() * 8;
-        tm.collect(acc, 5);
-        tm.mark(-1);
+        pf.d2h_bytes += counts.size() * 4;
+        if (const int rc = search.results(np, refit && pair_coef)) return rc;
+        const auto &info = search.info; const auto &ns = search.ns; const auto &rho = search.rho;
         for (int q = 0; q < np; q++) {
             const int t = prob_task[q];
             task_iter[t] += info[(size_t)q * 4]; task_sv[t] += info[(size_t)q * 4 + 2];
@@ -1013,18 +886,11 @@ static int svc_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
                 if (rho_out) rho_out[q] = rho[q];
                 if (pair_iter) pair_iter[q] = info[(size_t)q * 4];
                 if (pair_coef)
-                    for (int r = 0; r < n; r++) pair_coef[(size_t)q * n + h->perm[r]] = coef_host[(size_t)q * n + r];
+                    for (int r = 0; r < n; r++) pair_coef[(size_t)q * n + h->perm[r]] = search.coef[(size_t)q * n + r];
             }
         }
     }
-    cudaEventRecord(ev_end, st);
-    GS_CUDA(cudaStreamSynchronize(st));
-    tm.collect(acc, 5);
-    cudaEventElapsedTime(&pf.ms_total, ev_begin, ev_end);
-    pf.ms_tensor = h->tt.collect(); pf.tensor_flops = h->tt.flops;
-    pf.ms_gram = acc[0]; pf.ms_kernel_matrix = acc[1]; pf.ms_solve = acc[2]; pf.ms_score = acc[3];
-    pf.smo_iterations = total_iter;
-    pf.solve_bytes = solve_bytes;
+    if (const int rc = search.finish(total_iter, solve_bytes)) return rc;
 
     if (!refit) {
         for (int t = 0; t < n_tasks; t++) {
@@ -1068,10 +934,8 @@ int gs_debug_gram(gs_handle *h, double *S_out, double *xsq_out)
     if (!h) return GS_ERR_ARG;
     if (h->n == 0) { gs_set_error(h, "gs_debug_gram: no dataset"); return GS_ERR_NO_DATA; }
     GS_CUDA(cudaSetDevice(h->device));
-    const int n = (int)h->n, d = (int)h->d;
-    GS_CUDA(h->dS.reserve((size_t)n * n * 8));
-    GS_CUDA(h->dXsq.reserve((size_t)n * 8));
-    GS_CUDA(launch_gram_f64(h->x_dtype == GS_F64 ? h->dX64.p : h->dX.p, h->x_dtype, n, d, h->dS.as<double>(), h->dXsq.as<double>(), h->stream));
+    const int n = (int)h->n;
+    if (const int rc = build_gram(h, 0, h->stream)) return rc;
     std::vector<double> S((size_t)n * n), xs(n);
     GS_CUDA(cudaMemcpyAsync(S.data(), h->dS.p, S.size() * 8, cudaMemcpyDeviceToHost, h->stream));
     GS_CUDA(cudaMemcpyAsync(xs.data(), h->dXsq.p, xs.size() * 8, cudaMemcpyDeviceToHost, h->stream));

@@ -93,8 +93,6 @@ struct EvTimer {       // accumulates elapsed ms between consecutive marks on on
     }
 };
 
-inline uint64_t dbits(double x) { uint64_t u; memcpy(&u, &x, 8); return u; }   // bit pattern: map key of a gamma
-
 // Membership of every row in the training / test set of every CV split: two 64-bit words per row and kind (splits 0..127).
 // Replaces the per-task index arrays of the reference (base_search.py:81-82 islice(cv.split(...))): any splitter fits --
 // overlapping test sets (RepeatedKFold), rows in neither set (ShuffleSplit), rows that only ever train (PredefinedSplit -1).
@@ -139,7 +137,7 @@ struct gs_handle {
     DevBuf dS, dXsq;                  // float64 Gram [n][n], squared norms [n]
     DevBuf dK;                        // float32 kernel matrices (batch)
     DevBuf dWork[9];                  // per-search scratch
-    DevBuf dScore;                    // class counts / AUC pair counts of the non-default scorers
+    DevBuf dScore;                    // class counts / AUC pair counts of the SVC scorers, SVR's residual sums of squares
     int score_kind = 0, score_pos = 1;   // gs_set_scoring
     std::vector<double> class_w;         // gs_set_class_weight: [sets][n_classes]; empty = all ones
     int class_w_sets = 0;
@@ -245,6 +243,40 @@ double gs_score_from_counts(int kind, int pos_class, int n_classes, const int *c
 // (z_r - (dec[first_col][r] - rho[first_col]))^2, float64, fixed-order block reduction (deterministic, no atomics).
 cudaError_t launch_rss(const double *dec, const double *rho, int n, const double *z, SplitMasks sm, const VoteTask *tasks,
                        int n_tasks, double *rss, cudaStream_t st);
+
+// ---- kernel_svm.cu: the host steps the SVC and SVR searches share (an int return is a GS_* status) ----
+int build_gram(gs_handle *h, uint32_t flags, cudaStream_t st);   // S = X X^T -> h->dS, diag(S) -> h->dXsq
+struct SvmSearch {                                 // the state of one svc_run / svr_run call
+    gs_handle *h;
+    cudaStream_t st;
+    int n;
+    int64_t ldk;                                   // row stride of the float32 kernel matrices in h->dK
+    EvTimer tm;
+    float acc[5] = {0, 0, 0, 0, 0};                // event time by phase: 0 gram, 1 kernel matrix, 2 solve, 3 score, 4 other
+    cudaEvent_t ev_begin = nullptr, ev_end = nullptr;
+    std::vector<std::pair<int, double>> groups;    // (kernel, gamma) of each kernel matrix, in order of first use
+    std::vector<int> task_group;                   // task c * n_splits + k -> its group
+    std::vector<std::vector<int>> group_tasks;     // group -> its tasks, ascending
+    int per_batch = 0;                             // kernel matrices per batch
+    bool fast = false;                             // this batch enqueues the branch-free SMO instance before the general one,
+    const int *d_guard = nullptr;                  // with this SmoProblem::guard
+    double *d_rho = nullptr;                       // outputs of the batch's problems (h->dWork[5]): rho [np], info [np][4],
+    int *d_info = nullptr;                         // ns [np][12], and their host copies; coef [np][n] only when asked for
+    unsigned long long *d_ns = nullptr;
+    std::vector<int> info;
+    std::vector<unsigned long long> ns;
+    std::vector<double> rho, coef;
+    SvmSearch(gs_handle *h_, cudaStream_t st_) : h(h_), st(st_), n((int)h_->n), ldk(((int64_t)h_->n + 31) & ~31LL), tm(st_, h_->evp) {}
+    void begin();                                  // resets h->prof but gs_set_data's ms_h2d / h2d_bytes; begin event
+    // groups the tasks by kernel matrix; rejects an rbf gamma that is not finite and > 0, with who in the message
+    int group(const char *who, int n_cand, int n_splits, const int32_t *kernel, const double *gamma);
+    int plan_batches();                            // per_batch; reserves h->dK
+    int kernel_matrices(int g0, int g1);           // group g at h->dK + (g - g0) n ldk, the guard flag, fast
+    int workspaces(std::vector<SmoProblem> &probs);   // alpha / Gbar / scratch / coef / outputs of every problem
+    int decisions(int g0, int g1, const std::vector<int> &group_first);   // group g: columns from group_first[g - g0]
+    int results(int np, bool with_coef);           // downloads the batch's outputs, syncs, collects its phase times
+    int finish(int64_t smo_iterations, double solve_bytes);   // end event, sync, the profile's times and totals
+};
 
 // ---- gemm_tc.cu: wgmma + TMA contraction  C[M][N] = sum_k A[M][k] B[N][k]  (3xTF32 split, fp32 accumulate) ----
 struct alignas(64) TcMap { unsigned char bytes[128]; };            // CUtensorMap

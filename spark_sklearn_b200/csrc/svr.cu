@@ -3,13 +3,12 @@
 // An SVR fit on l training rows is libsvm's C-SVC Solver on 2l variables (svm.cpp solve_epsilon_svr): positions 0..l-1 are
 // the rows with y = +1 and linear term eps - z, positions l..2l-1 the same rows with y = -1 and linear term eps + z.  The
 // solve is the position-owned SMO kernel of smo.cu (its SVR instance), so the iterate sequence is libsvm's; everything
-// around it -- float64 Gram, float32 kernel matrices per (kernel, gamma), float64 decision values -- is the SVC pipeline.
+// around it -- float64 Gram, float32 kernel matrices per (kernel, gamma), float64 decision values -- is the host pipeline
+// it shares with SVC (kernel_svm.cu).
 #include "common.cuh"
 #include <algorithm>
 #include <cmath>
 #include <cstring>
-#include <cstdlib>
-#include <map>
 #include <numeric>
 
 namespace {
@@ -89,10 +88,11 @@ static int svr_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
     }
     GS_CUDA(cudaSetDevice(h->device));
     cudaStream_t st = h->stream;
-    const int n = (int)h->n, d = (int)h->d;
+    const int n = (int)h->n;
     const int n_splits = refit ? 1 : h->n_splits;
     const int n_tasks = n_cand * n_splits;
-    const int64_t ldk = ((int64_t)n + 31) & ~31LL;
+    SvmSearch search(h, st);
+    const int64_t ldk = search.ldk;
 
     // ---- training rows of every split, ascending ORIGINAL index (scikit-learn fits X[train]), validated before any launch ----
     std::vector<int> by_orig(n);
@@ -119,23 +119,7 @@ static int svr_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
         lmax = std::max(lmax, 2 * l);
     }
     sp_off[n_splits] = (int)rows_all.size();
-
-    // ---- groups by kernel matrix (kernel, gamma) ----
-    std::map<std::pair<int, uint64_t>, int> gmap;
-    std::vector<std::pair<int, double>> groups;
-    std::vector<int> task_group(n_tasks);
-    for (int c = 0; c < n_cand; c++)
-        for (int k = 0; k < n_splits; k++) {
-            const double g = kernel[c] == GS_KERNEL_RBF ? gamma[(size_t)c * n_splits + k] : 0.0;
-            if (kernel[c] == GS_KERNEL_RBF && !(g > 0 && std::isfinite(g))) { gs_set_error(h, "gs_svr: gamma must be > 0"); return GS_ERR_ARG; }
-            auto key = std::make_pair((int)kernel[c], dbits(g));
-            auto it = gmap.find(key);
-            if (it == gmap.end()) { it = gmap.emplace(key, (int)groups.size()).first; groups.emplace_back(kernel[c], g); }
-            task_group[(size_t)c * n_splits + k] = it->second;
-        }
-    const int n_groups = (int)groups.size();
-    std::vector<std::vector<int>> group_tasks(n_groups);
-    for (int t = 0; t < n_tasks; t++) group_tasks[task_group[t]].push_back(t);
+    if (const int rc = search.group("gs_svr", n_cand, n_splits, kernel, gamma)) return rc;   // groups by kernel matrix (kernel, gamma)
 
     // ---- per-split sizes and r2 denominators (they depend on the split only) ----
     std::vector<double> tss((size_t)n_splits * 2, 0.0), cnt((size_t)n_splits * 2, 0.0);
@@ -159,59 +143,15 @@ static int svr_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
     }
 
     gs_profile &pf = h->prof;
-    const float keep_h2d = pf.ms_h2d; const int64_t keep_h2d_bytes = pf.h2d_bytes;
-    memset(&pf, 0, sizeof pf);
-    pf.ms_h2d = keep_h2d; pf.h2d_bytes = keep_h2d_bytes;
-    float acc[5] = {0, 0, 0, 0, 0};   // 0 gram, 1 kernel matrix, 2 solve, 3 score, 4 other
-    h->evp.reset(); h->tt.reset();
-    EvTimer tm(st, h->evp);
-    cudaEvent_t ev_begin = h->evp.get(), ev_end = h->evp.get();
-    cudaEventRecord(ev_begin, st);
-    tm.mark(-1);
+    search.begin();
 
-    // ---- 1. Gram X X^T in float64 (GS_GRAM_TENSOR: the fp32-faithful tensor-core Gram, opt-in) ----
-    GS_CUDA(h->dS.reserve((size_t)n * n * 8));
-    GS_CUDA(h->dXsq.reserve((size_t)n * 8));
-    if (flags & GS_GRAM_TENSOR) {
-        const int dpad = (d + 31) & ~31;
-        const int64_t ld32 = ((int64_t)n + 3) & ~3LL;
-        DevBuf &bx = h->dWork[1], &bs = h->dWork[2], &bb = h->dWork[6];
-        GS_CUDA(bx.reserve((size_t)n * dpad * 4 * 3));
-        GS_CUDA(bs.reserve((size_t)n * ld32 * 4));
-        GS_CUDA(bb.reserve(sizeof(TcBatch) + 64));
-        float *xp = bx.as<float>(), *xh = xp + (size_t)n * dpad, *xl = xh + (size_t)n * dpad;
-        GS_CUDA(cudaMemsetAsync(xp, 0, (size_t)n * dpad * 4, st));
-        GS_CUDA(cudaMemcpy2DAsync(xp, (size_t)dpad * 4, h->dX.p, (size_t)d * 4, (size_t)d * 4, n, cudaMemcpyDeviceToDevice, st));
-        GS_CUDA(launch_split_tf32(xp, xh, xl, (size_t)n * dpad, st));
-        TcMap mh, ml;
-        GS_CUDA(tc_make_map(&mh, xh, n, dpad, dpad));
-        GS_CUDA(tc_make_map(&ml, xl, n, dpad, dpad));
-        TcBatch hb{0, 0, 0, dpad, bs.as<float>(), ld32};
-        GS_CUDA(cudaMemcpyAsync(bb.p, &hb, sizeof hb, cudaMemcpyHostToDevice, st));
-        h->tt.begin(h->evp, st);
-        GS_CUDA(launch_gemm_nt_tf32x3(mh, ml, mh, ml, bb.as<TcBatch>(), 1, n, n, 1.0f, false, st, true));
-        h->tt.end(h->evp, st, 3.0 * 2.0 * n * (double)n * dpad);
-        GS_CUDA(launch_widen_gram(bs.as<float>(), n, ld32, h->dS.as<double>(), h->dXsq.as<double>(), st));
-        pf.launches += 3;
-    } else {
-        GS_CUDA(launch_gram_f64(h->x_dtype == GS_F64 ? h->dX64.p : h->dX.p, h->x_dtype, n, d, h->dS.as<double>(), h->dXsq.as<double>(), st));
-        pf.launches++;
-    }
-    pf.gram_flops = 2.0 * n * (double)n * d;
-    pf.gram_bytes = (double)n * d * 4 + (double)n * n * ((flags & GS_GRAM_TENSOR) ? 4 : 8);
-    tm.mark(0);
+    // ---- 1. Gram X X^T ----
+    if (const int rc = build_gram(h, flags, st)) return rc;
+    search.tm.mark(0);
 
-    // ---- 2. kernel matrices in batches that fit in free HBM (the rule of gs_svc) ----
-    const size_t kbytes = (size_t)n * ldk * 4;
-    int gpb = n_groups;
-    if (h->dK.cap < kbytes * (size_t)n_groups) {
-        size_t free_b = 0, total_b = 0;
-        GS_CUDA(cudaMemGetInfo(&free_b, &total_b));
-        free_b += h->dK.cap;
-        const size_t budget = (size_t)(free_b * 0.6);
-        gpb = (int)std::max<size_t>(1, std::min<size_t>(n_groups, budget / std::max<size_t>(kbytes, 1)));
-        GS_CUDA(h->dK.reserve(kbytes * gpb));
-    }
+    // ---- 2. kernel matrices in batches that fit in free HBM ----
+    if (const int rc = search.plan_batches()) return rc;
+    const int n_groups = (int)search.groups.size(), gpb = search.per_batch;
     GS_CUDA(h->dWork[0].reserve(rows_all.size() * 4));
     GS_CUDA(cudaMemcpyAsync(h->dWork[0].p, rows_all.data(), rows_all.size() * 4, cudaMemcpyHostToDevice, st));
     pf.h2d_bytes += rows_all.size() * 4;
@@ -225,74 +165,40 @@ static int svr_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
 
     for (int g0 = 0; g0 < n_groups; g0 += gpb) {
         const int g1 = std::min(n_groups, g0 + gpb);
-        GS_CUDA(h->dWork[7].reserve(64));
-        GS_CUDA(cudaMemsetAsync(h->dWork[7].p, 0, 4, st));
-        bool fast = true;
-        for (int g = g0; g < g1; g++) {
-            GS_CUDA(launch_kernel_matrix(h->dS.as<double>(), h->dXsq.as<double>(), n, groups[g].first, groups[g].second,
-                                         h->dK.as<float>() + (size_t)(g - g0) * n * ldk, ldk, h->dWork[7].as<int>(), st));
-            pf.launches++;
-            fast = fast && groups[g].first == GS_KERNEL_RBF;
-        }
-        // the branch-free instance and its device guard, as in gs_svc (SmoProblem::guard)
-        if (getenv("B200GS_SMO_NOFAST") && atoi(getenv("B200GS_SMO_NOFAST"))) fast = false;
-        const int *d_guard = fast ? h->dWork[7].as<int>() : nullptr;
-        tm.mark(1);
+        if (const int rc = search.kernel_matrices(g0, g1)) return rc;
 
         // ---- 3. one problem per (candidate, split), ordered by group: column index == problem index ----
         std::vector<SmoProblem> probs;
         std::vector<SvrData> svr;
         std::vector<int> prob_task, group_first(g1 - g0 + 1, 0);
         std::vector<VoteTask> vtasks;
-        size_t wl = 0, ws = 0;
         for (int g = g0; g < g1; g++) {
             group_first[g - g0] = (int)probs.size();
-            for (int t : group_tasks[g]) {
+            for (int t : search.group_tasks[g]) {
                 const int c = t / n_splits, k = t % n_splits;
                 vtasks.push_back(VoteTask{(int)probs.size(), refit ? -100 : k});
                 SmoProblem P;
                 memset(&P, 0, sizeof P);
                 P.K = h->dK.as<float>() + (size_t)(g - g0) * n * ldk;
-                P.qd = groups[g].first == GS_KERNEL_LINEAR ? h->dXsq.as<double>() : nullptr;
+                P.qd = search.groups[g].first == GS_KERNEL_LINEAR ? h->dXsq.as<double>() : nullptr;
                 P.rows = d_rows + sp_off[k];
                 P.l = sp_off[k + 1] - sp_off[k];
                 P.n_pos = P.l / 2;
                 P.nseg = 0;                                   // bulk row copies take the whole row
                 P.ldk = ldk; P.C = Cv[c]; P.Cn = Cv[c]; P.eps = tol; P.max_iter = max_iter;
                 P.shrinking = (flags & GS_NO_SHRINKING) ? 0 : 1;
-                P.guard = d_guard;
-                const size_t wlen = ((size_t)P.l + 3) & ~(size_t)3;
-                P.alpha = (double *)wl; wl += wlen;           // offsets now, pointers below
-                P.Gbar = (double *)wl; wl += wlen;
-                P.scratch = (int *)ws; ws += 2 * (size_t)P.l + 64;
+                P.guard = search.d_guard;
                 probs.push_back(P);
-                svr.push_back(SvrData{nullptr, epsv[c]});
+                svr.push_back(SvrData{h->dZ64.as<double>(), epsv[c]});
                 prob_task.push_back(t);
             }
         }
         group_first[g1 - g0] = (int)probs.size();
         const int np = (int)probs.size();
-        GS_CUDA(h->dWork[1].reserve(wl * 8));
-        GS_CUDA(h->dWork[2].reserve(ws * 4));
-        GS_CUDA(h->dWork[3].reserve((size_t)np * n * 8));                 // coef columns
-        GS_CUDA(h->dWork[4].reserve((size_t)np * n * 8));                 // decision columns
-        GS_CUDA(h->dWork[5].reserve((size_t)np * (8 + 16 + 96 + 16) + 64)); // rho, info[4], ns[12], rss[2]
+        if (const int rc = search.workspaces(probs)) return rc;
         const size_t meta_bytes = (size_t)np * (sizeof(SmoProblem) + sizeof(SvrData) + 4) + vtasks.size() * sizeof(VoteTask) + 256;
         GS_CUDA(h->dWork[6].reserve(meta_bytes));
-        double *d_rho = h->dWork[5].as<double>();
-        double *d_rss = d_rho + np;
-        int *d_info = (int *)(d_rss + 2 * (size_t)np);
-        unsigned long long *d_ns = (unsigned long long *)(d_info + 4 * (size_t)np);
-        GS_CUDA(cudaMemsetAsync(d_ns, 0, (size_t)np * 12 * 8, st));
-        for (int q = 0; q < np; q++) {
-            SmoProblem &P = probs[q];
-            P.alpha = h->dWork[1].as<double>() + (size_t)P.alpha;
-            P.Gbar = h->dWork[1].as<double>() + (size_t)P.Gbar;
-            P.scratch = h->dWork[2].as<int>() + (size_t)P.scratch;
-            P.coef = h->dWork[3].as<double>() + (size_t)q * n;
-            P.out_rho = d_rho + q; P.out_info = d_info + 4 * (size_t)q; P.out_ns = d_ns + 12 * (size_t)q;
-            svr[q].z = h->dZ64.as<double>();
-        }
+        GS_CUDA(h->dScore.reserve((size_t)np * 2 * 8));                   // rss[np][2]
         // ---- 4. launch order: longest predicted first.  There is no iteration model for SVR yet; C x l orders the
         // problems (larger C and more rows mean more iterations in the measured searches) until one is calibrated.
         std::vector<double> cost(np);
@@ -314,9 +220,9 @@ static int svr_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
         GS_CUDA(cudaMemcpyAsync(d_vt, vtasks.data(), vtasks.size() * sizeof(VoteTask), cudaMemcpyHostToDevice, st));
         GS_CUDA(cudaMemsetAsync(h->dWork[3].p, 0, (size_t)np * n * 8, st));
         pf.h2d_bytes += (size_t)np * (sizeof(SmoProblem) + sizeof(SvrData) + 4) + vtasks.size() * sizeof(VoteTask);
-        tm.mark(4);
+        search.tm.mark(4);
         // ---- 5. solve: one launch per instance (branch-free first, then the guarded general one) ----
-        for (int inst = fast ? 1 : 0; inst >= 0; inst--) {
+        for (int inst = search.fast ? 1 : 0; inst >= 0; inst--) {
             std::string why;
             const cudaError_t ce = launch_smo_svr(d_probs, d_svr, d_order, np, lmax, inst == 1, (int)ldk, st, &why);
             if (ce != cudaSuccess) {
@@ -325,44 +231,23 @@ static int svr_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
             }
             pf.launches++;
         }
-        tm.mark(2);
+        search.tm.mark(2);
         // ---- 6. decision values (float64 kernel, every row) and residual sums of squares ----
         if (!refit) {
-            size_t part_doubles = 0;
-            std::vector<int> jch(g1 - g0, 1);
-            for (int g = g0; g < g1; g++) {
-                const int cols = group_first[g - g0 + 1] - group_first[g - g0];
-                jch[g - g0] = decision_chunks(n, cols, h->sm_count);
-                if (jch[g - g0] > 1) part_doubles = std::max(part_doubles, (size_t)jch[g - g0] * cols * n);
-            }
-            if (part_doubles) GS_CUDA(h->dWork[8].reserve(part_doubles * 8));
-            for (int g = g0; g < g1; g++) {
-                const int c0 = group_first[g - g0], c1 = group_first[g - g0 + 1], jc = jch[g - g0];
-                GS_CUDA(launch_decision(h->dS.as<double>(), h->dXsq.as<double>(), n, groups[g].first, groups[g].second,
-                                        h->dWork[3].as<double>() + (size_t)c0 * n, c1 - c0,
-                                        h->dWork[4].as<double>() + (size_t)c0 * n, jc > 1 ? h->dWork[8].as<double>() : nullptr, jc, st));
-                pf.launches += jc > 1 ? 2 : 1;
-            }
-            GS_CUDA(launch_rss(h->dWork[4].as<double>(), d_rho, n, h->dZ64.as<double>(), h->masks(), d_vt, (int)vtasks.size(), d_rss, st));
+            if (const int rc = search.decisions(g0, g1, group_first)) return rc;
+            GS_CUDA(launch_rss(h->dWork[4].as<double>(), search.d_rho, n, h->dZ64.as<double>(), h->masks(), d_vt, (int)vtasks.size(),
+                               h->dScore.as<double>(), st));
             pf.launches++;
         }
-        tm.mark(3);
+        search.tm.mark(3);
         // ---- results of this batch ----
-        std::vector<int> info((size_t)np * 4);
-        std::vector<unsigned long long> ns((size_t)np * 12);
-        std::vector<double> rho(np), rss((size_t)np * 2, 0.0), coef_host;
-        GS_CUDA(cudaMemcpyAsync(info.data(), d_info, info.size() * 4, cudaMemcpyDeviceToHost, st));
-        GS_CUDA(cudaMemcpyAsync(ns.data(), d_ns, ns.size() * 8, cudaMemcpyDeviceToHost, st));
-        GS_CUDA(cudaMemcpyAsync(rho.data(), d_rho, rho.size() * 8, cudaMemcpyDeviceToHost, st));
-        if (!refit) GS_CUDA(cudaMemcpyAsync(rss.data(), d_rss, rss.size() * 8, cudaMemcpyDeviceToHost, st));
-        if (refit && coef_out) {
-            coef_host.resize((size_t)np * n);
-            GS_CUDA(cudaMemcpyAsync(coef_host.data(), h->dWork[3].p, coef_host.size() * 8, cudaMemcpyDeviceToHost, st));
+        std::vector<double> rss((size_t)np * 2, 0.0);
+        if (!refit) {
+            GS_CUDA(cudaMemcpyAsync(rss.data(), h->dScore.p, rss.size() * 8, cudaMemcpyDeviceToHost, st));
+            pf.d2h_bytes += rss.size() * 8;
         }
-        GS_CUDA(cudaStreamSynchronize(st));
-        pf.d2h_bytes += info.size() * 4 + ns.size() * 8 + rho.size() * 8 + (refit ? 0 : rss.size() * 8) + coef_host.size() * 8;
-        tm.collect(acc, 5);
-        tm.mark(-1);
+        if (const int rc = search.results(np, refit && coef_out)) return rc;
+        const auto &info = search.info; const auto &ns = search.ns; const auto &rho = search.rho;
         for (int q = 0; q < np; q++) {
             const int t = prob_task[q];
             task_iter[t] = info[(size_t)q * 4]; task_sv[t] = info[(size_t)q * 4 + 2];
@@ -377,17 +262,10 @@ static int svr_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
             if (rho_out) *rho_out = rho[0];
             if (n_iter) *n_iter = info[0];
             if (coef_out)
-                for (int r = 0; r < n; r++) coef_out[h->perm[r]] = coef_host[r];
+                for (int r = 0; r < n; r++) coef_out[h->perm[r]] = search.coef[r];
         }
     }
-    cudaEventRecord(ev_end, st);
-    GS_CUDA(cudaStreamSynchronize(st));
-    tm.collect(acc, 5);
-    cudaEventElapsedTime(&pf.ms_total, ev_begin, ev_end);
-    pf.ms_tensor = h->tt.collect(); pf.tensor_flops = h->tt.flops;
-    pf.ms_gram = acc[0]; pf.ms_kernel_matrix = acc[1]; pf.ms_solve = acc[2]; pf.ms_score = acc[3];
-    pf.smo_iterations = total_iter;
-    pf.solve_bytes = solve_bytes;
+    if (const int rc = search.finish(total_iter, solve_bytes)) return rc;
 
     if (!refit) {
         for (int t = 0; t < n_tasks; t++) {

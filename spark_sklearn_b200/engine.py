@@ -174,8 +174,10 @@ class Engine:
         self._check(self._L.gs_set_data(self._h, _ptr(X), 0 if X.dtype == np.float32 else 1, X.shape[0], X.shape[1], _ptr(yc), _ptr(yt),
                                         _ptr(fold_id), int(n_splits)))
 
-    # -- map(fun).collect() for SVC (reference base_search.py:74-95) --
-    def svc(self, kernel, C, gamma, tol=1e-3, max_iter=-1, shrinking=True, return_train=True, flags=0):
+    # -- map(fun).collect() for SVC and epsilon-SVR (reference base_search.py:74-95) --
+    def _kernel_svm(self, fn, kernel, C, per_cand, gamma, tol, max_iter, shrinking, return_train, flags):
+        """gs_svc / gs_svr: kernel names or ids, C and the estimator's other per-candidate arrays (per_cand), gamma per
+        candidate or per (candidate, split) -> the per-(candidate, split) outputs"""
         kernel = np.ascontiguousarray([KERNEL_ID[k] if isinstance(k, str) else int(k) for k in kernel], np.int32)
         C = np.ascontiguousarray(C, np.float64)
         n_cand = len(C)
@@ -186,12 +188,15 @@ class Engine:
                    n_sv=np.zeros(shape, np.int32), fit_ms=np.zeros(shape, np.float32),
                    score_ms=np.zeros(shape, np.float32))
         fl = int(flags) | (GS_RETURN_TRAIN if return_train else 0) | (0 if shrinking else GS_NO_SHRINKING)
-        self._check(self._L.gs_svc(self._h, n_cand, _ptr(kernel), _ptr(C), _ptr(gamma), float(tol), int(max_iter), fl,
-                                   _ptr(out["test"]), _ptr(out["train"]), _ptr(out["n_iter"]), _ptr(out["n_sv"]),
-                                   _ptr(out["fit_ms"]), _ptr(out["score_ms"])))
+        self._check(fn(self._h, n_cand, _ptr(kernel), _ptr(C), *[_ptr(a) for a in per_cand], _ptr(gamma), float(tol),
+                       int(max_iter), fl, _ptr(out["test"]), _ptr(out["train"]), _ptr(out["n_iter"]), _ptr(out["n_sv"]),
+                       _ptr(out["fit_ms"]), _ptr(out["score_ms"])))
         if not return_train:
             out["train"] = None
         return out
+
+    def svc(self, kernel, C, gamma, tol=1e-3, max_iter=-1, shrinking=True, return_train=True, flags=0):
+        return self._kernel_svm(self._L.gs_svc, kernel, C, [], gamma, tol, max_iter, shrinking, return_train, flags)
 
     def svc_refit(self, kernel, C, gamma, n_classes, tol=1e-3, max_iter=-1, shrinking=True):
         n_pairs = n_classes * (n_classes - 1) // 2
@@ -210,25 +215,9 @@ class Engine:
             raise ValueError("y has shape %r; expected (%d,)" % (y.shape, self.n))
         self._check(self._L.gs_set_targets_f64(self._h, _ptr(y)))
 
-    # -- map(fun).collect() for epsilon-SVR --
     def svr(self, kernel, C, epsilon, gamma, tol=1e-3, max_iter=-1, shrinking=True, return_train=True, flags=0):
-        kernel = np.ascontiguousarray([KERNEL_ID[k] if isinstance(k, str) else int(k) for k in kernel], np.int32)
-        C = np.ascontiguousarray(C, np.float64)
-        n_cand = len(C)
-        epsilon = np.ascontiguousarray(np.broadcast_to(np.asarray(epsilon, np.float64), (n_cand,)))
-        gamma = np.ascontiguousarray(np.broadcast_to(np.asarray(gamma, np.float64).reshape(n_cand, -1),
-                                                     (n_cand, self.n_splits)))
-        shape = (n_cand, self.n_splits)
-        out = dict(test=np.zeros(shape), train=np.zeros(shape), n_iter=np.zeros(shape, np.int32),
-                   n_sv=np.zeros(shape, np.int32), fit_ms=np.zeros(shape, np.float32),
-                   score_ms=np.zeros(shape, np.float32))
-        fl = int(flags) | (GS_RETURN_TRAIN if return_train else 0) | (0 if shrinking else GS_NO_SHRINKING)
-        self._check(self._L.gs_svr(self._h, n_cand, _ptr(kernel), _ptr(C), _ptr(epsilon), _ptr(gamma), float(tol),
-                                   int(max_iter), fl, _ptr(out["test"]), _ptr(out["train"]), _ptr(out["n_iter"]),
-                                   _ptr(out["n_sv"]), _ptr(out["fit_ms"]), _ptr(out["score_ms"])))
-        if not return_train:
-            out["train"] = None
-        return out
+        epsilon = np.ascontiguousarray(np.broadcast_to(np.asarray(epsilon, np.float64), (len(C),)))
+        return self._kernel_svm(self._L.gs_svr, kernel, C, [epsilon], gamma, tol, max_iter, shrinking, return_train, flags)
 
     def svr_refit(self, kernel, C, epsilon, gamma, tol=1e-3, max_iter=-1, shrinking=True, flags=0):
         """-> (coef [n] by row: alpha+ - alpha-, rho, n_iter); prediction = sum coef k(x, x_row) - rho"""

@@ -273,7 +273,8 @@ class SVCAdapter:
 
 
 class _KernelGamma:
-    """gamma of one libsvm fit: sklearn svm/_base.py:278-286, shared by the SVC and SVR plans."""
+    """What the SVC and SVR plans share: the gamma of one libsvm fit (sklearn svm/_base.py:278-286), the kernel-matrix
+    affinity of the candidates and the Gram mode."""
 
     def _gamma(self, g, k):
         """'scale' uses the variance of the TRAINING fold (float64); k < 0: all rows."""
@@ -290,6 +291,22 @@ class _KernelGamma:
         if not (isinstance(g, numbers.Real) and g >= 0):
             raise ValueError("gamma must be >= 0 or 'scale'/'auto'; got %r" % (g,))
         return float(g)
+
+    def affinity(self):
+        """Candidates with the same (kernel, gamma) share a kernel matrix and a decision-value pass."""
+        try:
+            out = []
+            for cand in self.cands:
+                p = self._base_params(cand)
+                out.append((p["kernel"], self._gamma(p["gamma"], -1) if p["kernel"] == "rbf" else 0.0))
+            return out
+        except Exception:
+            return None
+
+    def _flags(self):
+        import os
+        # B200GS_GRAM=tensor: opt-in wgmma Gram (fp32-faithful; scores match to solver tolerance, not bit for bit)
+        return 2 if os.environ.get("B200GS_GRAM", "exact") == "tensor" else 0
 
 
 class SVCPlan(_KernelGamma, _Plan):
@@ -335,17 +352,6 @@ class SVCPlan(_KernelGamma, _Plan):
             return None                                 # invalid candidates are reported by evaluate()
         return out
 
-    def affinity(self):
-        """Candidates with the same (kernel, gamma) share a kernel matrix and a decision-value pass."""
-        try:
-            out = []
-            for cand in self.cands:
-                p = self._base_params(cand)
-                out.append((p["kernel"], self._gamma(p["gamma"], -1) if p["kernel"] == "rbf" else 0.0))
-            return out
-        except Exception:
-            return None
-
     def evaluate(self, my, return_train=True, error_score='raise'):
         ns = self.n_splits
         shape = (len(my), ns)
@@ -367,12 +373,9 @@ class SVCPlan(_KernelGamma, _Plan):
             C = [float(params[j]["C"]) for j in idx]
             gam = np.array([[self._gamma(params[j]["gamma"], k) if params[j]["kernel"] == "rbf" else 0.0
                              for k in range(ns)] for j in idx])
-            # B200GS_GRAM=tensor: opt-in wgmma Gram (fp32-faithful; scores match to solver tolerance, not bit for bit)
-            import os
-            flags = 2 if os.environ.get("B200GS_GRAM", "exact") == "tensor" else 0
             self.engine.set_scoring(self.score_kind, self.score_pos)
             r = self.engine.svc(kern, C, gam, tol=tol, max_iter=max_iter, shrinking=shrinking,
-                                return_train=return_train, flags=flags)
+                                return_train=return_train, flags=self._flags())
             for key in ("test", "fit_ms", "score_ms", "n_iter"):
                 res[key][idx] = r[key]
             if return_train:
@@ -480,22 +483,6 @@ class SVRPlan(_KernelGamma, _Plan):
             raise ValueError("C must be a positive number; got %r" % (p["C"],))
         if not (isinstance(p["epsilon"], numbers.Real) and p["epsilon"] >= 0):
             raise ValueError("epsilon must be a non-negative number; got %r" % (p["epsilon"],))
-
-    def affinity(self):
-        """Candidates with the same (kernel, gamma) share a kernel matrix and a decision-value pass."""
-        try:
-            out = []
-            for cand in self.cands:
-                p = self._base_params(cand)
-                out.append((p["kernel"], self._gamma(p["gamma"], -1) if p["kernel"] == "rbf" else 0.0))
-            return out
-        except Exception:
-            return None
-
-    def _flags(self):
-        import os
-        # B200GS_GRAM=tensor: opt-in wgmma Gram (fp32-faithful; scores match to solver tolerance, not bit for bit)
-        return 2 if os.environ.get("B200GS_GRAM", "exact") == "tensor" else 0
 
     max_rows = 8192        # training rows of one fit: 2 x 8192 solver variables, the largest resident-state SMO instance
 

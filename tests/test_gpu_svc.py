@@ -127,6 +127,26 @@ def test_no_shrinking_and_max_iter(engine):
             assert r["train"][0, k] == s.score(X[tr], y[tr])
 
 
+@pytest.mark.parametrize("method", ["svc", "svr"])
+def test_non_finite_gamma_is_rejected(engine, method):
+    """An infinite rbf gamma would put NaN on the kernel diagonal (-inf * 0): both searches refuse it before any launch."""
+    from spark_sklearn_b200.engine import EngineError
+    rng = np.random.RandomState(0)
+    X = rng.randn(40, 3).astype(np.float32)
+    fold_id = (np.arange(40) % 2).astype(np.int8)
+    if method == "svc":
+        engine.set_data(X, fold_id, 2, y_class=(np.arange(40) // 2 % 2).astype(np.int32))
+        search = lambda g: engine.svc(["rbf"], [1.0], [g])
+    else:
+        y = rng.randn(40)
+        engine.set_data(X, fold_id, 2, y_target=y.astype(np.float32))
+        engine.set_targets_f64(y)
+        search = lambda g: engine.svr(["rbf"], [1.0], [0.1], [g])
+    with pytest.raises(EngineError, match="gamma must be finite"):
+        search(np.inf)
+    assert np.all(np.isfinite(search(0.5)["test"]))        # the handle stays usable
+
+
 def test_python_api_iris(engine):
     """The reference's own example (tests/test_search_2.py:32-45, README): iris, SVC(gamma='auto')."""
     from sklearn import svm
