@@ -41,7 +41,7 @@ enum gs_status {
     GS_ERR_NUMERIC = -5      /* non-finite result (maps to the reference's error_score)      */
 };
 
-enum gs_kernel { GS_KERNEL_LINEAR = 0, GS_KERNEL_RBF = 1 };
+enum gs_kernel { GS_KERNEL_LINEAR = 0, GS_KERNEL_RBF = 1, GS_KERNEL_POLY = 2, GS_KERNEL_SIGMOID = 3 };
 enum gs_dtype { GS_F32 = 0, GS_F64 = 1 };
 
 enum gs_flags {
@@ -71,6 +71,14 @@ int gs_set_splits(gs_handle *h, const uint64_t *test_mask, const uint64_t *train
  * per fold), hence one weight set per split: w is [n_sets][n_classes], n_sets = n_splits (search), 1 (refit, or the same
  * weights for every split); w == NULL resets to all ones. */
 int gs_set_class_weight(gs_handle *h, const double *w, int32_t n_sets);
+
+/* Polynomial / sigmoid kernel parameters of the next gs_svc (n = n_cand), gs_svc_refit or gs_debug_kernel_matrix (n = 1):
+ * SVC(degree=..., coef0=...), one value per candidate.  libsvm's kernels (svm.cpp Kernel): poly = powi(gamma x.y + coef0,
+ * degree), sigmoid = tanh(gamma x.y + coef0); gamma is resolved per split as for rbf and may be any finite value >= 0.
+ * Linear and rbf candidates ignore both values.  degree == NULL resets every candidate to scikit-learn's defaults (degree 3,
+ * coef0 0), as does gs_set_data.  A call whose count differs from its n_cand fails with GS_ERR_ARG, as does a degree < 0 or a
+ * coef0 that is not finite.  gs_svr keeps rejecting the poly and sigmoid kernels (GS_ERR_UNSUPPORTED). */
+int gs_set_kernel_params(gs_handle *h, const int32_t *degree, const double *coef0, int32_t n);
 
 /* Sample weights of the following gs_ridge / gs_enet / gs_logreg calls and their refits.  Replaces: fit_params={'sample_weight': w}
  * handed to every task's estimator.fit (reference base_search.py:69,83-87; scikit-learn's _fit_and_score slices it by the
@@ -117,7 +125,8 @@ int gs_set_data(gs_handle *h, const void *X, int32_t x_dtype, int64_t n, int64_t
 /*
  * SVC (C-SVC, one-vs-one; replaces _fit_and_score -> SVC.fit/score = sklearn libsvm,
  * svm.cpp:2365 svm_train, :666 Solver::Solve, :2821 svm_predict_values).
- *   kernel[n_cand], C[n_cand]; gamma[n_cand*n_splits] (already resolved per fold: 'scale' depends
+ *   kernel[n_cand] (GS_KERNEL_*; poly / sigmoid read degree and coef0 from gs_set_kernel_params), C[n_cand];
+ *   gamma[n_cand*n_splits] (already resolved per fold: 'scale' depends
  *   on the training fold, sklearn svm/_base.py:278-286).  tol = SVC.tol, max_iter = SVC.max_iter
  *   (-1: none).  Outputs, all [n_cand*n_splits], candidate-major: test_scores / train_scores
  *   (accuracy, float64; train may be NULL without GS_RETURN_TRAIN), n_iter (sum over OvO pairs),
@@ -199,7 +208,8 @@ int gs_svr_refit(gs_handle *h, int32_t kernel, double C, double epsilon, double 
 /* ---- test hooks (used by tests/ to localise a parity failure to one kernel) ---------------- */
 /* S_out [n][n] float64 Gram X X^T and xsq_out [n] (either may be NULL), in ORIGINAL row order.  */
 int gs_debug_gram(gs_handle *h, double *S_out, double *xsq_out);
-/* K_out [n][n] float32 kernel matrix (the SMO solver's Q without the y_i*y_j sign), original order. */
+/* K_out [n][n] float32 kernel matrix (the SMO solver's Q without the y_i*y_j sign), original order; poly / sigmoid take
+ * degree and coef0 from gs_set_kernel_params (n = 1). */
 int gs_debug_kernel_matrix(gs_handle *h, int32_t kernel, double gamma, float *K_out);
 
 /* C[M][N] = sum_k A[M][k]*B[N][k] on the wgmma tensor-core path (3xTF32 split), host fp32 row-major in/out. */

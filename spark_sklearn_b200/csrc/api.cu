@@ -1,4 +1,5 @@
-// api.cu -- the C ABI of libb200gs.so (include/b200gs.h): lifecycle, dataset upload, SVC search/refit (SVR: svr.cu).
+// api.cu -- the C ABI of libb200gs.so (include/b200gs.h): lifecycle, dataset upload, SVC search/refit (linear, rbf, poly,
+// sigmoid kernels; SVR: svr.cu).
 // Host-side planning only; every floating-point operation of the hot path runs in the CUDA kernels
 // of gram.cu / smo.cu / score.cu.  There is no CPU fallback.
 #include "common.cuh"
@@ -89,6 +90,19 @@ int gs_set_class_weight(gs_handle *h, const double *w, int32_t n_sets)
         if (!(w[i] > 0) || !std::isfinite(w[i])) { gs_set_error(h, "gs_set_class_weight: weights must be positive and finite"); return GS_ERR_ARG; }
     h->class_w.assign(w, w + (size_t)n_sets * h->n_classes);
     h->class_w_sets = n_sets;
+    return GS_OK;
+}
+
+int gs_set_kernel_params(gs_handle *h, const int32_t *degree, const double *coef0, int32_t n)
+{
+    if (!h) return GS_ERR_ARG;
+    if (!degree || !coef0 || n <= 0) { h->kp_degree.clear(); h->kp_coef0.clear(); return GS_OK; }
+    for (int i = 0; i < n; i++)
+        if (degree[i] < 0 || !std::isfinite(coef0[i])) {
+            gs_set_error(h, "gs_set_kernel_params: degree must be >= 0 and coef0 finite"); return GS_ERR_ARG;
+        }
+    h->kp_degree.assign(degree, degree + n);
+    h->kp_coef0.assign(coef0, coef0 + n);
     return GS_OK;
 }
 
@@ -203,6 +217,7 @@ int gs_set_data(gs_handle *h, const void *X, int32_t x_dtype, int64_t n, int64_t
     h->class_w.clear(); h->class_w_sets = 0;
     h->sample_w.clear();
     h->z64.clear();
+    h->kp_degree.clear(); h->kp_coef0.clear();
     h->perm.resize(n);
     std::iota(h->perm.begin(), h->perm.end(), 0);
     h->n_classes = 0;
@@ -524,9 +539,16 @@ static int svc_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
     const int n_tasks = n_cand * n_splits;
     const int64_t ldk = ((int64_t)n + 31) & ~31LL;
     for (int c = 0; c < n_cand; c++) {
-        if (kernel[c] != GS_KERNEL_LINEAR && kernel[c] != GS_KERNEL_RBF) { gs_set_error(h, "gs_svc: unsupported kernel id"); return GS_ERR_UNSUPPORTED; }
+        if (kernel[c] < GS_KERNEL_LINEAR || kernel[c] > GS_KERNEL_SIGMOID) { gs_set_error(h, "gs_svc: unsupported kernel id"); return GS_ERR_UNSUPPORTED; }
         if (!(Cv[c] > 0)) { gs_set_error(h, "gs_svc: C must be > 0"); return GS_ERR_ARG; }
     }
+    if (!h->kp_degree.empty() && (int)h->kp_degree.size() != n_cand) {
+        gs_set_error(h, "gs_svc: gs_set_kernel_params was given " + std::to_string(h->kp_degree.size()) + " candidates, this call has " +
+                            std::to_string(n_cand));
+        return GS_ERR_ARG;
+    }
+    const int32_t *degree = h->kp_degree.empty() ? nullptr : h->kp_degree.data();
+    const double *coef0 = h->kp_coef0.empty() ? nullptr : h->kp_coef0.data();
 
     gs_profile &pf = h->prof;
     SvmSearch search(h, st);
@@ -584,8 +606,8 @@ static int svc_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
         return GS_ERR_UNSUPPORTED;
     }
 
-    // ---- 3. group tasks by kernel matrix (kernel, gamma); 4. memory plan: batches of kernel matrices that fit in free HBM ----
-    if (const int rc = search.group("gs_svc", n_cand, n_splits, kernel, gamma)) return rc;
+    // ---- 3. group tasks by kernel matrix (kernel, gamma, degree, coef0); 4. memory plan: batches of kernel matrices that fit in free HBM ----
+    if (const int rc = search.group("gs_svc", n_cand, n_splits, kernel, gamma, degree, coef0)) return rc;
     if (const int rc = search.plan_batches()) return rc;
     const int n_groups = (int)search.groups.size(), gpb = search.per_batch;
 
@@ -632,7 +654,7 @@ static int svc_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
                     SmoProblem P;
                     memset(&P, 0, sizeof P);
                     P.K = h->dK.as<float>() + (size_t)(g - g0) * n * ldk;
-                    P.qd = search.groups[g].first == GS_KERNEL_LINEAR ? h->dXsq.as<double>() : nullptr;
+                    P.qd = search.qd(g, g0);
                     P.rows = d_rows + sp_off[s];
                     P.l = sp_off[s + 1] - sp_off[s];
                     P.nseg = sp_nseg[s];
@@ -664,7 +686,7 @@ static int svc_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
         for (int q = 0; q < np; q++) {
             const int t = prob_task[q];
             const auto &grp = search.groups[search.task_group[t]];
-            cost[q] = gs_svc_predicted_iterations(grp.first, Cv[t / n_splits], grp.second, (int32_t)d) * (double)probs[q].l;
+            cost[q] = gs_svc_predicted_iterations(grp.kernel, Cv[t / n_splits], grp.gamma, (int32_t)d) * (double)probs[q].l;
         }
         std::vector<int> order(np);
         std::iota(order.begin(), order.end(), 0);
@@ -951,12 +973,16 @@ int gs_debug_gram(gs_handle *h, double *S_out, double *xsq_out)
 int gs_debug_kernel_matrix(gs_handle *h, int32_t kernel, double gamma, float *K_out)
 {
     if (!h || !K_out) return GS_ERR_ARG;
+    if (kernel < GS_KERNEL_LINEAR || kernel > GS_KERNEL_SIGMOID) { gs_set_error(h, "gs_debug_kernel_matrix: unsupported kernel id"); return GS_ERR_UNSUPPORTED; }
+    if (h->kp_degree.size() > 1) { gs_set_error(h, "gs_debug_kernel_matrix: gs_set_kernel_params was given more than one candidate"); return GS_ERR_ARG; }
+    const KernelSpec ks(kernel, gamma, h->kp_degree.empty() ? 3 : h->kp_degree[0], h->kp_coef0.empty() ? 0.0 : h->kp_coef0[0]);
     int st = gs_debug_gram(h, nullptr, nullptr);
     if (st) return st;
     const int n = (int)h->n;
     const int64_t ldk = ((int64_t)n + 31) & ~31LL;
     GS_CUDA(h->dK.reserve((size_t)n * ldk * 4));
-    GS_CUDA(launch_kernel_matrix(h->dS.as<double>(), h->dXsq.as<double>(), n, kernel, gamma, h->dK.as<float>(), ldk, nullptr, h->stream));
+    GS_CUDA(launch_kernel_matrix(h->dS.as<double>(), h->dXsq.as<double>(), n, ks.kernel, ks.gamma, ks.degree, ks.coef0, h->dK.as<float>(),
+                                 ldk, nullptr, nullptr, h->stream));
     std::vector<float> K((size_t)n * ldk);
     GS_CUDA(cudaMemcpyAsync(K.data(), h->dK.p, K.size() * 4, cudaMemcpyDeviceToHost, h->stream));
     GS_CUDA(cudaStreamSynchronize(h->stream));

@@ -108,6 +108,19 @@ __device__ __forceinline__ bool split_train(const SplitMasks &m, int r, int k)  
 {
     return k < 0 || ((m.tr[(size_t)r * 2 + (k >> 6)] >> (k & 63)) & 1ull);
 }
+// libsvm's poly / sigmoid kernel of a dot product s (svm.cpp Kernel::kernel_poly, kernel_sigmoid, powi), every operation
+// rounded on its own (no contraction): poly = powi(gamma*s + coef0, degree) by square-and-multiply, sigmoid = tanh(...)
+__device__ __forceinline__ double gs_kernel_of_dot(int kernel, double s, double gamma, int degree, double coef0)
+{
+    const double a = __dadd_rn(__dmul_rn(gamma, s), coef0);
+    if (kernel == GS_KERNEL_SIGMOID) return tanh(a);
+    double tmp = a, ret = 1.0;
+    for (int t = degree; t > 0; t /= 2) {
+        if (t % 2 == 1) ret = __dmul_rn(ret, tmp);
+        tmp = __dmul_rn(tmp, tmp);
+    }
+    return ret;
+}
 #endif
 
 struct gs_handle {
@@ -143,6 +156,8 @@ struct gs_handle {
     int class_w_sets = 0;
     std::vector<float> sample_w;         // gs_set_sample_weight: [n] internal order; empty = all ones
     DevBuf dSw;                          // its device copy
+    std::vector<int32_t> kp_degree;      // gs_set_kernel_params: per-candidate degree / coef0 of the next SVC call; empty = 3 / 0
+    std::vector<double> kp_coef0;
     std::vector<double> z64;             // gs_set_targets_f64: [n] float64 regression targets, internal order; empty = not set
     DevBuf dZ64;                         // their device copy
     gs_profile prof;
@@ -156,15 +171,16 @@ void gs_set_error(gs_handle *h, const std::string &msg);
 // S = X X^T in float64 from float32 X (exact products, float64 accumulation); xsq = diag(S).
 cudaError_t launch_gram_f64(const void *X, int x_dtype, int n, int d, double *S, double *xsq, cudaStream_t st);
 cudaError_t launch_widen_gram(const float *S32, int n, int64_t ld32, double *S, double *xsq, cudaStream_t st);
-// K[r][c] = (float) k(x_r, x_c) from S: rbf exp(-gamma*(xsq_r + xsq_c - 2 S_rc)) or linear S_rc.
+// K[r][c] = (float) k(x_r, x_c) from S: rbf exp(-gamma*(xsq_r + xsq_c - 2 S_rc)), linear S_rc, or libsvm's poly / sigmoid
+// of S_rc (degree and coef0 are read by those two only).  qd (may be null): [n] float64 k(x_r, x_r), rows in S's order.
 // *special (device int, pre-zeroed, may be null) is set when an entry is not a positive normal float.
-cudaError_t launch_kernel_matrix(const double *S, const double *xsq, int n, int kernel, double gamma,
-                                 float *K, int64_t ldk, int *special, cudaStream_t st);
+cudaError_t launch_kernel_matrix(const double *S, const double *xsq, int n, int kernel, double gamma, int degree, double coef0,
+                                 float *K, int64_t ldk, double *qd, int *special, cudaStream_t st);
 
 // ---- smo.cu ----
 struct SmoProblem {
     const float *K;       // float32 kernel matrix of this (kernel, gamma): [n][ldk]
-    const double *qd;     // float64 diagonal by dataset row (linear kernel) or nullptr (rbf: QD == 1)
+    const double *qd;     // float64 diagonal by dataset row (linear, poly, sigmoid) or nullptr (rbf: QD == 1)
     const int *rows;      // [l] dataset rows in sub-problem order: n_pos rows of the +1 class first
     double *alpha;        // [l] workspace: alpha by position
     double *Gbar;         // [l] workspace
@@ -215,7 +231,7 @@ cudaError_t launch_smo_colown(const SmoProblem *d_probs, const int *d_order, int
 // decision_chunks: into how many slabs the support-row range of one launch is split so that its CTAs fill the GPU in whole
 // rounds (157 row blocks on 528 resident CTAs of 132 SMs: 4 slabs = 628 CTAs = two rounds for 1.19 rounds of work; 10 slabs = 2.97).
 int decision_chunks(int n, int ncols, int sms);
-cudaError_t launch_decision(const double *S, const double *xsq, int n, int kernel, double gamma,
+cudaError_t launch_decision(const double *S, const double *xsq, int n, int kernel, double gamma, int degree, double coef0,
                             const double *coef, int ncols, double *dec, double *part, int jchunks, cudaStream_t st);
 struct VoteTask {          // one (candidate, fold) task
     int first_col;         // first decision column of this task inside its group (n_pairs consecutive)
@@ -246,6 +262,25 @@ cudaError_t launch_rss(const double *dec, const double *rho, int n, const double
 
 // ---- kernel_svm.cu: the host steps the SVC and SVR searches share (an int return is a GS_* status) ----
 int build_gram(gs_handle *h, uint32_t flags, cudaStream_t st);   // S = X X^T -> h->dS, diag(S) -> h->dXsq
+// One kernel matrix: the kernel and the parameters it reads.  Parameters a kernel ignores are stored as 0 (linear: all three,
+// rbf: degree and coef0, sigmoid: degree), so candidates that differ only in them share the matrix.
+struct KernelSpec {
+    int kernel;
+    double gamma;
+    int degree;
+    double coef0;
+    KernelSpec(int k, double g, int deg, double c0)
+        : kernel(k), gamma(k == GS_KERNEL_LINEAR ? 0.0 : g), degree(k == GS_KERNEL_POLY ? deg : 0),
+          coef0(k == GS_KERNEL_POLY || k == GS_KERNEL_SIGMOID ? c0 : 0.0) {}
+    bool has_qd() const { return kernel == GS_KERNEL_POLY || kernel == GS_KERNEL_SIGMOID; }   // a diagonal of its own
+    bool operator<(const KernelSpec &o) const
+    {
+        if (kernel != o.kernel) return kernel < o.kernel;
+        if (gamma != o.gamma) return gamma < o.gamma;
+        if (degree != o.degree) return degree < o.degree;
+        return coef0 < o.coef0;
+    }
+};
 struct SvmSearch {                                 // the state of one svc_run / svr_run call
     gs_handle *h;
     cudaStream_t st;
@@ -254,10 +289,11 @@ struct SvmSearch {                                 // the state of one svc_run /
     EvTimer tm;
     float acc[5] = {0, 0, 0, 0, 0};                // event time by phase: 0 gram, 1 kernel matrix, 2 solve, 3 score, 4 other
     cudaEvent_t ev_begin = nullptr, ev_end = nullptr;
-    std::vector<std::pair<int, double>> groups;    // (kernel, gamma) of each kernel matrix, in order of first use
+    std::vector<KernelSpec> groups;                // kernel and parameters of each kernel matrix, in order of first use
     std::vector<int> task_group;                   // task c * n_splits + k -> its group
     std::vector<std::vector<int>> group_tasks;     // group -> its tasks, ascending
     int per_batch = 0;                             // kernel matrices per batch
+    double *d_qd = nullptr;                        // per_batch float64 diagonals [n] behind them in h->dK (poly / sigmoid)
     bool fast = false;                             // this batch enqueues the branch-free SMO instance before the general one,
     const int *d_guard = nullptr;                  // with this SmoProblem::guard
     double *d_rho = nullptr;                       // outputs of the batch's problems (h->dWork[5]): rho [np], info [np][4],
@@ -268,10 +304,13 @@ struct SvmSearch {                                 // the state of one svc_run /
     std::vector<double> rho, coef;
     SvmSearch(gs_handle *h_, cudaStream_t st_) : h(h_), st(st_), n((int)h_->n), ldk(((int64_t)h_->n + 31) & ~31LL), tm(st_, h_->evp) {}
     void begin();                                  // resets h->prof but gs_set_data's ms_h2d / h2d_bytes; begin event
-    // groups the tasks by kernel matrix; rejects an rbf gamma that is not finite and > 0, with who in the message
-    int group(const char *who, int n_cand, int n_splits, const int32_t *kernel, const double *gamma);
-    int plan_batches();                            // per_batch; reserves h->dK
-    int kernel_matrices(int g0, int g1);           // group g at h->dK + (g - g0) n ldk, the guard flag, fast
+    // groups the tasks by kernel matrix; rejects an rbf gamma that is not finite and > 0, a poly / sigmoid gamma that is not
+    // finite and >= 0, with who in the message.  degree / coef0: per candidate, or null for scikit-learn's 3 / 0.
+    int group(const char *who, int n_cand, int n_splits, const int32_t *kernel, const double *gamma, const int32_t *degree,
+              const double *coef0);
+    int plan_batches();                            // per_batch; reserves h->dK (and room for the diagonals when a group has one)
+    int kernel_matrices(int g0, int g1);           // group g at h->dK + (g - g0) n ldk, its diagonal, the guard flag, fast
+    const double *qd(int g, int g0) const;         // SmoProblem::qd of group g in the batch from g0
     int workspaces(std::vector<SmoProblem> &probs);   // alpha / Gbar / scratch / coef / outputs of every problem
     int decisions(int g0, int g1, const std::vector<int> &group_first);   // group g: columns from group_first[g - g0]
     int results(int np, bool with_coef);           // downloads the batch's outputs, syncs, collects its phase times

@@ -56,19 +56,22 @@ void SvmSearch::begin()
     tm.mark(-1);
 }
 
-int SvmSearch::group(const char *who, int n_cand, int n_splits, const int32_t *kernel, const double *gamma)
+int SvmSearch::group(const char *who, int n_cand, int n_splits, const int32_t *kernel, const double *gamma,
+                     const int32_t *degree, const double *coef0)
 {
-    std::map<std::pair<int, double>, int> gmap;                      // gamma: finite and > 0, or 0.0 (linear)
+    std::map<KernelSpec, int> gmap;                                  // gamma: finite, > 0 for rbf, >= 0 for poly / sigmoid
     task_group.resize((size_t)n_cand * n_splits);
     for (int c = 0; c < n_cand; c++)
         for (int k = 0; k < n_splits; k++) {
-            const double g = kernel[c] == GS_KERNEL_RBF ? gamma[(size_t)c * n_splits + k] : 0.0;
-            if (kernel[c] == GS_KERNEL_RBF && !(g > 0 && std::isfinite(g))) {
+            const KernelSpec key(kernel[c], gamma[(size_t)c * n_splits + k], degree ? degree[c] : 3, coef0 ? coef0[c] : 0.0);
+            if (key.kernel == GS_KERNEL_RBF && !(key.gamma > 0 && std::isfinite(key.gamma))) {
                 gs_set_error(h, std::string(who) + ": gamma must be finite and > 0"); return GS_ERR_ARG;
             }
-            auto key = std::make_pair((int)kernel[c], g);
+            if (key.has_qd() && !(key.gamma >= 0 && std::isfinite(key.gamma))) {
+                gs_set_error(h, std::string(who) + ": gamma must be finite and >= 0"); return GS_ERR_ARG;
+            }
             auto it = gmap.find(key);
-            if (it == gmap.end()) { it = gmap.emplace(key, (int)groups.size()).first; groups.emplace_back(kernel[c], g); }
+            if (it == gmap.end()) { it = gmap.emplace(key, (int)groups.size()).first; groups.push_back(key); }
             task_group[(size_t)c * n_splits + k] = it->second;
         }
     group_tasks.resize(groups.size());
@@ -78,9 +81,12 @@ int SvmSearch::group(const char *who, int n_cand, int n_splits, const int32_t *k
 
 int SvmSearch::plan_batches()
 {
-    const size_t kbytes = (size_t)n * ldk * 4;
+    // a poly / sigmoid group also needs its float64 diagonal: per_batch of them follow the kernel matrices in h->dK
+    bool any_qd = false;
+    for (const KernelSpec &g : groups) any_qd = any_qd || g.has_qd();
+    const size_t kbytes = (size_t)n * ldk * 4, dbytes = any_qd ? (size_t)n * 8 : 0;
     per_batch = (int)groups.size();
-    if (h->dK.cap < kbytes * groups.size()) {
+    if (h->dK.cap < (kbytes + dbytes) * groups.size()) {
         // Ask the driver only when the buffer has to grow: cudaMemGetInfo takes anything from 0.1 to 100+ ms on a busy box
         // (it showed as outliers of this phase with the Gram already in flight), and a repeated search of the same
         // shape needs no new plan.
@@ -88,9 +94,10 @@ int SvmSearch::plan_batches()
         GS_CUDA(cudaMemGetInfo(&free_b, &total_b));
         free_b += h->dK.cap;
         const size_t budget = (size_t)(free_b * 0.6);
-        per_batch = (int)std::max<size_t>(1, std::min<size_t>(groups.size(), budget / std::max<size_t>(kbytes, 1)));
-        GS_CUDA(h->dK.reserve(kbytes * per_batch));
+        per_batch = (int)std::max<size_t>(1, std::min<size_t>(groups.size(), budget / std::max<size_t>(kbytes + dbytes, 1)));
+        GS_CUDA(h->dK.reserve((kbytes + dbytes) * per_batch));
     }
+    d_qd = any_qd ? (double *)(h->dK.as<char>() + kbytes * per_batch) : nullptr;
     return GS_OK;
 }
 
@@ -100,10 +107,12 @@ int SvmSearch::kernel_matrices(int g0, int g1)
     GS_CUDA(cudaMemsetAsync(h->dWork[7].p, 0, 4, st));
     fast = true;
     for (int g = g0; g < g1; g++) {
-        GS_CUDA(launch_kernel_matrix(h->dS.as<double>(), h->dXsq.as<double>(), n, groups[g].first, groups[g].second,
-                                     h->dK.as<float>() + (size_t)(g - g0) * n * ldk, ldk, h->dWork[7].as<int>(), st));
+        const KernelSpec &ks = groups[g];
+        GS_CUDA(launch_kernel_matrix(h->dS.as<double>(), h->dXsq.as<double>(), n, ks.kernel, ks.gamma, ks.degree, ks.coef0,
+                                     h->dK.as<float>() + (size_t)(g - g0) * n * ldk, ldk,
+                                     ks.has_qd() ? d_qd + (size_t)(g - g0) * n : nullptr, h->dWork[7].as<int>(), st));
         h->prof.launches++;
-        fast = fast && groups[g].first == GS_KERNEL_RBF;
+        fast = fast && ks.kernel == GS_KERNEL_RBF;
     }
     // The branch-free SMO instance needs rbf (QD == 1) and only positive normal floats in K.  The second condition is a
     // device flag the kernel-matrix kernels raise: both instances are enqueued and the wrong one returns at once
@@ -113,6 +122,13 @@ int SvmSearch::kernel_matrices(int g0, int g1)
     d_guard = fast ? h->dWork[7].as<int>() : nullptr;
     tm.mark(1);
     return GS_OK;
+}
+
+const double *SvmSearch::qd(int g, int g0) const
+{
+    if (groups[g].kernel == GS_KERNEL_LINEAR) return h->dXsq.as<double>();   // k(x, x) = x.x
+    if (groups[g].has_qd()) return d_qd + (size_t)(g - g0) * n;
+    return nullptr;                                                           // rbf: QD == 1
 }
 
 int SvmSearch::workspaces(std::vector<SmoProblem> &probs)
@@ -155,7 +171,8 @@ int SvmSearch::decisions(int g0, int g1, const std::vector<int> &group_first)
     if (part_doubles) GS_CUDA(h->dWork[8].reserve(part_doubles * 8));
     for (int g = g0; g < g1; g++) {
         const int c0 = group_first[g - g0], c1 = group_first[g - g0 + 1], jc = jch[g - g0];
-        GS_CUDA(launch_decision(h->dS.as<double>(), h->dXsq.as<double>(), n, groups[g].first, groups[g].second,
+        const KernelSpec &ks = groups[g];
+        GS_CUDA(launch_decision(h->dS.as<double>(), h->dXsq.as<double>(), n, ks.kernel, ks.gamma, ks.degree, ks.coef0,
                                 h->dWork[3].as<double>() + (size_t)c0 * n, c1 - c0,
                                 h->dWork[4].as<double>() + (size_t)c0 * n, jc > 1 ? h->dWork[8].as<double>() : nullptr, jc, st));
         h->prof.launches += jc > 1 ? 2 : 1;

@@ -3,10 +3,10 @@
 // libsvm predicts with float64 kernel values (svm.cpp:2821-2904 svm_predict_values calls
 // Kernel::k_function in double; the float32 rounding applies only to the training Q matrix), so the
 // decision values are NOT formed from the float32 K matrix.  They are a float64 product
-//      dec[c][r] = sum_j k64(r, j) * coef[c][j],   k64 = exp(-gamma*d2(r,j)) or S_rj
+//      dec[c][r] = sum_j k64(r, j) * coef[c][j],   k64 = exp(-gamma*d2(r,j)), S_rj, or the poly / sigmoid of S_rj
 // evaluated for ALL rows r at once (test rows give the test score, the other rows the train score)
 // and for all sub-models c that share one (kernel, gamma): one pass over the float64 Gram per gamma,
-// with the exp fused into the operand load.  coef is zero outside a sub-model's training rows.
+// with the exp (or powi / tanh) fused into the operand load.  coef is zero outside a sub-model's training rows.
 #include "common.cuh"
 #include <algorithm>
 
@@ -16,11 +16,13 @@ constexpr int TR = 64, TJ = 32;
 
 // TC = columns per block (multiple of 8, the group's column count rounded up to 8 so no lane multiplies padding).  The float64 exp of a (row, SV) pair is the expensive part (n^2 of them per
 // block row), so a block takes as many coefficient columns as the group has, up to 96 (static shared memory): the kernel values are computed once
-// per group instead of once per 32 columns.
-template <int TC>
+// per group instead of once per 32 columns.  PS: the poly / sigmoid instance (gs_kernel_of_dot in the operand load); the
+// linear / rbf instances are compiled without it, so their register use and occupancy -- and hence decision_chunks -- stay
+// those of the two-kernel build.
+template <int TC, bool PS>
 __global__ void __launch_bounds__(256)
 decision_kernel(const double *__restrict__ S, const double *__restrict__ xsq, int n, int kernel, double gamma,
-                const double *__restrict__ coef, int ncols, double *__restrict__ dec, int jlen)
+                int degree, double coef0, const double *__restrict__ coef, int ncols, double *__restrict__ dec, int jlen)
 {
     // blockIdx.z = chunk of the j (support-row) range: chunk z sums j in [z*jlen, (z+1)*jlen) into slab z of `dec`
     // (slab stride ncols*n); sum_slabs_kernel adds the slabs in ascending order.  One chunk per row block leaves one
@@ -49,7 +51,9 @@ decision_kernel(const double *__restrict__ S, const double *__restrict__ xsq, in
             double v = 0.0;
             if (r < n && jok) {
                 const double sv = S[(size_t)r * n + j];
-                if (kernel == GS_KERNEL_RBF) {
+                if (PS) {
+                    v = gs_kernel_of_dot(kernel, sv, gamma, degree, coef0);
+                } else if (kernel == GS_KERNEL_RBF) {
                     const double d2 = __dsub_rn(__dadd_rn(xsq[r], xj), __dmul_rn(2.0, sv));
                     v = exp(__dmul_rn(ng, d2));
                 } else {
@@ -288,10 +292,10 @@ static int decision_ctas_per_sm(int tc)
     const int slot = tc / 8;
     if (cache[slot] == 0) {
         int nb = 0;
-#define GS_OCC(T) case T: cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, decision_kernel<T>, 256, 0); break;
+#define GS_OCC(T) case T: cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, decision_kernel<T, false>, 256, 0); break;
         switch (tc) {
             GS_OCC(8) GS_OCC(16) GS_OCC(24) GS_OCC(32) GS_OCC(40) GS_OCC(48) GS_OCC(56) GS_OCC(64) GS_OCC(72) GS_OCC(80) GS_OCC(88)
-            default: cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, decision_kernel<96>, 256, 0); break;
+            default: cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, decision_kernel<96, false>, 256, 0); break;
         }
 #undef GS_OCC
         cache[slot] = nb > 0 ? nb : 1;
@@ -318,7 +322,7 @@ int decision_chunks(int n, int ncols, int sms)
     return best;
 }
 
-cudaError_t launch_decision(const double *S, const double *xsq, int n, int kernel, double gamma,
+cudaError_t launch_decision(const double *S, const double *xsq, int n, int kernel, double gamma, int degree, double coef0,
                             const double *coef, int ncols, double *dec, double *part, int jchunks, cudaStream_t st)
 {
     if (ncols <= 0) return cudaSuccess;
@@ -327,10 +331,12 @@ cudaError_t launch_decision(const double *S, const double *xsq, int n, int kerne
     const int jlen = ((n + jchunks - 1) / jchunks + TJ - 1) / TJ * TJ;
     dim3 grid((n + TR - 1) / TR, (ncols + tc - 1) / tc, jchunks);
     double *out = jchunks > 1 ? part : dec;
-#define GS_DEC(T) case T: decision_kernel<T><<<grid, 256, 0, st>>>(S, xsq, n, kernel, gamma, coef, ncols, out, jlen); break;
+    const bool ps = kernel == GS_KERNEL_POLY || kernel == GS_KERNEL_SIGMOID;
+#define GS_DEC(T) case T: if (ps) decision_kernel<T, true><<<grid, 256, 0, st>>>(S, xsq, n, kernel, gamma, degree, coef0, coef, ncols, out, jlen); \
+                          else decision_kernel<T, false><<<grid, 256, 0, st>>>(S, xsq, n, kernel, gamma, degree, coef0, coef, ncols, out, jlen); break;
     switch (tc) {
         GS_DEC(8) GS_DEC(16) GS_DEC(24) GS_DEC(32) GS_DEC(40) GS_DEC(48) GS_DEC(56) GS_DEC(64) GS_DEC(72) GS_DEC(80) GS_DEC(88)
-        default: decision_kernel<96><<<grid, 256, 0, st>>>(S, xsq, n, kernel, gamma, coef, ncols, out, jlen); break;
+        default: GS_DEC(96)
     }
 #undef GS_DEC
     if (jchunks > 1) {

@@ -119,7 +119,7 @@ static int svr_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
         lmax = std::max(lmax, 2 * l);
     }
     sp_off[n_splits] = (int)rows_all.size();
-    if (const int rc = search.group("gs_svr", n_cand, n_splits, kernel, gamma)) return rc;   // groups by kernel matrix (kernel, gamma)
+    if (const int rc = search.group("gs_svr", n_cand, n_splits, kernel, gamma, nullptr, nullptr)) return rc;   // groups by kernel matrix (kernel, gamma)
 
     // ---- per-split sizes and r2 denominators (they depend on the split only) ----
     std::vector<double> tss((size_t)n_splits * 2, 0.0), cnt((size_t)n_splits * 2, 0.0);
@@ -180,7 +180,7 @@ static int svr_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
                 SmoProblem P;
                 memset(&P, 0, sizeof P);
                 P.K = h->dK.as<float>() + (size_t)(g - g0) * n * ldk;
-                P.qd = search.groups[g].first == GS_KERNEL_LINEAR ? h->dXsq.as<double>() : nullptr;
+                P.qd = search.qd(g, g0);
                 P.rows = d_rows + sp_off[k];
                 P.l = sp_off[k + 1] - sp_off[k];
                 P.n_pos = P.l / 2;

@@ -12,7 +12,8 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libb200gs.so")
 
 GS_RETURN_TRAIN, GS_GRAM_TENSOR, GS_NO_SHRINKING = 1, 2, 4
-KERNEL_ID = {"linear": 0, "rbf": 1}
+KERNEL_ID = {"linear": 0, "rbf": 1, "poly": 2, "sigmoid": 3}
+_PARAM_KERNELS = (2, 3)            # the kernels that read degree / coef0 (gs_set_kernel_params)
 
 _lib = None
 
@@ -50,6 +51,8 @@ def load_library():
     L.gs_set_splits.restype = c.c_int
     L.gs_set_class_weight.argtypes = [vp, vp, i32]
     L.gs_set_class_weight.restype = c.c_int
+    L.gs_set_kernel_params.argtypes = [vp, vp, vp, i32]
+    L.gs_set_kernel_params.restype = c.c_int
     L.gs_set_sample_weight.argtypes = [vp, vp]
     L.gs_set_sample_weight.restype = c.c_int
     L.gs_set_scoring.argtypes = [vp, i32, i32]
@@ -195,17 +198,35 @@ class Engine:
             out["train"] = None
         return out
 
-    def svc(self, kernel, C, gamma, tol=1e-3, max_iter=-1, shrinking=True, return_train=True, flags=0):
-        return self._kernel_svm(self._L.gs_svc, kernel, C, [], gamma, tol, max_iter, shrinking, return_train, flags)
+    def _with_kernel_params(self, kernel_ids, degree, coef0, call):
+        """call() with gs_set_kernel_params set to degree / coef0 (scalars or one per candidate) when a poly or sigmoid
+        candidate is present, reset afterwards; a call without one sets nothing"""
+        if not any(k in _PARAM_KERNELS for k in kernel_ids):
+            return call()
+        n = len(kernel_ids)
+        deg = np.ascontiguousarray(np.broadcast_to(np.asarray(3 if degree is None else degree, np.int64), (n,)), np.int32)
+        c0 = np.ascontiguousarray(np.broadcast_to(np.asarray(0.0 if coef0 is None else coef0, np.float64), (n,)))
+        self._check(self._L.gs_set_kernel_params(self._h, _ptr(deg), _ptr(c0), n))
+        try:
+            return call()
+        finally:
+            self._L.gs_set_kernel_params(self._h, None, None, 0)
 
-    def svc_refit(self, kernel, C, gamma, n_classes, tol=1e-3, max_iter=-1, shrinking=True):
+    def svc(self, kernel, C, gamma, tol=1e-3, max_iter=-1, shrinking=True, return_train=True, flags=0, degree=None, coef0=None):
+        """degree / coef0: scalars or one per candidate, read by the poly and sigmoid candidates (defaults 3 / 0.0)"""
+        ids = [KERNEL_ID[k] if isinstance(k, str) else int(k) for k in kernel]
+        return self._with_kernel_params(ids, degree, coef0, lambda: self._kernel_svm(
+            self._L.gs_svc, ids, C, [], gamma, tol, max_iter, shrinking, return_train, flags))
+
+    def svc_refit(self, kernel, C, gamma, n_classes, tol=1e-3, max_iter=-1, shrinking=True, degree=3, coef0=0.0):
         n_pairs = n_classes * (n_classes - 1) // 2
         coef = np.zeros((n_pairs, self.n))
         rho = np.zeros(n_pairs)
         it = np.zeros(n_pairs, np.int32)
         k = KERNEL_ID[kernel] if isinstance(kernel, str) else int(kernel)
-        self._check(self._L.gs_svc_refit(self._h, k, float(C), float(gamma), float(tol), int(max_iter),
-                                         0 if shrinking else GS_NO_SHRINKING, _ptr(coef), _ptr(rho), _ptr(it)))
+        self._with_kernel_params([k], degree, coef0, lambda: self._check(self._L.gs_svc_refit(
+            self._h, k, float(C), float(gamma), float(tol), int(max_iter), 0 if shrinking else GS_NO_SHRINKING, _ptr(coef),
+            _ptr(rho), _ptr(it))))
         return coef, rho, it
 
     def set_targets_f64(self, y):
@@ -298,10 +319,11 @@ class Engine:
         self._check(self._L.gs_debug_gram(self._h, _ptr(S), _ptr(xsq)))
         return S, xsq
 
-    def debug_kernel_matrix(self, kernel, gamma):
+    def debug_kernel_matrix(self, kernel, gamma, degree=3, coef0=0.0):
         K = np.zeros((self.n, self.n), np.float32)
         k = KERNEL_ID[kernel] if isinstance(kernel, str) else int(kernel)
-        self._check(self._L.gs_debug_kernel_matrix(self._h, k, float(gamma), _ptr(K)))
+        self._with_kernel_params([k], degree, coef0,
+                                 lambda: self._check(self._L.gs_debug_kernel_matrix(self._h, k, float(gamma), _ptr(K))))
         return K
 
     def debug_gemm_nt(self, A, B):

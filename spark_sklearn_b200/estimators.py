@@ -2,7 +2,8 @@
 and turn refit buffers back into genuine fitted scikit-learn estimators for ``best_estimator_``
 (reference base_search.py:165-174 delegates ``predict`` & co. to it).
 
-Only estimators with a CUDA path are accepted (SVC and SVR rbf/linear, Ridge, LogisticRegression -- the
+Only estimators with a CUDA path are accepted (SVC with the linear, rbf, poly and sigmoid kernels, SVR rbf/linear, Ridge,
+LogisticRegression -- the
 families the reference ships examples for); anything else raises: no CPU fallback.
 """
 import numbers
@@ -293,12 +294,19 @@ class _KernelGamma:
         return float(g)
 
     def affinity(self):
-        """Candidates with the same (kernel, gamma) share a kernel matrix and a decision-value pass."""
+        """Candidates with the same kernel matrix -- (kernel, gamma), plus coef0 for sigmoid and degree and coef0 for poly --
+        share it and a decision-value pass."""
         try:
             out = []
             for cand in self.cands:
                 p = self._base_params(cand)
-                out.append((p["kernel"], self._gamma(p["gamma"], -1) if p["kernel"] == "rbf" else 0.0))
+                kern = p["kernel"]
+                key = (kern, self._gamma(p["gamma"], -1) if kern != "linear" else 0.0)
+                if kern == "poly":
+                    key += (int(p["degree"]), float(p["coef0"]))
+                elif kern == "sigmoid":
+                    key += (float(p["coef0"]),)
+                out.append(key)
             return out
         except Exception:
             return None
@@ -310,7 +318,8 @@ class _KernelGamma:
 
 
 class SVCPlan(_KernelGamma, _Plan):
-    """sklearn.svm.SVC (C-SVC).  Scalars per candidate: kernel, C, gamma (resolved per fold)."""
+    """sklearn.svm.SVC (C-SVC).  Scalars per candidate: kernel, C, gamma (resolved per fold for every kernel but linear),
+    degree and coef0 (poly, sigmoid)."""
     scorers = CLASSIFICATION_SCORERS
     # what one more (kernel, gamma) group costs a GPU, in the units of costs() (thousands of SMO iterations of one candidate's
     # folds): a kernel matrix + a float64 decision-value pass, against the SMO time of one unit (ratio calibrated on a 148-SM GPU)
@@ -327,8 +336,15 @@ class SVCPlan(_KernelGamma, _Plan):
         self._var_cache = {}
 
     def _check(self, p):
-        if p["kernel"] not in ("rbf", "linear"):
-            raise NotImplementedError("SVC kernel=%r has no CUDA path (rbf and linear do)" % (p["kernel"],))
+        if p["kernel"] not in ("rbf", "linear", "poly", "sigmoid"):
+            raise NotImplementedError("SVC kernel=%r has no CUDA path (linear, rbf, poly and sigmoid do)" % (p["kernel"],))
+        # scikit-learn's parameter constraints (SVC._parameter_constraints), checked whatever the kernel
+        if not (isinstance(p["degree"], numbers.Integral) and p["degree"] >= 0):
+            raise ValueError("The 'degree' parameter of SVC must be an int in the range [0, inf); got %r" % (p["degree"],))
+        if not isinstance(p["coef0"], numbers.Real):
+            raise ValueError("The 'coef0' parameter of SVC must be a float; got %r" % (p["coef0"],))
+        if p["degree"] > np.iinfo(np.int32).max:
+            raise NotImplementedError("SVC degree=%r: the CUDA path takes a 32-bit degree" % (p["degree"],))
         if p.get("probability") not in (False, "deprecated", None):
             raise NotImplementedError("SVC probability=True is not supported by the CUDA path")
         if p.get("break_ties"):
@@ -371,11 +387,12 @@ class SVCPlan(_KernelGamma, _Plan):
             self._set_class_weight(params[idx[0]].get("class_weight"))
             kern = [params[j]["kernel"] for j in idx]
             C = [float(params[j]["C"]) for j in idx]
-            gam = np.array([[self._gamma(params[j]["gamma"], k) if params[j]["kernel"] == "rbf" else 0.0
+            gam = np.array([[self._gamma(params[j]["gamma"], k) if params[j]["kernel"] != "linear" else 0.0
                              for k in range(ns)] for j in idx])
             self.engine.set_scoring(self.score_kind, self.score_pos)
             r = self.engine.svc(kern, C, gam, tol=tol, max_iter=max_iter, shrinking=shrinking,
-                                return_train=return_train, flags=self._flags())
+                                return_train=return_train, flags=self._flags(),
+                                degree=[int(params[j]["degree"]) for j in idx], coef0=[float(params[j]["coef0"]) for j in idx])
             for key in ("test", "fit_ms", "score_ms", "n_iter"):
                 res[key][idx] = r[key]
             if return_train:
@@ -392,9 +409,9 @@ class SVCPlan(_KernelGamma, _Plan):
         self._check(p)
         gamma = self._gamma(p["gamma"], -1)          # all rows train (svm/_base.py:278-286)
         cw_ = self._set_class_weight(p.get("class_weight"), refit=True)
-        coef, rho, n_iter = self.engine.svc_refit(p["kernel"], p["C"], gamma if p["kernel"] == "rbf" else 0.0,
+        coef, rho, n_iter = self.engine.svc_refit(p["kernel"], p["C"], gamma if p["kernel"] != "linear" else 0.0,
                                                   len(self.classes), tol=p["tol"], max_iter=p["max_iter"],
-                                                  shrinking=p["shrinking"])
+                                                  shrinking=p["shrinking"], degree=int(p["degree"]), coef0=float(p["coef0"]))
         self.engine.set_class_weight(None)
         est = clone(self.estimator).set_params(**best_params)
         est = materialize_svc(est, self.X, self.y_class, self.classes, coef, rho, n_iter, gamma)

@@ -84,6 +84,17 @@ def _svr(n=1000, d=32, grid=None, cv=5, name="svr_small"):
                 param_grid=grid, cv=cv, search="grid")
 
 
+def _svc_kernels(n=3000, d=128, cv=5, name="svc_kernels_mid"):
+    """SVC over the poly and sigmoid kernels (with a few rbf and linear candidates) on the config-2 data recipe: the
+    list-of-dicts grid shape of the reference's own cv_results_ example (grid_search.py:120-160)."""
+    X, y = _svc_data(n, d)
+    grid = [{"kernel": ["poly"], "degree": [2, 3], "coef0": [0.0, 1.0], "C": [0.1, 1.0, 10.0]},
+            {"kernel": ["sigmoid"], "gamma": [1.0 / 1024, "scale"], "coef0": [-1.0, 0.0], "C": [0.1, 1.0, 10.0]},
+            {"kernel": ["rbf"], "gamma": [1.0 / 512], "C": [1.0, 10.0]},
+            {"kernel": ["linear"], "C": [0.01]}]
+    return dict(name=name, X=X, y=y, estimator="SVC", est_params={}, param_grid=grid, cv=cv, search="grid")
+
+
 WORKLOADS = {
     "c1": _c1, "c2": _c2, "c3": _c3, "c4": _c4, "c5": _c5,
     # reduced-size variants: same recipes, sizes the CPU oracle finishes in seconds
@@ -101,6 +112,9 @@ WORKLOADS = {
                                                  "epsilon": [0.1]}, name="svr_mid"),
     "svr_c6": lambda: _svr(n=10000, d=512, grid={"C": np.logspace(-1, 2.5, 8), "gamma": np.geomspace(1.0 / 4096, 1.0 / 256, 8),
                                                  "epsilon": [0.1]}, name="svr_c6"),
+    # SVC poly / sigmoid: the golden-sized grid and the same grid on config-2 data (tools/bench_kernels.py)
+    "svc_kernels_mid": _svc_kernels,
+    "svc_kernels_c2": lambda: _svc_kernels(n=10000, d=512, name="svc_kernels_c2"),
 }
 
 
