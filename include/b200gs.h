@@ -205,6 +205,26 @@ int gs_svr(gs_handle *h, int32_t n_cand, const int32_t *kernel, const double *C,
 int gs_svr_refit(gs_handle *h, int32_t kernel, double C, double epsilon, double gamma, double tol, int32_t max_iter,
                  uint32_t flags, double *coef, double *rho, int32_t *n_iter);
 
+/*
+ * LinearSVC (penalty='l2', loss='squared_hinge', primal: replaces LinearSVC.fit/score = sklearn liblinear linear.cpp train /
+ * train_one with L2R_L2LOSS_SVC, l2r_l2_svc_fun and tron.cpp TRON, the trust-region Newton method with conjugate gradients).
+ * C[n_cand]; tol / max_iter as LinearSVC's.  fit_intercept != 0: every row gets the regularised feature intercept_scaling
+ * (> 0, scikit-learn's bias).  Two classes: one fit per (candidate, split), class 0 = -1.  Three or more: one-vs-rest, one fit
+ * per class, whose negative rows get the unweighted C (linear.cpp train).  Class weights: gs_set_class_weight (one set per
+ * split or one for all); sample weights: gs_set_sample_weight, float64, a row with weight 0 leaves the fit.  Splits: fold ids
+ * or gs_set_splits masks.  Each fit follows liblinear's iterate in float64 (X is widened exactly; the products run on the
+ * FP64 tensor cores).  Scores: accuracy or gs_set_scoring's scorer from the float64 decision values (binary: > 0 ->
+ * class 1; one-vs-rest: first arg-max).  n_iter: [n_cand][n_splits], TRON iterations, the maximum over the one-vs-rest
+ * fits (LinearSVC.n_iter_).  Every class needs a row of positive weight in every training set (GS_ERR_UNSUPPORTED).
+ * gs_linsvc_refit: all rows; coef_out [rows][d + 1] = liblinear's raw weights (features, then the weight of the bias
+ * feature: intercept_ = intercept_scaling x that; 0 without an intercept), rows = 1 (binary) or n_classes; n_iter [rows].
+ */
+int gs_linsvc(gs_handle *h, int32_t n_cand, const double *C, double tol, int32_t max_iter, int32_t fit_intercept,
+              double intercept_scaling, uint32_t flags, double *test_scores, double *train_scores, int32_t *n_iter,
+              float *fit_ms, float *score_ms);
+int gs_linsvc_refit(gs_handle *h, double C, double tol, int32_t max_iter, int32_t fit_intercept, double intercept_scaling,
+                    double *coef_out, int32_t *n_iter);
+
 /* ---- test hooks (used by tests/ to localise a parity failure to one kernel) ---------------- */
 /* S_out [n][n] float64 Gram X X^T and xsq_out [n] (either may be NULL), in ORIGINAL row order.  */
 int gs_debug_gram(gs_handle *h, double *S_out, double *xsq_out);
@@ -214,6 +234,9 @@ int gs_debug_kernel_matrix(gs_handle *h, int32_t kernel, double gamma, float *K_
 
 /* C[M][N] = sum_k A[M][k]*B[N][k] on the wgmma tensor-core path (3xTF32 split), host fp32 row-major in/out. */
 int gs_debug_gemm_nt(gs_handle *h, const float *A, int32_t M, const float *B, int32_t N, int32_t K, float *C);
+/* C[M][N] = sum_k A[M][k]*B[N][k] on the FP64 tensor-core path of gs_linsvc (K > 1024: split-K with the fixed-order sum of
+ * the partials), host float64 row-major in/out. */
+int gs_debug_gemm_f64(gs_handle *h, const double *A, int32_t M, const double *B, int32_t N, int32_t K, double *C);
 
 /* ---- planning helpers (host only, no device work; used by gs_svc itself and by the multi-GPU host driver) -------- */
 /* Predicted SMO iterations (thousands, for ~8000 training rows) of one C-SVC sub-problem: the model that orders the

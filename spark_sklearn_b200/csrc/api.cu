@@ -79,7 +79,7 @@ __global__ void gather_rows_kernel(const T *__restrict__ src, const int *__restr
 
 extern "C" {
 
-int gs_version(void) { return 101; }
+int gs_version(void) { return 102; }
 
 int gs_set_class_weight(gs_handle *h, const double *w, int32_t n_sets)
 {
@@ -112,16 +112,19 @@ int gs_set_sample_weight(gs_handle *h, const double *w)
     if (!w) { h->sample_w.clear(); return GS_OK; }
     if (h->n == 0) { gs_set_error(h, "gs_set_sample_weight: no dataset (call gs_set_data first)"); return GS_ERR_NO_DATA; }
     std::vector<float> sw((size_t)h->n);
+    std::vector<double> sw64((size_t)h->n);
     for (int64_t i = 0; i < h->n; i++) {
         const double v = w[h->perm[i]];
         if (!(v >= 0) || !std::isfinite(v)) { gs_set_error(h, "gs_set_sample_weight: weights must be finite and >= 0"); return GS_ERR_ARG; }
         sw[i] = (float)v;                                     // scikit-learn: _check_sample_weight(..., dtype=X.dtype)
+        sw64[i] = v;                                          // LinearSVC: _check_sample_weight(..., dtype=np.float64)
     }
     GS_CUDA(cudaSetDevice(h->device));
     GS_CUDA(h->dSw.reserve((size_t)h->n * 4));
     GS_CUDA(cudaMemcpyAsync(h->dSw.p, sw.data(), (size_t)h->n * 4, cudaMemcpyHostToDevice, h->stream));
     GS_CUDA(cudaStreamSynchronize(h->stream));
     h->sample_w.swap(sw);
+    h->sample_w64.swap(sw64);
     return GS_OK;
 }
 

@@ -155,6 +155,7 @@ struct gs_handle {
     std::vector<double> class_w;         // gs_set_class_weight: [sets][n_classes]; empty = all ones
     int class_w_sets = 0;
     std::vector<float> sample_w;         // gs_set_sample_weight: [n] internal order; empty = all ones
+    std::vector<double> sample_w64;      // the same weights in float64 (gs_linsvc; valid while sample_w is not empty)
     DevBuf dSw;                          // its device copy
     std::vector<int32_t> kp_degree;      // gs_set_kernel_params: per-candidate degree / coef0 of the next SVC call; empty = 3 / 0
     std::vector<double> kp_coef0;
@@ -334,3 +335,11 @@ cudaError_t launch_sum_partials(const float *partial, int n_chunks, int64_t per,
 cudaError_t launch_gemm_nt_tf32x3(const TcMap &a_hi, const TcMap &a_lo, const TcMap &b_hi, const TcMap &b_lo,
                                   const TcBatch *d_batches, int n_batches, int M, int N, float alpha, bool accumulate,
                                   cudaStream_t st, bool symmetric = false);
+
+// ---- gemm_f64.cu: FP64 tensor-core (DMMA) contraction  C[M][N] = sum_k A[M][k] B[N][k], float64 throughout ----
+// M, N multiples of 64; K and kchunk multiples of 16; every row read (A rows < M, B rows < N, k < K) must exist.
+// Split-K: chunk z of [z*kchunk, min(K, (z+1)*kchunk)) writes C + z*c_chunk_stride.
+cudaError_t launch_gemm_nt_f64(const double *A, int64_t lda, const double *B, int64_t ldb, double *C, int64_t ldc, int M, int N,
+                               int K, int kchunk, int64_t c_chunk_stride, cudaStream_t st);
+// out[i] = sum over q = 0, 1, ... of partial[q * per + i], in that order (out == partial is allowed)
+cudaError_t launch_sum_partials_f64(const double *partial, int n_chunks, int64_t per, double *out, cudaStream_t st);

@@ -74,6 +74,9 @@ def load_library():
     L.gs_svr_refit.argtypes = [vp, i32, dbl, dbl, dbl, dbl, i32, u32, vp, vp, vp]
     L.gs_logreg.argtypes = [vp, i32, vp, dbl, i32, i32, u32, vp, vp, vp, vp, vp]
     L.gs_logreg_refit.argtypes = [vp, dbl, dbl, i32, i32, vp, vp]
+    L.gs_linsvc.argtypes = [vp, i32, vp, dbl, i32, i32, dbl, u32, vp, vp, vp, vp, vp]
+    L.gs_linsvc_refit.argtypes = [vp, dbl, dbl, i32, i32, dbl, vp, vp]
+    L.gs_debug_gemm_f64.argtypes = [vp, vp, i32, vp, i32, i32, vp]
     L.gs_get_profile.argtypes = [vp, c.POINTER(GsProfile)]
     L.gs_debug_gram.argtypes = [vp, vp, vp]
     L.gs_debug_kernel_matrix.argtypes = [vp, i32, dbl, vp]
@@ -88,7 +91,8 @@ def load_library():
     L.gs_svc_simulate.restype = dbl
     for f in ("gs_create", "gs_set_data", "gs_svc", "gs_svc_refit", "gs_ridge", "gs_ridge_refit", "gs_enet", "gs_enet_refit", "gs_set_targets_f64",
               "gs_svr", "gs_svr_refit", "gs_logreg",
-              "gs_logreg_refit", "gs_get_profile", "gs_debug_gram", "gs_debug_kernel_matrix", "gs_debug_gemm_nt"):
+              "gs_logreg_refit", "gs_linsvc", "gs_linsvc_refit", "gs_get_profile", "gs_debug_gram", "gs_debug_kernel_matrix",
+              "gs_debug_gemm_nt", "gs_debug_gemm_f64"):
         getattr(L, f).restype = c.c_int
     _lib = L
     return L
@@ -312,6 +316,28 @@ class Engine:
             return coef[0, :-1].copy(), float(coef[0, -1]), int(it[0])
         return coef[:, :-1].copy(), coef[:, -1].copy(), int(it[0])
 
+    def linsvc(self, C, tol=1e-4, max_iter=1000, fit_intercept=True, intercept_scaling=1.0, return_train=True):
+        """LinearSVC (squared hinge, L2, primal TRON) per (candidate, split); n_iter = LinearSVC.n_iter_ of each fit"""
+        C = np.ascontiguousarray(C, np.float64)
+        shape = (len(C), self.n_splits)
+        out = dict(test=np.zeros(shape), train=np.zeros(shape), n_iter=np.zeros(shape, np.int32),
+                   fit_ms=np.zeros(shape, np.float32), score_ms=np.zeros(shape, np.float32))
+        self._check(self._L.gs_linsvc(self._h, len(C), _ptr(C), float(tol), int(max_iter), int(bool(fit_intercept)),
+                                      float(intercept_scaling), GS_RETURN_TRAIN if return_train else 0, _ptr(out["test"]),
+                                      _ptr(out["train"]), _ptr(out["n_iter"]), _ptr(out["fit_ms"]), _ptr(out["score_ms"])))
+        if not return_train:
+            out["train"] = None
+        return out
+
+    def linsvc_refit(self, C, tol=1e-4, max_iter=1000, fit_intercept=True, intercept_scaling=1.0):
+        """-> (raw [rows][d + 1]: liblinear's weights, the bias feature's last; n_iter [rows]); rows = 1 (binary) or n_classes"""
+        rows = self.n_classes if self.n_classes > 2 else 1
+        raw = np.zeros((rows, self.d + 1))
+        it = np.zeros(rows, np.int32)
+        self._check(self._L.gs_linsvc_refit(self._h, float(C), float(tol), int(max_iter), int(bool(fit_intercept)),
+                                            float(intercept_scaling), _ptr(raw), _ptr(it)))
+        return raw, it
+
     # -- test hooks --
     def debug_gram(self):
         S = np.zeros((self.n, self.n))
@@ -331,6 +357,13 @@ class Engine:
         B = np.ascontiguousarray(B, np.float32)
         C = np.zeros((A.shape[0], B.shape[0]), np.float32)
         self._check(self._L.gs_debug_gemm_nt(self._h, _ptr(A), A.shape[0], _ptr(B), B.shape[0], A.shape[1], _ptr(C)))
+        return C
+
+    def debug_gemm_f64(self, A, B):
+        A = np.ascontiguousarray(A, np.float64)
+        B = np.ascontiguousarray(B, np.float64)
+        C = np.zeros((A.shape[0], B.shape[0]))
+        self._check(self._L.gs_debug_gemm_f64(self._h, _ptr(A), A.shape[0], _ptr(B), B.shape[0], A.shape[1], _ptr(C)))
         return C
 
     def profile(self):

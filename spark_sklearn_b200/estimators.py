@@ -3,8 +3,8 @@ and turn refit buffers back into genuine fitted scikit-learn estimators for ``be
 (reference base_search.py:165-174 delegates ``predict`` & co. to it).
 
 Only estimators with a CUDA path are accepted (SVC with the linear, rbf, poly and sigmoid kernels, SVR rbf/linear, Ridge,
-LogisticRegression -- the
-families the reference ships examples for); anything else raises: no CPU fallback.
+Lasso / ElasticNet, LogisticRegression, LinearSVC with the primal squared-hinge solver -- the families the reference ships
+examples for); anything else raises: no CPU fallback.
 """
 import numbers
 import warnings
@@ -95,7 +95,7 @@ class Folds:
 def adapter_for(estimator):
     from sklearn.linear_model import ElasticNet, Lasso, LogisticRegression, Ridge
     from sklearn.pipeline import Pipeline
-    from sklearn.svm import SVC, SVR
+    from sklearn.svm import SVC, SVR, LinearSVC
     t = type(estimator)
     if t is SVC:
         return SVCAdapter
@@ -107,13 +107,15 @@ def adapter_for(estimator):
         return LogRegAdapter
     if t in (Lasso, ElasticNet):
         return ENetAdapter
+    if t is LinearSVC:
+        return LinearSVCAdapter
     if t is Pipeline and len(estimator.steps) == 1:
         # the reference's own search tests wrap the estimator in a one-step Pipeline and search 'step__param'
         # (python/spark_sklearn/tests/test_search_2.py:69-93): the step's adapter runs, the names are translated
         return PipelineAdapter(estimator.steps[0][0], adapter_for(estimator.steps[0][1]))
     raise NotImplementedError(
-        "spark_sklearn_b200 has CUDA paths for SVC, SVR, Ridge, Lasso, ElasticNet and LogisticRegression (bare or as the only "
-        "step of a Pipeline); got %s (no CPU fallback)" % t.__name__)
+        "spark_sklearn_b200 has CUDA paths for SVC, SVR, Ridge, Lasso, ElasticNet, LogisticRegression and LinearSVC (bare or as "
+        "the only step of a Pipeline); got %s (no CPU fallback)" % t.__name__)
 
 
 def _as_matrix(X):
@@ -864,3 +866,115 @@ class LogRegPlan(_Plan):
         est.n_iter_ = np.array([it], np.int32)
         est.n_features_in_ = self.X.shape[1]
         return est
+
+
+# ------------------------------------------------------------------ LinearSVC -----------------
+class LinearSVCAdapter:
+    multi_device = True        # plan(..., device=d): one plan per GPU of the in-process scheduler
+    scorers = CLASSIFICATION_SCORERS
+
+    @staticmethod
+    def plan(estimator, cands, X, y, fold_id, n_splits, device=None):
+        return LinearSVCPlan(estimator, cands, X, y, fold_id, n_splits, device)
+
+
+class LinearSVCPlan(_Plan):
+    """sklearn.svm.LinearSVC with liblinear's primal solver (L2R_L2LOSS_SVC: TRON, csrc/linsvc.cu).  X reaches the device in
+    float32 or float64 and is widened exactly, as scikit-learn's fit converts it to float64.  Every fit resolves dual='auto'
+    from its own training set, as LinearSVC.fit does; a fit that resolves to the dual solver has no CUDA path."""
+    scorers = CLASSIFICATION_SCORERS
+    supports_sample_weight = True
+
+    def __init__(self, estimator, cands, X, y, fold_id, n_splits, device=None):
+        super().__init__(estimator, cands, X, y, fold_id, n_splits, device)
+        if y is None:
+            raise ValueError("LinearSVC needs y")
+        self.classes, self.y_class = np.unique(np.asarray(y), return_inverse=True)
+        if len(self.classes) < 2:
+            raise ValueError("This solver needs samples of at least 2 classes in the data, but the data contains only one "
+                             "class: %r" % (self.classes[0],))
+        if len(self.classes) > 64:
+            raise NotImplementedError("LinearSVC CUDA path handles up to 64 classes (got %d)" % len(self.classes))
+        self._set_data(self.X, y_class=self.y_class.astype(np.int32))
+
+    def _check(self, p, n_rows):
+        """scikit-learn's own checks in LinearSVC.fit's order (parameter constraints, dual resolution on a training set of
+        n_rows rows, the liblinear solver of the combination: ValueError), then the combinations without a CUDA path"""
+        from sklearn.svm import LinearSVC
+        from sklearn.svm._base import _get_liblinear_solver_type
+        from sklearn.svm._classes import _validate_dual_parameter
+        LinearSVC(**p)._validate_params()
+        dual = _validate_dual_parameter(p["dual"], p["loss"], p["penalty"], p["multi_class"],
+                                        np.empty((n_rows, self.X.shape[1]), np.bool_))
+        if p["multi_class"] == "crammer_singer":
+            raise NotImplementedError("LinearSVC multi_class='crammer_singer' has no CUDA path (one-vs-rest does)")
+        _get_liblinear_solver_type(p["multi_class"], p["penalty"], p["loss"], dual)
+        if dual:
+            raise NotImplementedError(
+                "LinearSVC fit on %d rows x %d features resolves to the dual solver (dual=%r), which has no CUDA path (the "
+                "primal solver, dual=False with at least as many rows as features, does)" % (n_rows, self.X.shape[1], p["dual"]))
+        if p["penalty"] != "l2":
+            raise NotImplementedError("LinearSVC penalty=%r has no CUDA path (l2 does)" % (p["penalty"],))
+
+    def _params(self, cand, ks):
+        p = self._base_params(cand)
+        for k in ks:
+            self._check(p, int(np.count_nonzero(self._train_rows(k))))
+        return p
+
+    def evaluate(self, my, return_train=True, error_score='raise'):
+        shape = (len(my), self.n_splits)
+        res = dict(test=np.zeros(shape), train=np.zeros(shape), fit_ms=np.zeros(shape), score_ms=np.zeros(shape),
+                   n_iter=np.zeros(shape, np.int64))
+        groups = {}
+        for j, ci in enumerate(my):
+            p = self._params(self.cands[ci], range(self.n_splits))
+            cw = p.get("class_weight")
+            cwk = None if cw is None else (cw if isinstance(cw, str) else tuple(sorted(cw.items())))
+            key = (float(p["tol"]), int(p["max_iter"]), bool(p["fit_intercept"]), float(p["intercept_scaling"]), cwk)
+            groups.setdefault(key, []).append((j, float(p["C"]), cw))
+        prof = {}
+        for (tol, mi, fi, isc, _cwk), items in groups.items():
+            idx = [j for j, _, _ in items]
+            self._set_class_weight(items[0][2])
+            self.engine.set_scoring(self.score_kind, self.score_pos)
+            r = self.engine.linsvc([c for _, c, _ in items], tol=tol, max_iter=mi, fit_intercept=fi, intercept_scaling=isc,
+                                   return_train=return_train)
+            for key in ("test", "fit_ms", "score_ms", "n_iter"):
+                res[key][idx] = r[key]
+            if return_train:
+                res["train"][idx] = r["train"]
+            for k, v in self.engine.profile().items():
+                prof[k] = prof.get(k, 0) + v
+        self.engine.set_class_weight(None)
+        self._prof = prof
+        self.n_iter_ = res["n_iter"]
+        return self._finish(res, return_train, error_score, len(my))
+
+    def refit(self, best_params):
+        p = self._params(best_params, [-1])
+        self._set_class_weight(p.get("class_weight"), refit=True)
+        raw, n_iter = self.engine.linsvc_refit(p["C"], p["tol"], p["max_iter"], p["fit_intercept"], p["intercept_scaling"])
+        self.engine.set_class_weight(None)
+        est = clone(self.estimator).set_params(**best_params)
+        return materialize_linsvc(est, self.classes, raw, n_iter, self.X.shape[1])
+
+
+def materialize_linsvc(est, classes, raw, n_iter, n_features):
+    """Fill a (cloned, parametrised) sklearn.svm.LinearSVC with the fitted state of liblinear's raw weights raw
+    [rows][n_features + 1] (the bias feature's weight last) and the per-fit iteration counts (svm/_base.py:1296-1310
+    _fit_liblinear, svm/_classes.py:330-351 LinearSVC.fit), with scikit-learn's ConvergenceWarning."""
+    raw = np.asarray(raw, np.float64)
+    est.classes_ = np.asarray(classes)
+    if est.fit_intercept:
+        est.coef_ = raw[:, :n_features].copy()
+        est.intercept_ = est.intercept_scaling * raw[:, n_features]
+    else:
+        est.coef_ = raw[:, :n_features].copy()
+        est.intercept_ = 0.0
+    est.n_iter_ = int(np.max(n_iter))
+    est.n_features_in_ = int(n_features)
+    if est.n_iter_ >= est.max_iter:
+        from sklearn.exceptions import ConvergenceWarning
+        warnings.warn("Liblinear failed to converge, increase the number of iterations.", ConvergenceWarning)
+    return est

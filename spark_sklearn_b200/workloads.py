@@ -95,6 +95,27 @@ def _svc_kernels(n=3000, d=128, cv=5, name="svc_kernels_mid"):
     return dict(name=name, X=X, y=y, estimator="SVC", est_params={}, param_grid=grid, cv=cv, search="grid")
 
 
+def _linsvc(which="small"):
+    """LinearSVC (primal TRON): the config-3 data with 8 C values (small), a 3-class set (multi), and config 3's own
+    search shape on its data (c3: 256 random C candidates x 5 folds = 1280 fits of 40000 x 256, all primal)."""
+    from scipy.stats import loguniform
+    if which == "multi":
+        from sklearn.datasets import make_classification
+        from sklearn.preprocessing import StandardScaler
+        X, y = make_classification(n_samples=3000, n_features=64, n_informative=16, n_redundant=0, n_classes=3,
+                                   class_sep=0.8, flip_y=0.02, random_state=0)
+        X = np.ascontiguousarray(StandardScaler().fit_transform(X).astype(np.float32))
+        return dict(name="linsvc_multi", X=X, y=y.astype(np.int64), estimator="LinearSVC", est_params={},
+                    param_grid={"C": np.logspace(-3, 1, 6)}, cv=5, search="grid")
+    if which == "c3":
+        w = _c3(name="linsvc_c3")
+        w.update(estimator="LinearSVC", param_distributions={"C": loguniform(1e-4, 1e2)})
+        return w
+    w = _c3(n=4000, d=32, name="linsvc_small")
+    w.update(estimator="LinearSVC", search="grid", param_grid={"C": np.logspace(-4, 2, 8)})
+    return w
+
+
 WORKLOADS = {
     "c1": _c1, "c2": _c2, "c3": _c3, "c4": _c4, "c5": _c5,
     # reduced-size variants: same recipes, sizes the CPU oracle finishes in seconds
@@ -115,6 +136,10 @@ WORKLOADS = {
     # SVC poly / sigmoid: the golden-sized grid and the same grid on config-2 data (tools/bench_kernels.py)
     "svc_kernels_mid": _svc_kernels,
     "svc_kernels_c2": lambda: _svc_kernels(n=10000, d=512, name="svc_kernels_c2"),
+    # LinearSVC, primal TRON (csrc/linsvc.cu): golden-sized binary and 3-class grids, and config 3's search (tools/bench_linsvc.py)
+    "linsvc_small": _linsvc,
+    "linsvc_multi": lambda: _linsvc("multi"),
+    "linsvc_c3": lambda: _linsvc("c3"),
 }
 
 
@@ -136,6 +161,9 @@ def make_estimator(w):
     if w["estimator"] == "SVR":
         from sklearn.svm import SVR
         return SVR(**w["est_params"])
+    if w["estimator"] == "LinearSVC":
+        from sklearn.svm import LinearSVC
+        return LinearSVC(**w["est_params"])
     if w["estimator"] in ("Lasso", "ElasticNet"):
         import sklearn.linear_model as lm
         return getattr(lm, w["estimator"])(**w["est_params"])
