@@ -247,11 +247,9 @@ double gs_svc_predicted_iterations(int32_t kernel, double C, double gamma, int32
  * the SM count (the makespan model documented in DESIGN.md section 4). */
 int32_t gs_svc_cluster_count(const double *cost_desc, int32_t n, int32_t sm_count);
 /* Three-tier schedule of the slot-layout solver: of problems sorted by descending predicted cost, *n_cluster go on 4-CTA
- * clusters, the next *n_exclusive get an SM each, the rest share SMs two by two.  The split is the one whose SIMULATED
- * makespan is smallest (event simulation of the block scheduler handing freed SMs to the pending shared CTAs, csrc/api.cu);
- * gs_svc_simulate returns that makespan for a given split (cost x per-iteration-time units; test hook). */
+ * clusters, the next *n_exclusive get an SM each, the rest share SMs two by two.  The split is the one whose predicted
+ * makespan is smallest (the closed-form model documented in csrc/api.cu and DESIGN.md section 4). */
 void gs_svc_schedule(const double *cost_desc, int32_t n, int32_t sm_count, int32_t *n_cluster, int32_t *n_exclusive);
-double gs_svc_simulate(const double *cost_desc, int32_t n, int32_t sm_count, int32_t n_cluster, int32_t n_exclusive);
 
 /* ---- measurement ----------------------------------------------------------------------- */
 typedef struct gs_profile {

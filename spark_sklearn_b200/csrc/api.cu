@@ -9,8 +9,6 @@
 #include <cstdio>
 #include <cstdlib>
 #include <map>
-#include <mutex>
-#include <queue>
 #include <numeric>
 
 static std::string g_create_error;
@@ -79,7 +77,7 @@ __global__ void gather_rows_kernel(const T *__restrict__ src, const int *__restr
 
 extern "C" {
 
-int gs_version(void) { return 102; }
+int gs_version(void) { return 103; }
 
 int gs_set_class_weight(gs_handle *h, const double *w, int32_t n_sets)
 {
@@ -367,7 +365,7 @@ extern "C" int32_t gs_svc_cluster_count(const double *cost_desc, int32_t n, int3
 //                        0.50 sum(rest) / SMs left, 0.78 c[n_cl + n_ex]  shared SMs: throughput, and the longest shared
 //                                                                        problem (paired for most of its life, alone at the end) )
 // in units of (cost x shared-SM iteration time).  More specialised SMs only for a clear (3 %) predicted gain.
-static void schedule_closed_form(const double *cost_desc, int32_t n, int32_t sm_count, int32_t *n_cluster, int32_t *n_exclusive)
+extern "C" void gs_svc_schedule(const double *cost_desc, int32_t n, int32_t sm_count, int32_t *n_cluster, int32_t *n_exclusive)
 {
     if (n_cluster) *n_cluster = 0;
     if (n_exclusive) *n_exclusive = 0;
@@ -388,133 +386,6 @@ static void schedule_closed_form(const double *cost_desc, int32_t n, int32_t sm_
     }
     if (n_cluster) *n_cluster = bc;
     if (n_exclusive) *n_exclusive = be;
-}
-
-// Alternative (B200GS_SCHEDULE=simulate; also the test hook gs_svc_simulate): the makespan of a candidate split is SIMULATED,
-// not bounded by a formula: the block scheduler hands every SM that a finished cluster or exclusive problem gives back to
-// the pending CTAs of the shared launch, so "SMs left for the shared tier" is not a constant.  It was no faster than the
-// closed form above where it was calibrated (148-SM GPUs), so that stays the default.  Inputs: per-iteration time RATIOS of
-// an 8000-row sub-problem from the same calibration: 3.55 us on a 4-CTA cluster, 5.45 alone on an SM, 9.4 when two share one.
-namespace {
-constexpr double RATE_CLUSTER = 3.55, RATE_SOLO = 5.45, RATE_PAIR = 9.4;
-
-// Event simulation of one launch: cost_desc[0..nc) on clusters (4 SMs each), [nc, nc+ne) alone on an SM, the others in
-// launch order on the two slots of every SM as it becomes free.  Returns the makespan in cost x rate units.
-double simulate_tiers(const double *c, int n, int sms, int nc, int ne)
-{
-    if (nc < 0 || ne < 0 || nc + ne > n || 4 * nc + ne > sms) return 1e300;
-    struct Ev { double t; int sm, slot, ver; bool operator<(const Ev &o) const { return t > o.t; } };
-    struct Sm { double rem[2] = {0, 0}; bool busy[2] = {false, false}; int ver[2] = {0, 0}; double last = 0; };
-    std::vector<Sm> sm(sms);
-    std::priority_queue<Ev> ev;
-    double end = 0;
-    int s = 0;
-    for (int i = 0; i < nc; i++) { const double t = c[i] * RATE_CLUSTER; end = std::max(end, t); for (int k = 0; k < 4; k++) ev.push(Ev{t, s++, -1, 0}); }
-    for (int i = 0; i < ne; i++) { const double t = c[nc + i] * RATE_SOLO; end = std::max(end, t); ev.push(Ev{t, s++, -1, 0}); }
-    for (; s < sms; s++) ev.push(Ev{0.0, s, -1, 0});
-    int next = nc + ne;
-    auto resched = [&](int q, double t) {
-        Sm &m = sm[q];
-        const double per = (m.busy[0] && m.busy[1]) ? RATE_PAIR : RATE_SOLO;
-        for (int k = 0; k < 2; k++)
-            if (m.busy[k]) ev.push(Ev{t + m.rem[k] * per, q, k, ++m.ver[k]});
-    };
-    while (!ev.empty()) {
-        const Ev e = ev.top(); ev.pop();
-        Sm &m = sm[e.sm];
-        if (e.slot < 0) {                                           // the SM joins the shared tier
-            m.last = e.t;
-            for (int k = 0; k < 2 && next < n; k++) { m.rem[k] = c[next++]; m.busy[k] = true; }
-            resched(e.sm, e.t);
-            continue;
-        }
-        if (!m.busy[e.slot] || e.ver != m.ver[e.slot]) continue;     // superseded by a rate change
-        const double rate = 1.0 / ((m.busy[0] && m.busy[1]) ? RATE_PAIR : RATE_SOLO), dt = e.t - m.last;
-        for (int k = 0; k < 2; k++)
-            if (m.busy[k]) m.rem[k] = std::max(0.0, m.rem[k] - dt * rate);
-        m.last = e.t;
-        m.busy[e.slot] = false;
-        end = std::max(end, e.t);
-        if (next < n) { m.rem[e.slot] = c[next++]; m.busy[e.slot] = true; }
-        resched(e.sm, e.t);
-    }
-    return end;
-}
-}  // namespace
-
-extern "C" double gs_svc_simulate(const double *cost_desc, int32_t n, int32_t sm_count, int32_t n_cluster, int32_t n_exclusive)
-{
-    if (!cost_desc || n < 1 || sm_count < 1) return 0.0;
-    return simulate_tiers(cost_desc, n, sm_count, n_cluster, n_exclusive);
-}
-
-static void schedule_simulated(const double *cost_desc, int32_t n, int32_t sm_count, int32_t *n_cluster, int32_t *n_exclusive)
-{
-    if (n_cluster) *n_cluster = 0;
-    if (n_exclusive) *n_exclusive = 0;
-    if (!cost_desc || n < 2 || sm_count < 8) return;
-    // a repeated search of the same shape re-uses the last answer
-    static std::mutex mu;
-    static std::vector<double> last_cost;
-    static int last_sms = 0, last_c = 0, last_e = 0;
-    {
-        std::lock_guard<std::mutex> lk(mu);
-        if (last_sms == sm_count && (int)last_cost.size() == n && std::equal(last_cost.begin(), last_cost.end(), cost_desc)) {
-            if (n_cluster) *n_cluster = last_c;
-            if (n_exclusive) *n_exclusive = last_e;
-            return;
-        }
-    }
-    const double *c = cost_desc;
-    std::vector<double> suffix(n + 1, 0.0);
-    for (int q = n - 1; q >= 0; q--) suffix[q] = suffix[q + 1] + c[q];
-    // candidates: tier boundaries at changes of the predicted cost (the folds of one candidate stay in one tier)
-    std::vector<int> cut;
-    for (int q = 0; q <= n - 1; q++)
-        if (q == 0 || c[q - 1] > c[q] * (1.0 + 1e-9)) cut.push_back(q);
-    double best = simulate_tiers(c, n, sm_count, 0, 0);
-    int bc = 0, be = 0;
-    const int max_cl = std::min(n - 1, sm_count / 4);
-    // at most ~12 x 24 candidate splits (costs that are all distinct, e.g. one-vs-one pairs of different sizes, would
-    // otherwise give one boundary per problem): every k-th boundary among those a tier can reach
-    std::vector<int> cut_c, cut_e;
-    for (int q : cut) { if (q <= max_cl) cut_c.push_back(q); if (q <= sm_count - 8) cut_e.push_back(q); }
-    auto thin = [](std::vector<int> &v, size_t keep) {
-        if (v.size() <= keep) return;
-        std::vector<int> w;
-        for (size_t i = 0; i < keep; i++) w.push_back(v[i * (v.size() - 1) / (keep - 1)]);
-        w.erase(std::unique(w.begin(), w.end()), w.end());
-        v.swap(w);
-    };
-    thin(cut_c, 12); thin(cut_e, 24);
-    for (int nc : cut_c) {
-        for (int pos : cut_e) {
-            const int ne = pos - nc;
-            if (ne < 0 || (nc == 0 && ne == 0)) continue;
-            if (4 * nc + ne > sm_count - 8 || nc + ne >= n) break;
-            // lower bounds: the longest problem of every tier, and the SM time of the whole split
-            double lb = std::max(nc ? c[0] * RATE_CLUSTER : 0.0, std::max(ne ? c[nc] * RATE_SOLO : 0.0, c[nc + ne] * RATE_SOLO));
-            lb = std::max(lb, (4.0 * RATE_CLUSTER * (suffix[0] - suffix[nc]) + RATE_SOLO * (suffix[nc] - suffix[nc + ne]) +
-                               0.5 * RATE_PAIR * suffix[nc + ne]) / sm_count);
-            if (lb >= 0.985 * best) continue;
-            const double t = simulate_tiers(c, n, sm_count, nc, ne);
-            // specialised SMs only for a clear (1.5 %) predicted gain; near-ties go to the split that uses fewer of them
-            if (t < 0.985 * best || (t < best && 4 * nc + ne <= 4 * bc + be)) { best = t; bc = nc; be = ne; }
-        }
-    }
-    {
-        std::lock_guard<std::mutex> lk(mu);
-        last_cost.assign(cost_desc, cost_desc + n); last_sms = sm_count; last_c = bc; last_e = be;
-    }
-    if (n_cluster) *n_cluster = bc;
-    if (n_exclusive) *n_exclusive = be;
-}
-
-extern "C" void gs_svc_schedule(const double *cost_desc, int32_t n, int32_t sm_count, int32_t *n_cluster, int32_t *n_exclusive)
-{
-    const char *mode = getenv("B200GS_SCHEDULE");
-    if (mode && !strcmp(mode, "simulate")) schedule_simulated(cost_desc, n, sm_count, n_cluster, n_exclusive);
-    else schedule_closed_form(cost_desc, n, sm_count, n_cluster, n_exclusive);
 }
 
 static int svc_run(gs_handle *h, int n_cand, const int32_t *kernel, const double *Cv, const double *gamma,
@@ -716,10 +587,9 @@ static int svc_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
         //   * fewer problems than SMs: everything on the widest cluster that fits;
         //   * otherwise the number of clustered problems minimises a three-term makespan model (below): none for a
         //     throughput-bound search (config 4), exactly the ten 66-68k-iteration problems for config 2 (at 148 and 132 SMs).
-        // Development switches: B200GS_SMO_CLUSTER (0/2/4/8),
-        // B200GS_SMO_CLUSTER_N.
         std::string why;
-        // single-CTA launches go to the slot-layout kernel (smo_lean.cu) when every problem of the batch has one
+        // single-CTA launches go to the slot-layout kernel (smo_lean.cu) when every problem of the batch has one;
+        // B200GS_SMO_LEAN=0 forces the position-owned kernel (smo.cu)
         int max_slots = 0;
         bool lean_ok = lmax < 16383 && !(getenv("B200GS_SMO_LEAN") && atoi(getenv("B200GS_SMO_LEAN")) == 0);
         for (int q = 0; q < np && lean_ok; q++) {
@@ -740,7 +610,7 @@ static int svc_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
         //   * fewer problems than SMs: everything on the widest cluster that fits;
         //   * otherwise the three-tier schedule of the slot-layout kernel, or -- when a problem has no slot layout -- the
         //     two-tier schedule of the position-owned kernel (gs_svc_cluster_count).
-        // Development switches: B200GS_SMO_CLUSTER (0/2/4/8), B200GS_SMO_CLUSTER_N, B200GS_SMO_EXCLUSIVE_N.
+        // B200GS_SMO_CLUSTER (0/2/4/8) and B200GS_SMO_CLUSTER_N force the cluster size and the number of clustered problems.
         int cl = 0, n_cl = 0, n_ex = 0;
         if (lmax > 2048) {
             if (np * 8 <= h->sm_count) { cl = 8; n_cl = np; }
@@ -757,8 +627,6 @@ static int svc_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
         if (const char *e = getenv("B200GS_SMO_CLUSTER")) { cl = atoi(e); if (n_cl == 0) n_cl = std::max(1, np * 6 / 100); }
         if (const char *e = getenv("B200GS_SMO_CLUSTER_N")) n_cl = std::min(np, atoi(e));
         if (!(cl == 2 || cl == 4 || cl == 8) || lmax > smo_colown_max_rows(cl) || lmax <= 2048) n_cl = 0;
-        if (const char *e = getenv("B200GS_SMO_EXCLUSIVE_N")) n_ex = atoi(e);
-        if (!lean_ok) n_ex = 0;
         n_ex = std::max(0, std::min(n_ex, np - n_cl));
         if (n_cl > 0 || n_ex > 0) {
             // The latency tiers must get their SMs before the shared-SM launch floods the GPU (a late start of the critical

@@ -3,7 +3,6 @@
 #include "common.cuh"
 #include <algorithm>
 #include <cmath>
-#include <cstdlib>
 #include <map>
 
 // Default: float64 on the FP64 pipe (libsvm-faithful, gram.cu).  GS_GRAM_TENSOR: wgmma tensor cores, 3xTF32 split,
@@ -118,7 +117,6 @@ int SvmSearch::kernel_matrices(int g0, int g1)
     // device flag the kernel-matrix kernels raise: both instances are enqueued and the wrong one returns at once
     // (SmoProblem::guard), so the host never waits in the middle of a search and everything it prepares next overlaps
     // the Gram and kernel-matrix kernels already in flight.
-    if (getenv("B200GS_SMO_NOFAST") && atoi(getenv("B200GS_SMO_NOFAST"))) fast = false;   // development switch: general instance only, unguarded
     d_guard = fast ? h->dWork[7].as<int>() : nullptr;
     tm.mark(1);
     return GS_OK;

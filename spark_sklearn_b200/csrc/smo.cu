@@ -35,7 +35,6 @@
 //     resident in shared memory (27 B/row, 221 KB), the Q_i row of the owned positions in registers.
 // Per iteration: two dependent gathers of a K row (HBM/L2), three CTA barriers.
 #include "smo_common.cuh"
-#include <cstdlib>
 
 namespace {
 
@@ -725,27 +724,20 @@ cudaError_t launch_cfg(const SmoProblem *probs, const int *order, int n_prob, bo
                 : launch_one<NT, KPT, SMEM_STATE, false, false, ROWBUF, SVR>(probs, order, n_prob, rowcap, svr, st);
 }
 
-int env_int(const char *name, int dflt)
-{
-    const char *v = getenv(name);
-    return v && *v ? atoi(v) : dflt;
-}
-
 // the tier choice of launch_smo / launch_smo_svr: lmax positions (C-SVC rows, or twice the SVR training rows)
 template <bool SVR>
 cudaError_t launch_tiers(const SmoProblem *d_probs, const int *d_order, int n_prob, int lmax, bool fast, int rowcap,
                          const SvrData *svr, cudaStream_t st, std::string *why)
 {
     if (n_prob <= 0) return cudaSuccess;
-    const bool prof = env_int("B200GS_SMO_PROF", 0) != 0;          // development switch: per-phase cycle counters
-    if (env_int("B200GS_SMO_NOFAST", 0)) fast = false;
+    const bool prof = prof_enabled();
     if (lmax <= 512) return launch_cfg<128, 4, true, false, SVR>(d_probs, d_order, n_prob, fast, prof, 0, svr, st);
     if (lmax <= 2048) return launch_cfg<256, 8, true, false, SVR>(d_probs, d_order, n_prob, fast, prof, 0, svr, st);
     if (lmax <= 4096) return launch_cfg<512, 8, true, false, SVR>(d_probs, d_order, n_prob, fast, prof, 0, svr, st);
     if (lmax <= 8192) {
         // 8192 rows of state without G_bar = 152 KB; the row buffer may use what is left of the 227 KB
         const bool rowbuf_fits = (size_t)8192 * 19 + 128 + (size_t)rowcap * 4 + 4096 <= 227 * 1024;
-        if (rowbuf_fits && env_int("B200GS_SMO_ROWBUF", 1))
+        if (rowbuf_fits)
             return launch_cfg<1024, 8, true, true, SVR>(d_probs, d_order, n_prob, fast, prof, rowcap, svr, st);
         return launch_cfg<1024, 8, true, false, SVR>(d_probs, d_order, n_prob, fast, prof, 0, svr, st);
     }

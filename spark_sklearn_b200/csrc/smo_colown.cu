@@ -28,7 +28,6 @@
 // reconstruction and calculate_rho walk positions in ascending order through position-indexed global scratch.
 #include "smo_common.cuh"
 #include <cooperative_groups.h>
-#include <cstdlib>
 
 namespace cg = cooperative_groups;
 
@@ -835,9 +834,7 @@ cudaError_t launch_co(const SmoProblem *probs, const int *order, int n_prob, int
 template <int NT, int KPT, int CL>
 cudaError_t launch_co_f(const SmoProblem *p, const int *o, int n, int lmax, bool fast, cudaStream_t st)
 {
-    const char *e = getenv("B200GS_SMO_PROF");
-    const bool prof = e && atoi(e) != 0;                                    // development switch: per-phase cycle counters
-    if (prof) return fast ? launch_co<NT, KPT, CL, true, true>(p, o, n, lmax, st) : launch_co<NT, KPT, CL, false, true>(p, o, n, lmax, st);
+    if (prof_enabled()) return fast ? launch_co<NT, KPT, CL, true, true>(p, o, n, lmax, st) : launch_co<NT, KPT, CL, false, true>(p, o, n, lmax, st);
     return fast ? launch_co<NT, KPT, CL, true, false>(p, o, n, lmax, st) : launch_co<NT, KPT, CL, false, false>(p, o, n, lmax, st);
 }
 
@@ -862,23 +859,14 @@ cudaError_t launch_smo_colown(const SmoProblem *d_probs, const int *d_order, int
 {
     if (n_prob <= 0) return cudaSuccess;
     if (lmax > smo_colown_max_rows(cl)) return cudaErrorInvalidValue;
-    int nt = 0;
-    if (const char *e = getenv("B200GS_SMO_NT")) nt = atoi(e);                  // development switch
     // 512 threads at most: the register-resident state needs more than the 64 registers a 1024-thread CTA leaves a thread
-    if (cl == 2) {
-        if (nt == 1024) return launch_co_f<1024, 4, 2>(d_probs, d_order, n_prob, lmax, fast, st);
-        return launch_co_f<512, 8, 2>(d_probs, d_order, n_prob, lmax, fast, st);
-    }
+    if (cl == 2) return launch_co_f<512, 8, 2>(d_probs, d_order, n_prob, lmax, fast, st);
     if (cl == 4) {
         if (lmax > 8192) return launch_co_f<512, 8, 4>(d_probs, d_order, n_prob, lmax, fast, st);
-        if (nt == 256) return launch_co_f<256, 8, 4>(d_probs, d_order, n_prob, lmax, fast, st);
-        if (nt == 1024) return launch_co_f<1024, 2, 4>(d_probs, d_order, n_prob, lmax, fast, st);
         return launch_co_f<512, 4, 4>(d_probs, d_order, n_prob, lmax, fast, st);
     }
     if (cl == 8) {
         if (lmax > 8192) return launch_co_f<512, 4, 8>(d_probs, d_order, n_prob, lmax, fast, st);
-        if (nt == 512) return launch_co_f<512, 2, 8>(d_probs, d_order, n_prob, lmax, fast, st);
-        if (nt == 1024) return launch_co_f<1024, 1, 8>(d_probs, d_order, n_prob, lmax, fast, st);
         return launch_co_f<256, 4, 8>(d_probs, d_order, n_prob, lmax, fast, st);
     }
     return cudaErrorInvalidValue;

@@ -1,6 +1,8 @@
-// smo_common.cuh -- helpers shared by the single-CTA (smo.cu) and the cluster (smo_colown.cu) SMO kernels.
+// smo_common.cuh -- helpers shared by the position-owned (smo.cu), slot-layout (smo_lean.cu) and cluster (smo_colown.cu)
+// SMO kernels.
 #pragma once
 #include "common.cuh"
+#include <cstdlib>
 #include <math_constants.h>
 
 namespace smo {
@@ -10,6 +12,14 @@ constexpr int ST_LOWER = 0, ST_UPPER = 1, ST_FREE = 2;
 constexpr int F_YPOS = 4, F_UP = 8, F_LOW = 16, F_MARK = 32;
 constexpr int IDX_SHIFT = 5;                 // packed index = (position << 5) | (flags & 31)
 constexpr int SAFETY_MAX_ITER = 10000000;    // max_iter=-1 is "no limit" in libsvm; bound a runaway solve
+
+// B200GS_SMO_PROF=1 launches the PROF instances: per-phase cycle counters of every sub-problem in out_ns[2..] (a
+// diagnostic: the iterates are the same)
+inline bool prof_enabled()
+{
+    const char *e = getenv("B200GS_SMO_PROF");
+    return e && atoi(e) != 0;
+}
 
 __device__ __forceinline__ int mkflags(bool ypos, int st)
 {

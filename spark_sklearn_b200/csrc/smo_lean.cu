@@ -35,7 +35,6 @@
 //   * float32 -> float64 widening of a positive normal K entry is ONE integer multiply-add (u * 2^29 + 0x38 << 56).
 #include "smo_common.cuh"
 #include <algorithm>
-#include <cstdlib>
 #include <type_traits>
 
 namespace {
@@ -143,7 +142,7 @@ struct LeanRed {                                      // static shared scratch; 
     unsigned b_k1[32], b_pf[32], b_k2[32], b_fl[32];  // phase B warp records (approximate arg-max, stop-test bits)
     float b_kq[32]; double b_al[32], b_mg[32];        // ... the warp winner's K_i value, alpha and m
     double al_i;                                      // alpha_i (published by warp 0 before barrier 2)
-    double bc_d[4]; int bc_i[2];                      // shared-SM instance: the two-variable update broadcast by warp 0
+    double bc_d[4]; int bc_i[2];                      // the two-variable update broadcast by warp 0
     unsigned x_hi[32], x_lo[32], x_pf[32];            // exact tie-break records (rare path)
     float x_kq[32]; double x_al[32], x_mg[32];
     double dm[32], dm2[32]; int cnt[32];              // cold-path reductions
@@ -152,10 +151,7 @@ struct LeanRed {                                      // static shared scratch; 
 };
 
 // NT threads, G groups of 4 consecutive slots per thread: NT * G * 4 slots, NT * G * 48 bytes of shared memory
-// SOLO: the sub-problem has its SM to itself (exclusive tier, or fewer problems than SMs): every warp evaluates the two-variable
-// update (no third barrier: latency).  Otherwise two sub-problems share the SM and issue slots are the scarce resource: warp 0
-// evaluates it once and the others wait at a third barrier, which the co-resident CTA fills.
-template <int NT, int G, bool FAST, bool PROF, bool SOLO>
+template <int NT, int G, bool FAST, bool PROF>
 __global__ void __launch_bounds__(NT, (NT * G >= 4096 || NT >= 1024 ? 1 : 2048 / (NT * G / 2) > 8 ? 8 : 2048 / (NT * G / 2)))
 smo_lean_kernel(const SmoProblem *__restrict__ probs, const int *__restrict__ order)
 {
@@ -709,13 +705,14 @@ smo_lean_kernel(const SmoProblem *__restrict__ probs, const int *__restrict__ or
         const int slot_i = (int)((pi >> SLOT_SHIFT) & SLOT_MASK), slot_j = (int)((pj >> SLOT_SHIFT) & SLOT_MASK);
         float kvj[KPT];
         load_row(col_j, kvj);                                    // in flight during the scalar update
-        // analytic two-variable update.  SOLO: evaluated by EVERY warp (uniform) -- its ~250 dependent instructions run under
-        // the row-j fetch that each warp waits for anyway and the CTA needs no third barrier (a single warp computing it kept
-        // the other fifteen parked).  Shared SM: warp 0 alone (4000 fewer warp-instructions per iteration).
+        // analytic two-variable update, evaluated by warp 0 alone behind a third barrier: issue slots are the scarce resource
+        // when two sub-problems share the SM, and the co-resident CTA fills the barrier.  Every warp evaluating it redundantly
+        // (no third barrier) was slower: config 2's solve phase took 342.2 ms against 331.8 ms (one H100 SXM capped at 400 W,
+        // B200GS_SMO_TIMELINE, same run).
         double a = 0, b = 0, ai_new = 0, aj_new = 0;
         int sti = 0, stj = 0;
         const bool yi = slot_i < ysplit, yj = slot_j < ysplit;
-        if (SOLO || warp == 0) {
+        if (warp == 0) {
             const double Ci = yi ? Cc : Cneg, Cj = yj ? Cc : Cneg;             // per-class C (class_weight, svm.cpp:1393-1396 get_C)
             const double Gi = yi ? -gmax : gmax;                 // G = -y m (exact)
             const double Gj = yj ? -mg_j : mg_j;
@@ -749,19 +746,15 @@ smo_lean_kernel(const SmoProblem *__restrict__ probs, const int *__restrict__ or
             a = yi ? -dai : dai;                                 // a = -y_i dalpha_i
             b = yj ? -daj : daj;                                 // b = -y_j dalpha_j
             ai_new = ai; aj_new = aj;
-            if constexpr (!SOLO) {
-                if (lane == 0) {
-                    red.bc_d[0] = a; red.bc_d[1] = b; red.bc_d[2] = ai; red.bc_d[3] = aj;
-                    red.bc_i[0] = sti; red.bc_i[1] = stj;
-                }
+            if (lane == 0) {
+                red.bc_d[0] = a; red.bc_d[1] = b; red.bc_d[2] = ai; red.bc_d[3] = aj;
+                red.bc_i[0] = sti; red.bc_i[1] = stj;
             }
         }
         tick(4);
-        if constexpr (!SOLO) {
-            __syncthreads();                                                      // barrier 3
-            a = red.bc_d[0]; b = red.bc_d[1]; ai_new = red.bc_d[2]; aj_new = red.bc_d[3];
-            sti = red.bc_i[0]; stj = red.bc_i[1];
-        }
+        __syncthreads();                                                          // barrier 3
+        a = red.bc_d[0]; b = red.bc_d[1]; ai_new = red.bc_d[2]; aj_new = red.bc_d[3];
+        sti = red.bc_i[0]; stj = red.bc_i[1];
         tick(5);
         {
             // the OWNERS of i and j store alpha and the slot word (new status and set membership) and patch their flag mask;
@@ -926,13 +919,13 @@ smo_lean_kernel(const SmoProblem *__restrict__ probs, const int *__restrict__ or
     }
 }
 
-template <int NT, int G, bool FAST, bool PROF, bool SOLO>
+template <int NT, int G, bool FAST, bool PROF>
 cudaError_t launch_lean_one(const SmoProblem *probs, const int *order, int n_prob, bool exclusive, cudaStream_t st)
 {
     constexpr int LCAP = NT * G * 4;
     // exclusive: ask for more than half of the SM's 227 KB so that no second CTA (of this or of the shared launch) fits
     const size_t smem = exclusive ? std::max<size_t>((size_t)LCAP * 12, 132 * 1024) : (size_t)LCAP * 12;
-    auto kern = smo_lean_kernel<NT, G, FAST, PROF, SOLO>;
+    auto kern = smo_lean_kernel<NT, G, FAST, PROF>;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
     e = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
@@ -941,23 +934,11 @@ cudaError_t launch_lean_one(const SmoProblem *probs, const int *order, int n_pro
     return cudaGetLastError();
 }
 
-template <int NT, int G, bool SOLO>
-cudaError_t launch_lean_cfg2(const SmoProblem *probs, const int *order, int n_prob, bool fast, bool prof, bool excl, cudaStream_t st)
-{
-    if (prof) return fast ? launch_lean_one<NT, G, true, true, SOLO>(probs, order, n_prob, excl, st) : launch_lean_one<NT, G, false, true, SOLO>(probs, order, n_prob, excl, st);
-    return fast ? launch_lean_one<NT, G, true, false, SOLO>(probs, order, n_prob, excl, st) : launch_lean_one<NT, G, false, false, SOLO>(probs, order, n_prob, excl, st);
-}
-
 template <int NT, int G>
-cudaError_t launch_lean_cfg(const SmoProblem *probs, const int *order, int n_prob, bool fast, bool prof, bool excl, bool solo, cudaStream_t st)
+cudaError_t launch_lean_cfg(const SmoProblem *probs, const int *order, int n_prob, bool fast, bool prof, bool excl, cudaStream_t st)
 {
-    return solo ? launch_lean_cfg2<NT, G, true>(probs, order, n_prob, fast, prof, excl, st) : launch_lean_cfg2<NT, G, false>(probs, order, n_prob, fast, prof, excl, st);
-}
-
-int env_int(const char *name, int dflt)
-{
-    const char *v = getenv(name);
-    return v && *v ? atoi(v) : dflt;
+    if (prof) return fast ? launch_lean_one<NT, G, true, true>(probs, order, n_prob, excl, st) : launch_lean_one<NT, G, false, true>(probs, order, n_prob, excl, st);
+    return fast ? launch_lean_one<NT, G, true, false>(probs, order, n_prob, excl, st) : launch_lean_one<NT, G, false, false>(probs, order, n_prob, excl, st);
 }
 
 }  // namespace
@@ -970,20 +951,14 @@ int smo_lean_max_slots() { return 16384; }
 cudaError_t launch_smo_lean(const SmoProblem *d_probs, const int *d_order, int n_prob, int max_slots, bool fast, bool exclusive, cudaStream_t st)
 {
     if (n_prob <= 0) return cudaSuccess;
-    const bool prof = env_int("B200GS_SMO_PROF", 0) != 0;                    // development switch: per-phase cycle counters
-    if (env_int("B200GS_SMO_NOFAST", 0)) fast = false;
-    // Two instances of the two-variable update: warp 0 evaluates it behind a third barrier, or every warp evaluates it
-    // redundantly (SOLO).  The barrier instance is the default: config 2's solve phase takes 331.8 ms with it and 342.2 ms with
-    // SOLO (one H100 SXM capped at 400 W, B200GS_SMO_TIMELINE, same run).
-    bool solo = false;
-    if (const char *e = getenv("B200GS_LEAN_SOLO")) solo = atoi(e) != 0;      // development switch
+    const bool prof = prof_enabled();
     // A problem alone on its SM spreads over 1024 threads x 8 slots instead of 512 x 16 (bit-identical trajectories): config 2's
-    // solve phase takes 331.8 ms with it and 352.6 ms without (same H100 run as above).  B200GS_LEAN_EXCL_WIDE=0: off.
-    if (exclusive && max_slots > 4096 && max_slots <= 8192 && env_int("B200GS_LEAN_EXCL_WIDE", 1))
-        return launch_lean_cfg<1024, 2>(d_probs, d_order, n_prob, fast, prof, exclusive, solo, st);
-    if (max_slots <= 2048) return launch_lean_cfg<128, 4>(d_probs, d_order, n_prob, fast, prof, exclusive, solo, st);
-    if (max_slots <= 4096) return launch_lean_cfg<256, 4>(d_probs, d_order, n_prob, fast, prof, exclusive, solo, st);
-    if (max_slots <= 8192) return launch_lean_cfg<512, 4>(d_probs, d_order, n_prob, fast, prof, exclusive, solo, st);
-    if (max_slots <= 16384) return launch_lean_cfg<1024, 4>(d_probs, d_order, n_prob, fast, prof, exclusive, solo, st);
+    // solve phase takes 331.8 ms with it and 352.6 ms without (one H100 SXM capped at 400 W, B200GS_SMO_TIMELINE, same run).
+    if (exclusive && max_slots > 4096 && max_slots <= 8192)
+        return launch_lean_cfg<1024, 2>(d_probs, d_order, n_prob, fast, prof, exclusive, st);
+    if (max_slots <= 2048) return launch_lean_cfg<128, 4>(d_probs, d_order, n_prob, fast, prof, exclusive, st);
+    if (max_slots <= 4096) return launch_lean_cfg<256, 4>(d_probs, d_order, n_prob, fast, prof, exclusive, st);
+    if (max_slots <= 8192) return launch_lean_cfg<512, 4>(d_probs, d_order, n_prob, fast, prof, exclusive, st);
+    if (max_slots <= 16384) return launch_lean_cfg<1024, 4>(d_probs, d_order, n_prob, fast, prof, exclusive, st);
     return cudaErrorInvalidValue;
 }

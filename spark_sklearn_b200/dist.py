@@ -56,79 +56,11 @@ def assign_candidates(n_cand, world, costs=None):
     return [sorted(p) for p in parts]
 
 
-def assign_groups(n_cand, world, costs, keys, max_imbalance=1.08):
-    """Experimental (B200GS_DEAL=groups): deal whole affinity groups (for SVC: all candidates sharing one gamma, which
-    share one kernel matrix and one decision-value pass) instead of single candidates.  Groups are sorted by total
-    predicted cost and dealt in snake order; if there are fewer than 2*world groups or the predicted loads differ by
-    more than ``max_imbalance`` the cost-balanced candidate dealing is used instead."""
-    costs = np.asarray(costs, dtype=np.float64)
-    groups = {}
-    for c, k in enumerate(keys):
-        groups.setdefault(k, []).append(c)
-    if len(groups) < 2 * world:
-        return assign_candidates(n_cand, world, costs)
-    order = sorted(groups, key=lambda k: (-costs[groups[k]].sum(), str(k)))
-    parts = [[] for _ in range(world)]
-    for pos, k in enumerate(order):
-        lap, r = divmod(pos, world)
-        parts[r if lap % 2 == 0 else world - 1 - r].extend(groups[k])
-    load = [costs[p].sum() for p in parts]
-    if min(load) <= 0 or max(load) > max_imbalance * min(load):
-        return assign_candidates(n_cand, world, costs)
-    return [sorted(p) for p in parts]
-
-
-def assign_affinity(n_cand, world, costs, keys, group_cost):
-    """Cost dealing that keeps affinity groups together (for SVC: candidates sharing a gamma share one kernel matrix and one
-    float64 decision-value pass per GPU -- `group_cost` in the units of `costs`).  Two tiers:
-      1. the 2*world most expensive candidates (the fits that set the makespan) are dealt one by one in snake order, exactly
-         as assign_candidates does: every rank gets the same share of the critical path;
-      2. the others travel in half-groups (the candidates of one group, split in two by cost): longest half-group first onto
-         the rank whose load after taking it -- plus group_cost if the rank does not hold that group yet -- is smallest.
-    Deterministic and identical on every rank; ranks may end with different candidate counts (the gather pads)."""
-    costs = np.asarray(costs, dtype=np.float64)
-    order = np.argsort(-costs, kind="stable")
-    n_heavy = min(n_cand, 2 * world)
-    parts = [[] for _ in range(world)]
-    load = np.zeros(world)
-    have = [set() for _ in range(world)]
-    for pos, c in enumerate(order[:n_heavy]):
-        lap, k = divmod(pos, world)
-        r = k if lap % 2 == 0 else world - 1 - k
-        c = int(c)
-        load[r] += costs[c] + (0.0 if keys[c] in have[r] else group_cost)
-        parts[r].append(c); have[r].add(keys[c])
-    groups = {}
-    for c in order[n_heavy:]:
-        groups.setdefault(keys[int(c)], []).append(int(c))                 # descending cost inside a group
-    units = []
-    for k, members in groups.items():
-        half = -(-len(members) // 2)
-        for piece in (members[:half], members[half:]):
-            if piece:
-                units.append((float(costs[piece].sum()), str(k), k, piece))
-    units.sort(key=lambda u: (-u[0], u[1]))
-    for ucost, _, k, piece in units:
-        t = [load[r] + ucost + (0.0 if k in have[r] else group_cost) for r in range(world)]
-        r = int(np.argmin(t))
-        load[r] = t[r]; parts[r].extend(piece); have[r].add(k)
-    return [sorted(p) for p in parts]
-
-
 def assign_for_plan(plan, n_cand, world):
-    """The dealing used by the search driver and by bench.py: by predicted cost (default) or, with B200GS_DEAL=groups,
-    by affinity group where that still balances."""
-    import os
+    """The dealing used by the search driver and by bench.py: by the plan's predicted cost per candidate, if it has one."""
     if world == 1:
         return assign_candidates(n_cand, 1)
     costs = plan.costs() if hasattr(plan, "costs") else None
-    mode = os.environ.get("B200GS_DEAL", "cost")
-    if costs is not None and mode in ("groups", "affinity"):
-        keys = plan.affinity() if hasattr(plan, "affinity") else None
-        if keys is not None and mode == "groups":
-            return assign_groups(n_cand, world, costs, keys)
-        if keys is not None:
-            return assign_affinity(n_cand, world, costs, keys, getattr(plan, "group_cost", 0.0))
     return assign_candidates(n_cand, world, costs)
 
 

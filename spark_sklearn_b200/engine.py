@@ -87,8 +87,6 @@ def load_library():
     L.gs_svc_cluster_count.restype = i32
     L.gs_svc_schedule.argtypes = [vp, i32, i32, vp, vp]
     L.gs_svc_schedule.restype = None
-    L.gs_svc_simulate.argtypes = [vp, i32, i32, i32, i32]
-    L.gs_svc_simulate.restype = dbl
     for f in ("gs_create", "gs_set_data", "gs_svc", "gs_svc_refit", "gs_ridge", "gs_ridge_refit", "gs_enet", "gs_enet_refit", "gs_set_targets_f64",
               "gs_svr", "gs_svr_refit", "gs_logreg",
               "gs_logreg_refit", "gs_linsvc", "gs_linsvc_refit", "gs_get_profile", "gs_debug_gram", "gs_debug_kernel_matrix",

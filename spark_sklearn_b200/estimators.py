@@ -233,10 +233,6 @@ class _Plan:
         """Predicted relative cost of every candidate (None: all alike) -- used to balance candidates over GPUs."""
         return None
 
-    def affinity(self):
-        """Per candidate, a hashable key of the device work it shares with others (None: nothing shared)."""
-        return None
-
     def close(self):
         pass
 
@@ -276,8 +272,7 @@ class SVCAdapter:
 
 
 class _KernelGamma:
-    """What the SVC and SVR plans share: the gamma of one libsvm fit (sklearn svm/_base.py:278-286), the kernel-matrix
-    affinity of the candidates and the Gram mode."""
+    """What the SVC and SVR plans share: the gamma of one libsvm fit (sklearn svm/_base.py:278-286) and the Gram mode."""
 
     def _gamma(self, g, k):
         """'scale' uses the variance of the TRAINING fold (float64); k < 0: all rows."""
@@ -295,24 +290,6 @@ class _KernelGamma:
             raise ValueError("gamma must be >= 0 or 'scale'/'auto'; got %r" % (g,))
         return float(g)
 
-    def affinity(self):
-        """Candidates with the same kernel matrix -- (kernel, gamma), plus coef0 for sigmoid and degree and coef0 for poly --
-        share it and a decision-value pass."""
-        try:
-            out = []
-            for cand in self.cands:
-                p = self._base_params(cand)
-                kern = p["kernel"]
-                key = (kern, self._gamma(p["gamma"], -1) if kern != "linear" else 0.0)
-                if kern == "poly":
-                    key += (int(p["degree"]), float(p["coef0"]))
-                elif kern == "sigmoid":
-                    key += (float(p["coef0"]),)
-                out.append(key)
-            return out
-        except Exception:
-            return None
-
     def _flags(self):
         import os
         # B200GS_GRAM=tensor: opt-in wgmma Gram (fp32-faithful; scores match to solver tolerance, not bit for bit)
@@ -323,9 +300,6 @@ class SVCPlan(_KernelGamma, _Plan):
     """sklearn.svm.SVC (C-SVC).  Scalars per candidate: kernel, C, gamma (resolved per fold for every kernel but linear),
     degree and coef0 (poly, sigmoid)."""
     scorers = CLASSIFICATION_SCORERS
-    # what one more (kernel, gamma) group costs a GPU, in the units of costs() (thousands of SMO iterations of one candidate's
-    # folds): a kernel matrix + a float64 decision-value pass, against the SMO time of one unit (ratio calibrated on a 148-SM GPU)
-    group_cost = 7.0
 
     def __init__(self, estimator, cands, X, y, fold_id, n_splits, device=None):
         super().__init__(estimator, cands, X, y, fold_id, n_splits, device)

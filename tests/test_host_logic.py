@@ -332,25 +332,6 @@ def test_assign_candidates_is_a_balanced_partition():
     assert assign_candidates(5, 2, [1, np.nan, 2, 3, 4]) == [[0, 2, 4], [1, 3]]   # unusable costs: strided
 
 
-def test_assign_groups_keeps_groups_whole_or_falls_back():
-    from spark_sklearn_b200.dist import assign_groups, assign_candidates
-    nc, ng, world = 8, 16, 2                                                # the 2-GPU weak-scaling grid: 8 C x 16 gamma
-    C = np.logspace(-1, 2.5, nc); G = np.geomspace(1 / 4096, 1 / 256, ng)
-    cc, gg = np.meshgrid(C, G, indexing="ij")
-    gd = gg.ravel() * 512
-    cost = np.minimum(4 + 10.3 * (cc.ravel() * gd) ** 0.95, 9 + 7.3 / gd)
-    keys = [("rbf", g) for g in gg.ravel()]
-    parts = assign_groups(len(cost), world, cost, keys)
-    assert sorted(sum(parts, [])) == list(range(len(cost)))
-    assert all(len({keys[c] for c in p}) == ng // world for p in parts)      # 8 whole gamma groups per rank
-    load = [cost[p].sum() for p in parts]
-    assert max(load) <= 1.08 * min(load)
-    # too few groups for the ranks, or loads that cannot balance: candidate dealing
-    assert assign_groups(len(cost), 16, cost, keys) == assign_candidates(len(cost), 16, cost)
-    skew = cost.copy(); skew[np.array([k == keys[0] for k in keys])] *= 100
-    assert assign_groups(len(cost), world, skew, keys) == assign_candidates(len(cost), world, skew)
-
-
 def test_in_process_scheduler_deals_candidates_over_devices_and_merges(monkeypatch):
     """One fit() over several devices without torch.distributed (north_star: "a single in-process scheduler"): a plan and a
     host thread per device, candidates dealt by predicted cost, host-side merge -- cv_results_ identical to the
@@ -383,28 +364,6 @@ def test_in_process_scheduler_deals_candidates_over_devices_and_merges(monkeypat
                 np.testing.assert_array_equal(np.asarray(v, float), np.asarray(multi.cv_results_[k], float), err_msg=k)
         assert multi.best_params_ == single.best_params_
         np.testing.assert_array_equal(multi.predict(X), single.predict(X))
-
-
-def test_assign_affinity_balances_cost_and_gathers_groups():
-    from spark_sklearn_b200.dist import assign_affinity, assign_candidates
-    nc, ng, world = 16, 32, 8                                               # the 8-GPU weak-scaling grid: 16 C x 32 gamma
-    C = np.logspace(-1, 2.5, nc); G = np.geomspace(1 / 4096, 1 / 256, ng)
-    cc, gg = np.meshgrid(C, G, indexing="ij")
-    gd = gg.ravel() * 512
-    cost = np.minimum(4 + 10.3 * (cc.ravel() * gd) ** 0.95, 9 + 7.3 / gd)
-    keys = [("rbf", g) for g in gg.ravel()]
-    parts = assign_affinity(len(cost), world, cost, keys, 7.0)
-    assert sorted(sum(parts, [])) == list(range(len(cost)))
-    groups = [len({keys[c] for c in p}) for p in parts]
-    base = [len({keys[c] for c in p}) for p in assign_candidates(len(cost), world, cost)]
-    assert max(groups) <= 0.6 * max(base)                                   # far fewer gamma groups per rank than cost dealing (~28-32)
-    load = [cost[p].sum() for p in parts]
-    assert max(load) <= 1.10 * min(load)
-    top = np.argsort(-cost)[:world]                                         # the heaviest candidates still land on distinct ranks
-    assert len({r for r, p in enumerate(parts) for c in top if c in p}) == world
-    for n, w in ((7, 3), (6, 4), (5, 8)):                                   # tiny searches: still a partition
-        p = assign_affinity(n, w, np.arange(n, 0, -1.0), list(range(n)), 1.0)
-        assert sorted(sum(p, [])) == list(range(n))
 
 
 # ------------------------------------------------------------------ multi-rank (gloo, CPU) --------
@@ -532,58 +491,6 @@ def test_bench_weak_scaling_grids_keep_64_candidates_per_gpu():
     idx, rel, _ = bench.cpu_sample(w, cands, 16, 0.4)                     # many steps: cheaper tasks, stated in the line
     assert 0.3 <= rel <= 0.5
     assert bench.scaled_workload("c2", 4)["golden"] == "c4_svc_rbf_16x16"    # the N=4 weak grid is config 4: parity asserted in-run
-
-
-def test_simulated_schedule_opt_in(monkeypatch):
-    """B200GS_SCHEDULE=simulate (gs_svc_schedule chosen by simulating the block scheduler; measured no better than the closed
-    form, so opt-in) and the simulator itself (gs_svc_simulate): on the measured
-    iteration counts of configs 2 and 4, on the per-rank shares of the 8-GPU weak-scaling grid and on cost profiles it was
-    not calibrated on.  Properties, not constants: a throughput-bound profile gets no latency tier; a profile with a few
-    dominant problems puts exactly those on clusters; the simulated makespan never exceeds the all-shared schedule's;
-    specialised SMs never exceed the GPU; the simulator reproduces the measured tier timeline of config 2."""
-    import ctypes
-    from spark_sklearn_b200 import engine
-    from spark_sklearn_b200 import dist as D
-    L = engine.load_library()
-    monkeypatch.setenv("B200GS_SCHEDULE", "simulate")
-
-    def sched(cost, sms=148):
-        c = np.sort(np.asarray(cost, float))[::-1].copy()
-        a, b = ctypes.c_int32(), ctypes.c_int32()
-        L.gs_svc_schedule(c.ctypes.data, len(c), sms, ctypes.byref(a), ctypes.byref(b))
-        return a.value, b.value, c
-
-    def makespan(c, nc, ne, sms=148):
-        return L.gs_svc_simulate(c.ctypes.data, len(c), sms, nc, ne)
-
-    _, _, it2 = _golden_svc("c2_svc_rbf_8x8")
-    _, _, it4 = _golden_svc("c4_svc_rbf_16x16")
-    nc, ne, c = sched(it2.ravel())
-    assert 10 <= nc <= 20 and 10 <= ne <= 45 and 4 * nc + ne <= 140           # the 66-68k group on clusters, the 43-48k tier alone
-    assert makespan(c, nc, ne) <= 0.6 * makespan(c, 0, 0)
-    # the simulator's calibration point (148 SMs, B200GS_SMO_TIMELINE, 10 clusters + 35 exclusive): the tiers end at 242 / 255 / 237 ms
-    assert abs(makespan(c, 10, 35) * 1e-3 - 255.0) <= 0.05 * 255.0
-    assert sched(it4.ravel())[:2] == (0, 0)                                    # 1280 problems: throughput-bound
-    assert makespan(np.sort(it4.ravel())[::-1].copy(), 0, 40) > makespan(np.sort(it4.ravel())[::-1].copy(), 0, 0)
-    # a rank of the 8-GPU weak-scaling grid holds two classes of long problems (67k and 54k predicted iterations): both
-    # belong on clusters (the closed form used before left the second class on exclusive SMs, which was slower where the simulator was calibrated)
-    Cs, gs = np.logspace(-1, 2.5, 16), np.geomspace(1 / 4096, 1 / 256, 32)
-    costs = np.array([L.gs_svc_predicted_iterations(1, float(C), float(g), 512) for C in Cs for g in gs])
-    part = D.assign_candidates(len(costs), 8, costs)[0]
-    nc, ne, c = sched(np.repeat(costs[part], 5))
-    assert nc == 15 and c[nc] * 5.45 <= c[0] * 3.55 * 1.1
-    rng = np.random.default_rng(0)
-    for trial in range(20):                                                    # unseen profiles
-        n = int(rng.integers(150, 3000))
-        cost = rng.lognormal(0.0, rng.uniform(0.2, 1.5), n)
-        nc, ne, c = sched(cost)
-        assert 4 * nc + ne <= 140 and nc + ne < n
-        assert makespan(c, nc, ne) <= makespan(c, 0, 0) * (1 + 1e-12)
-    flat = np.ones(2000)
-    assert sched(flat)[:2] == (0, 0)
-    spiky = np.r_[np.full(5, 100.0), np.ones(400)]                             # five dominant problems
-    nc, ne, _ = sched(spiky)
-    assert nc == 5 and ne == 0
 
 
 def test_one_step_pipeline_adapter_translates_names_and_wraps_the_refit(monkeypatch):

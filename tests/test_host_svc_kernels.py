@@ -1,6 +1,6 @@
 """Host-side logic of SVC with the poly and sigmoid kernels (no GPU): parameter checks, per-fold gamma, the degree / coef0
-arrays handed to the engine, kernel-matrix affinity, the engine's kernel-parameter setter calls, and cv_results_ of the
-reference's documented grid through an oracle-backed plan."""
+arrays handed to the engine, the engine's kernel-parameter setter calls, and cv_results_ of the reference's documented
+grid through an oracle-backed plan."""
 import numpy as np
 import pytest
 from sklearn.svm import SVC
@@ -75,20 +75,6 @@ def test_degree_coef0_and_per_fold_gamma_reach_the_engine(fake):
     np.testing.assert_array_equal(call["gamma"][3], 1.0 / X.shape[1])
     np.testing.assert_array_equal(call["gamma"][4], 0.0)
     assert len(set(scale)) > 1
-
-
-def test_affinity_keys_follow_the_parameters_each_kernel_reads(fake):
-    X, y = _data()
-    cands = [{"kernel": "rbf", "degree": 2}, {"kernel": "rbf", "degree": 4}, {"kernel": "rbf", "coef0": 1.0},
-             {"kernel": "poly", "degree": 2}, {"kernel": "poly", "degree": 3}, {"kernel": "poly", "degree": 3, "coef0": 1.0},
-             {"kernel": "sigmoid", "degree": 2}, {"kernel": "sigmoid", "degree": 5}, {"kernel": "sigmoid", "coef0": 1.0},
-             {"kernel": "linear", "degree": 7, "coef0": 2.0}, {"kernel": "linear"}]
-    plan, _ = _plan(SVC(gamma=0.5), cands, X, y)
-    k = plan.affinity()
-    assert k[0] == k[1] == k[2] == ("rbf", 0.5)                    # rbf ignores degree and coef0: one kernel matrix
-    assert len({k[3], k[4], k[5]}) == 3
-    assert k[6] == k[7] != k[8]                                     # sigmoid ignores degree
-    assert k[9] == k[10] == ("linear", 0.0)
 
 
 @pytest.mark.parametrize("bad", [{"degree": -1}, {"degree": 2.0}, {"degree": "3"}, {"coef0": "1"}, {"coef0": None},

@@ -13,7 +13,7 @@ est = WL.make_estimator(w); X, y = w["X"], w["y"]; cands = WL.candidates(w)
 splits = list(check_cv(w["cv"], y, classifier=is_classifier(est)).split(X, y))
 fold_id = fold_ids_from_splits(splits, len(y))
 plan = adapter_for(est).plan(est, cands, X, y, fold_id, len(splits))
-parts = D.assign_for_plan(plan, len(cands), n_gpus)      # B200GS_DEAL=groups tries the affinity dealing
+parts = D.assign_for_plan(plan, len(cands), n_gpus)
 for r in ranks:
     for rep in range(3):
         out = plan.evaluate(parts[r], return_train=True); p = plan.profile()
