@@ -229,8 +229,30 @@ int gs_linsvc_refit(gs_handle *h, double C, double tol, int32_t max_iter, int32_
 /* S_out [n][n] float64 Gram X X^T and xsq_out [n] (either may be NULL), in ORIGINAL row order.  */
 int gs_debug_gram(gs_handle *h, double *S_out, double *xsq_out);
 /* K_out [n][n] float32 kernel matrix (the SMO solver's Q without the y_i*y_j sign), original order; poly / sigmoid take
- * degree and coef0 from gs_set_kernel_params (n = 1). */
-int gs_debug_kernel_matrix(gs_handle *h, int32_t kernel, double gamma, float *K_out);
+ * degree and coef0 from gs_set_kernel_params (n = 1).  Optional outputs (NULL: not computed): qd_out [n] the float64
+ * diagonal k(x_r, x_r) the solver reads (poly / sigmoid only, GS_ERR_ARG for the other kernels); *special_out the guard
+ * flag that sends a search to the general SMO instance: 1 when K holds a zero, a subnormal, a negative or a non-finite
+ * value, else 0. */
+int gs_debug_kernel_matrix(gs_handle *h, int32_t kernel, double gamma, float *K_out, double *qd_out, int32_t *special_out);
+/* dec_out [ncols][n] = sum_j k64(r, j) coef[c][j], the float64 decision values of the SVC / SVR scorers (kernel recomputed
+ * in float64 from the Gram; rows r, j in original order).  jchunks = 0: the search's own split of the support rows into
+ * slabs, reported in *jchunks_used (may be NULL); 1..64: that many slabs. */
+int gs_debug_decision(gs_handle *h, int32_t kernel, double gamma, int32_t degree, double coef0, const double *coef, int32_t ncols,
+                      int32_t jchunks, double *dec_out, int32_t *jchunks_used);
+/* One scorer kernel on the dataset's labels / targets and splits.  dec [ncols][n] decision values (original row order),
+ * rho [ncols] (unused by the AUC kinds); task t reads the columns from first_col[t] (n_classes (n_classes - 1) / 2 of them
+ * for the vote kinds, one otherwise) with split fold[t].  out, per task:
+ *   GS_DEBUG_SCORE_VOTE          int32 [4] = {test correct, test rows, training correct, training rows}
+ *   GS_DEBUG_SCORE_CLASS_COUNTS  int32 [2 (test, training)][n_classes][3 = support, true positives, predicted]
+ *   GS_DEBUG_SCORE_AUC_F64       uint64 [4] = {test wins, test ties, training wins, training ties} of the pairs (row of class
+ *                                1, row of class 0) on -dec (the SVC search's sign); two classes
+ *   GS_DEBUG_SCORE_AUC_F32       the same on (float)dec, sign +1 (LogisticRegression's float32 z)
+ *   GS_DEBUG_SCORE_RSS           float64 [2] = residual sums of squares sum (z - (dec - rho))^2 over the test / training rows
+ *                                (regression dataset after gs_set_targets_f64) */
+enum { GS_DEBUG_SCORE_VOTE = 0, GS_DEBUG_SCORE_CLASS_COUNTS = 1, GS_DEBUG_SCORE_AUC_F64 = 2, GS_DEBUG_SCORE_AUC_F32 = 3,
+       GS_DEBUG_SCORE_RSS = 4 };
+int gs_debug_score(gs_handle *h, int32_t kind, const double *dec, const double *rho, int32_t ncols, const int32_t *first_col,
+                   const int32_t *fold, int32_t n_tasks, void *out);
 
 /* C[M][N] = sum_k A[M][k]*B[N][k] on the wgmma tensor-core path (3xTF32 split), host fp32 row-major in/out. */
 int gs_debug_gemm_nt(gs_handle *h, const float *A, int32_t M, const float *B, int32_t N, int32_t K, float *C);

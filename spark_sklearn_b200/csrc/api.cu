@@ -841,24 +841,165 @@ int gs_debug_gram(gs_handle *h, double *S_out, double *xsq_out)
     return GS_OK;
 }
 
-int gs_debug_kernel_matrix(gs_handle *h, int32_t kernel, double gamma, float *K_out)
+int gs_debug_kernel_matrix(gs_handle *h, int32_t kernel, double gamma, float *K_out, double *qd_out, int32_t *special_out)
 {
     if (!h || !K_out) return GS_ERR_ARG;
     if (kernel < GS_KERNEL_LINEAR || kernel > GS_KERNEL_SIGMOID) { gs_set_error(h, "gs_debug_kernel_matrix: unsupported kernel id"); return GS_ERR_UNSUPPORTED; }
     if (h->kp_degree.size() > 1) { gs_set_error(h, "gs_debug_kernel_matrix: gs_set_kernel_params was given more than one candidate"); return GS_ERR_ARG; }
     const KernelSpec ks(kernel, gamma, h->kp_degree.empty() ? 3 : h->kp_degree[0], h->kp_coef0.empty() ? 0.0 : h->kp_coef0[0]);
+    if (qd_out && !ks.has_qd()) { gs_set_error(h, "gs_debug_kernel_matrix: qd_out is only computed for the poly and sigmoid kernels"); return GS_ERR_ARG; }
     int st = gs_debug_gram(h, nullptr, nullptr);
     if (st) return st;
     const int n = (int)h->n;
     const int64_t ldk = ((int64_t)n + 31) & ~31LL;
-    GS_CUDA(h->dK.reserve((size_t)n * ldk * 4));
+    const size_t kbytes = (size_t)n * ldk * 4;
+    GS_CUDA(h->dK.reserve(kbytes + (qd_out ? (size_t)n * 8 : 0)));
+    double *d_qd = qd_out ? (double *)(h->dK.as<char>() + kbytes) : nullptr;      // as SvmSearch lays it out: behind K
+    int *d_special = nullptr;
+    if (special_out) {
+        GS_CUDA(h->dWork[7].reserve(64));
+        GS_CUDA(cudaMemsetAsync(h->dWork[7].p, 0, 4, h->stream));
+        d_special = h->dWork[7].as<int>();
+    }
     GS_CUDA(launch_kernel_matrix(h->dS.as<double>(), h->dXsq.as<double>(), n, ks.kernel, ks.gamma, ks.degree, ks.coef0, h->dK.as<float>(),
-                                 ldk, nullptr, nullptr, h->stream));
+                                 ldk, d_qd, d_special, h->stream));
     std::vector<float> K((size_t)n * ldk);
+    std::vector<double> qd(qd_out ? n : 0);
+    int32_t special = 0;
     GS_CUDA(cudaMemcpyAsync(K.data(), h->dK.p, K.size() * 4, cudaMemcpyDeviceToHost, h->stream));
+    if (qd_out) GS_CUDA(cudaMemcpyAsync(qd.data(), d_qd, qd.size() * 8, cudaMemcpyDeviceToHost, h->stream));
+    if (special_out) GS_CUDA(cudaMemcpyAsync(&special, d_special, 4, cudaMemcpyDeviceToHost, h->stream));
     GS_CUDA(cudaStreamSynchronize(h->stream));
     for (int r = 0; r < n; r++)
         for (int c = 0; c < n; c++) K_out[(size_t)h->perm[r] * n + h->perm[c]] = K[(size_t)r * ldk + c];
+    if (qd_out)
+        for (int r = 0; r < n; r++) qd_out[h->perm[r]] = qd[r];
+    if (special_out) *special_out = special;
+    return GS_OK;
+}
+
+int gs_debug_decision(gs_handle *h, int32_t kernel, double gamma, int32_t degree, double coef0, const double *coef, int32_t ncols,
+                      int32_t jchunks, double *dec_out, int32_t *jchunks_used)
+{
+    if (!h) return GS_ERR_ARG;
+    if (h->n == 0) { gs_set_error(h, "gs_debug_decision: no dataset"); return GS_ERR_NO_DATA; }
+    if (kernel < GS_KERNEL_LINEAR || kernel > GS_KERNEL_SIGMOID) { gs_set_error(h, "gs_debug_decision: unsupported kernel id"); return GS_ERR_UNSUPPORTED; }
+    if (!coef || !dec_out || ncols < 1 || jchunks < 0 || jchunks > 64 || degree < 0 || !std::isfinite(gamma) || !std::isfinite(coef0)) {
+        gs_set_error(h, "gs_debug_decision: bad arguments (1..64 slabs or 0 for the search's choice)"); return GS_ERR_ARG;
+    }
+    GS_CUDA(cudaSetDevice(h->device));
+    cudaStream_t st = h->stream;
+    const int n = (int)h->n;
+    const KernelSpec ks(kernel, gamma, degree, coef0);
+    if (const int rc = build_gram(h, 0, st)) return rc;
+    const int jc = jchunks == 0 ? decision_chunks(n, ncols, h->sm_count) : jchunks;
+    const size_t cells = (size_t)ncols * n;
+    std::vector<double> buf(cells);
+    for (int c = 0; c < ncols; c++)
+        for (int r = 0; r < n; r++) buf[(size_t)c * n + r] = coef[(size_t)c * n + h->perm[r]];
+    // the buffers SvmSearch::decisions uses: coef columns, decision columns, slab partial sums
+    GS_CUDA(h->dWork[3].reserve(cells * 8));
+    GS_CUDA(h->dWork[4].reserve(cells * 8));
+    if (jc > 1) GS_CUDA(h->dWork[8].reserve(cells * jc * 8));
+    GS_CUDA(cudaMemcpyAsync(h->dWork[3].p, buf.data(), cells * 8, cudaMemcpyHostToDevice, st));
+    GS_CUDA(launch_decision(h->dS.as<double>(), h->dXsq.as<double>(), n, ks.kernel, ks.gamma, ks.degree, ks.coef0, h->dWork[3].as<double>(),
+                            ncols, h->dWork[4].as<double>(), jc > 1 ? h->dWork[8].as<double>() : nullptr, jc, st));
+    GS_CUDA(cudaMemcpyAsync(buf.data(), h->dWork[4].p, cells * 8, cudaMemcpyDeviceToHost, st));
+    GS_CUDA(cudaStreamSynchronize(st));
+    for (int c = 0; c < ncols; c++)
+        for (int r = 0; r < n; r++) dec_out[(size_t)c * n + h->perm[r]] = buf[(size_t)c * n + r];
+    if (jchunks_used) *jchunks_used = jc;
+    return GS_OK;
+}
+
+int gs_debug_score(gs_handle *h, int32_t kind, const double *dec, const double *rho, int32_t ncols, const int32_t *first_col,
+                   const int32_t *fold, int32_t n_tasks, void *out)
+{
+    if (!h) return GS_ERR_ARG;
+    if (h->n == 0) { gs_set_error(h, "gs_debug_score: no dataset"); return GS_ERR_NO_DATA; }
+    if (kind < GS_DEBUG_SCORE_VOTE || kind > GS_DEBUG_SCORE_RSS) { gs_set_error(h, "gs_debug_score: unknown kind"); return GS_ERR_ARG; }
+    const bool auc = kind == GS_DEBUG_SCORE_AUC_F64 || kind == GS_DEBUG_SCORE_AUC_F32;
+    if (!dec || (!rho && !auc) || !first_col || !fold || !out || ncols < 1 || n_tasks < 1) {
+        gs_set_error(h, "gs_debug_score: bad arguments"); return GS_ERR_ARG;
+    }
+    const int nc = h->n_classes;
+    int n_pairs = 1;
+    if (kind == GS_DEBUG_SCORE_RSS) {
+        if (h->classification || h->z64.empty()) { gs_set_error(h, "gs_debug_score: RSS needs a regression dataset and gs_set_targets_f64"); return GS_ERR_NO_DATA; }
+    } else {
+        if (!h->classification) { gs_set_error(h, "gs_debug_score: this scorer needs class labels"); return GS_ERR_ARG; }
+        if (nc < 2 || nc > 32) { gs_set_error(h, "gs_debug_score: the vote kernels take 2..32 classes"); return GS_ERR_UNSUPPORTED; }
+        if (auc && nc != 2) { gs_set_error(h, "gs_debug_score: AUC pair counts need two classes"); return GS_ERR_ARG; }
+        if (!auc) n_pairs = nc * (nc - 1) / 2;
+    }
+    for (int t = 0; t < n_tasks; t++)
+        if (first_col[t] < 0 || first_col[t] > ncols - n_pairs || fold[t] < 0 || fold[t] >= h->n_splits) {
+            gs_set_error(h, "gs_debug_score: task " + std::to_string(t) + " reads a column or a split that does not exist");
+            return GS_ERR_ARG;
+        }
+    GS_CUDA(cudaSetDevice(h->device));
+    cudaStream_t st = h->stream;
+    const int n = (int)h->n;
+    const size_t cells = (size_t)ncols * n;
+    GS_CUDA(h->dWork[4].reserve(cells * 8));
+    if (kind == GS_DEBUG_SCORE_AUC_F32) {                       // LogisticRegression's float32 decision values
+        std::vector<float> s(cells);
+        for (int c = 0; c < ncols; c++)
+            for (int r = 0; r < n; r++) s[(size_t)c * n + r] = (float)dec[(size_t)c * n + h->perm[r]];
+        GS_CUDA(cudaMemcpyAsync(h->dWork[4].p, s.data(), cells * 4, cudaMemcpyHostToDevice, st));
+        GS_CUDA(cudaStreamSynchronize(st));
+    } else {
+        std::vector<double> s(cells);
+        for (int c = 0; c < ncols; c++)
+            for (int r = 0; r < n; r++) s[(size_t)c * n + r] = dec[(size_t)c * n + h->perm[r]];
+        GS_CUDA(cudaMemcpyAsync(h->dWork[4].p, s.data(), cells * 8, cudaMemcpyHostToDevice, st));
+        GS_CUDA(cudaStreamSynchronize(st));
+    }
+    // rho [ncols], then VoteTask [n_tasks] (the AUC kernels: the column list, then the fold list -- the same 8 bytes per task)
+    GS_CUDA(h->dWork[5].reserve((size_t)ncols * 8 + (size_t)n_tasks * sizeof(VoteTask)));
+    double *d_rho = h->dWork[5].as<double>();
+    int *d_meta = (int *)(d_rho + ncols);
+    if (rho) GS_CUDA(cudaMemcpyAsync(d_rho, rho, (size_t)ncols * 8, cudaMemcpyHostToDevice, st));
+    static_assert(sizeof(VoteTask) == 2 * sizeof(int), "VoteTask is {first_col, fold}");
+    std::vector<int> meta((size_t)n_tasks * 2);
+    for (int t = 0; t < n_tasks; t++) {
+        if (auc) { meta[t] = first_col[t]; meta[(size_t)n_tasks + t] = fold[t]; }
+        else { meta[(size_t)t * 2] = first_col[t]; meta[(size_t)t * 2 + 1] = fold[t]; }
+    }
+    GS_CUDA(cudaMemcpyAsync(d_meta, meta.data(), meta.size() * 4, cudaMemcpyHostToDevice, st));
+    GS_CUDA(cudaStreamSynchronize(st));                          // meta is a local: copied before it goes
+    size_t per_task = 0;
+    switch (kind) {
+    case GS_DEBUG_SCORE_VOTE: per_task = 4 * 4; break;
+    case GS_DEBUG_SCORE_CLASS_COUNTS: per_task = (size_t)2 * nc * 3 * 4; break;
+    case GS_DEBUG_SCORE_RSS: per_task = 2 * 8; break;
+    default: per_task = 4 * 8; break;
+    }
+    const size_t out_bytes = per_task * n_tasks;
+    GS_CUDA(h->dScore.reserve(out_bytes));
+    GS_CUDA(cudaMemsetAsync(h->dScore.p, 0, out_bytes, st));
+    const VoteTask *d_vt = (const VoteTask *)d_meta;
+    switch (kind) {
+    case GS_DEBUG_SCORE_VOTE:
+        GS_CUDA(launch_vote(h->dWork[4].as<double>(), d_rho, n, nc, h->dY.as<int>(), h->masks(), d_vt, n_tasks, h->dScore.as<int>(), st));
+        break;
+    case GS_DEBUG_SCORE_CLASS_COUNTS:
+        GS_CUDA(launch_vote_classes(h->dWork[4].as<double>(), d_rho, n, nc, h->dY.as<int>(), h->masks(), d_vt, n_tasks, h->dScore.as<int>(), st));
+        break;
+    case GS_DEBUG_SCORE_AUC_F64:                                 // as the SVC search: libsvm's dec - rho, positive = first class
+        GS_CUDA(launch_auc_pairs_f64(h->dWork[4].as<double>(), n, n, h->class_start[1], h->masks(), d_meta, d_meta + n_tasks, n_tasks,
+                                     -1, h->dScore.as<unsigned long long>(), st));
+        break;
+    case GS_DEBUG_SCORE_AUC_F32:                                 // as LogisticRegression: larger z = the second class
+        GS_CUDA(launch_auc_pairs_f32(h->dWork[4].as<float>(), n, n, h->class_start[1], h->masks(), d_meta, d_meta + n_tasks, n_tasks,
+                                     +1, h->dScore.as<unsigned long long>(), st));
+        break;
+    default:
+        GS_CUDA(launch_rss(h->dWork[4].as<double>(), d_rho, n, h->dZ64.as<double>(), h->masks(), d_vt, n_tasks, h->dScore.as<double>(), st));
+        break;
+    }
+    GS_CUDA(cudaMemcpyAsync(out, h->dScore.p, out_bytes, cudaMemcpyDeviceToHost, st));
+    GS_CUDA(cudaStreamSynchronize(st));
     return GS_OK;
 }
 

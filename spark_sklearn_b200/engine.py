@@ -79,7 +79,9 @@ def load_library():
     L.gs_debug_gemm_f64.argtypes = [vp, vp, i32, vp, i32, i32, vp]
     L.gs_get_profile.argtypes = [vp, c.POINTER(GsProfile)]
     L.gs_debug_gram.argtypes = [vp, vp, vp]
-    L.gs_debug_kernel_matrix.argtypes = [vp, i32, dbl, vp]
+    L.gs_debug_kernel_matrix.argtypes = [vp, i32, dbl, vp, vp, vp]
+    L.gs_debug_decision.argtypes = [vp, i32, dbl, i32, dbl, vp, i32, i32, vp, vp]
+    L.gs_debug_score.argtypes = [vp, i32, vp, vp, i32, vp, vp, i32, vp]
     L.gs_debug_gemm_nt.argtypes = [vp, vp, i32, vp, i32, i32, vp]
     L.gs_svc_predicted_iterations.argtypes = [i32, dbl, dbl, i32]
     L.gs_svc_predicted_iterations.restype = dbl
@@ -90,7 +92,7 @@ def load_library():
     for f in ("gs_create", "gs_set_data", "gs_svc", "gs_svc_refit", "gs_ridge", "gs_ridge_refit", "gs_enet", "gs_enet_refit", "gs_set_targets_f64",
               "gs_svr", "gs_svr_refit", "gs_logreg",
               "gs_logreg_refit", "gs_linsvc", "gs_linsvc_refit", "gs_get_profile", "gs_debug_gram", "gs_debug_kernel_matrix",
-              "gs_debug_gemm_nt", "gs_debug_gemm_f64"):
+              "gs_debug_decision", "gs_debug_score", "gs_debug_gemm_nt", "gs_debug_gemm_f64"):
         getattr(L, f).restype = c.c_int
     _lib = L
     return L
@@ -343,12 +345,54 @@ class Engine:
         self._check(self._L.gs_debug_gram(self._h, _ptr(S), _ptr(xsq)))
         return S, xsq
 
-    def debug_kernel_matrix(self, kernel, gamma, degree=3, coef0=0.0):
+    def debug_kernel_matrix(self, kernel, gamma, degree=3, coef0=0.0, return_guard=False):
+        """K [n][n] float32; with return_guard: (K, qd, flag), qd the float64 diagonal (poly / sigmoid, else None) and flag
+        the kernel-matrix kernel's guard (1: K holds a zero, subnormal, negative or non-finite value)"""
         K = np.zeros((self.n, self.n), np.float32)
         k = KERNEL_ID[kernel] if isinstance(kernel, str) else int(kernel)
-        self._with_kernel_params([k], degree, coef0,
-                                 lambda: self._check(self._L.gs_debug_kernel_matrix(self._h, k, float(gamma), _ptr(K))))
-        return K
+        qd = np.zeros(self.n) if return_guard and k in _PARAM_KERNELS else None
+        flag = np.zeros(1, np.int32) if return_guard else None
+        self._with_kernel_params([k], degree, coef0, lambda: self._check(self._L.gs_debug_kernel_matrix(
+            self._h, k, float(gamma), _ptr(K), _ptr(qd), _ptr(flag))))
+        return (K, qd, int(flag[0])) if return_guard else K
+
+    def debug_decision(self, kernel, gamma, coef, degree=3, coef0=0.0, jchunks=0):
+        """coef [ncols][n] -> (dec [ncols][n] float64 decision values, slab count used); jchunks 0 = the search's choice"""
+        coef = np.ascontiguousarray(np.atleast_2d(coef), np.float64)
+        if coef.shape[1] != self.n:
+            raise ValueError("debug_decision: coef has %d columns; expected n = %d" % (coef.shape[1], self.n))
+        dec = np.zeros_like(coef)
+        used = np.zeros(1, np.int32)
+        k = KERNEL_ID[kernel] if isinstance(kernel, str) else int(kernel)
+        self._check(self._L.gs_debug_decision(self._h, k, float(gamma), int(degree), float(coef0), _ptr(coef), coef.shape[0],
+                                              int(jchunks), _ptr(dec), _ptr(used)))
+        return dec, int(used[0])
+
+    SCORE_KINDS = {"vote": 0, "class_counts": 1, "auc_f64": 2, "auc_f32": 3, "rss": 4}
+
+    def debug_score(self, kind, dec, rho, first_col, fold):
+        """One scorer kernel (include/b200gs.h gs_debug_score) on dec [ncols][n] and rho [ncols] for the tasks
+        (first_col[t], fold[t]) -> vote [t][4] int32, class_counts [t][2][n_classes][3] int32, auc_f64 / auc_f32 [t][4]
+        uint64, rss [t][2] float64"""
+        k = self.SCORE_KINDS[kind]
+        dec = np.ascontiguousarray(np.atleast_2d(dec), np.float64)
+        rho = None if rho is None else np.ascontiguousarray(rho, np.float64)
+        first_col = np.ascontiguousarray(first_col, np.int32)
+        fold = np.ascontiguousarray(fold, np.int32)
+        t = len(first_col)
+        if fold.shape != (t,) or dec.shape[1] != self.n or (rho is not None and rho.shape != (dec.shape[0],)):
+            raise ValueError("debug_score: first_col / fold / dec / rho shapes disagree")
+        if kind == "vote":
+            out = np.zeros((t, 4), np.int32)
+        elif kind == "class_counts":
+            out = np.zeros((t, 2, self.n_classes, 3), np.int32)
+        elif kind == "rss":
+            out = np.zeros((t, 2))
+        else:
+            out = np.zeros((t, 4), np.uint64)
+        self._check(self._L.gs_debug_score(self._h, k, _ptr(dec), _ptr(rho), dec.shape[0], _ptr(first_col), _ptr(fold), t,
+                                           _ptr(out)))
+        return out
 
     def debug_gemm_nt(self, A, B):
         A = np.ascontiguousarray(A, np.float32)

@@ -137,6 +137,41 @@ def test_engine_sets_kernel_params_only_for_poly_and_sigmoid():
     assert eng._L.calls[0][1][3] == 1
 
 
+def test_engine_debug_kernel_matrix_guard_outputs():
+    """debug_kernel_matrix asks for the float64 diagonal (poly / sigmoid only) and the guard flag only with return_guard"""
+    eng = _engine()
+    K = eng.debug_kernel_matrix("rbf", 0.5)
+    assert K.shape == (10, 10)
+    (name, args), = eng._L.calls
+    assert name == "gs_debug_kernel_matrix" and len(args) == 6 and args[4:] == (None, None)
+    for kernel, with_qd in (("rbf", False), ("linear", False), ("poly", True), ("sigmoid", True)):
+        eng = _engine()
+        K, qd, flag = eng.debug_kernel_matrix(kernel, 0.5, return_guard=True)
+        (args,) = [a for name, a in eng._L.calls if name == "gs_debug_kernel_matrix"]
+        assert (args[4] is not None) == with_qd and args[5] is not None, kernel
+        assert K.shape == (10, 10) and flag == 0 and (qd.shape == (10,) if with_qd else qd is None), kernel
+
+
+def test_engine_debug_score_and_decision_arguments():
+    eng = _engine()
+    eng.n_classes = 3
+    for kind, shape, dtype in (("vote", (4, 4), np.int32), ("class_counts", (4, 2, 3, 3), np.int32),
+                               ("auc_f64", (4, 4), np.uint64), ("auc_f32", (4, 4), np.uint64), ("rss", (4, 2), np.float64)):
+        out = eng.debug_score(kind, np.zeros((3, 10)), np.zeros(3), [0, 0, 0, 0], [0, 1, 0, 1])
+        assert out.shape == shape and out.dtype == dtype, kind
+        name, args = eng._L.calls[-1]
+        assert name == "gs_debug_score" and args[1] == eng.SCORE_KINDS[kind] and args[4] == 3 and args[7] == 4
+    with pytest.raises(ValueError):
+        eng.debug_score("vote", np.zeros((3, 10)), np.zeros(3), [0, 0], [0])
+    with pytest.raises(ValueError):
+        eng.debug_score("vote", np.zeros((3, 9)), np.zeros(3), [0], [0])
+    dec, used = eng.debug_decision("poly", 0.5, np.zeros((5, 10)), degree=4, coef0=-1.0, jchunks=3)
+    name, args = eng._L.calls[-1]
+    assert name == "gs_debug_decision" and dec.shape == (5, 10) and args[1:5] == (2, 0.5, 4, -1.0) and args[6:8] == (5, 3)
+    with pytest.raises(ValueError):
+        eng.debug_decision("rbf", 0.5, np.zeros((5, 9)))
+
+
 def test_randomized_search_over_degree(fake):
     from scipy.stats import randint
     from sklearn.model_selection import ParameterSampler
