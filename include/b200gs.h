@@ -225,7 +225,40 @@ int gs_linsvc(gs_handle *h, int32_t n_cand, const double *C, double tol, int32_t
 int gs_linsvc_refit(gs_handle *h, double C, double tol, int32_t max_iter, int32_t fit_intercept, double intercept_scaling,
                     double *coef_out, int32_t *n_iter);
 
+/*
+ * k-nearest neighbours (replaces KNeighborsClassifier / KNeighborsRegressor .fit/score: a fit stores its training rows,
+ * the scorer's predict runs scikit-learn's brute-force ArgKmin, sklearn/metrics/_pairwise_distances_reduction, and the
+ * vote of neighbors/_classification.py, _regression.py, _base.py _get_weights).  n_neighbors[n_cand]
+ * (1..GS_KNN_MAX_NEIGHBORS), weights[n_cand] (GS_KNN_UNIFORM, GS_KNN_DISTANCE), metric[n_cand] (GS_KNN_EUCLIDEAN,
+ * GS_KNN_MANHATTAN).  For each metric present the call computes the distances once, in row slabs (no n x n matrix is
+ * kept): Euclidean orders by scikit-learn's surrogate xsq[c] - 2 x_r.x_c (float64) and its distance is
+ * sqrt(max(surrogate + xsq[r], 0)) (float32 X: both rounded to float32, as EuclideanDistance32 does), a row's distance
+ * to itself being exactly 0; Manhattan is the float64 sum of the differences rounded in X's dtype, in feature order,
+ * then rounded to X's dtype (ManhattanDistance32/64.dist).  One selection per metric then keeps, for every evaluated
+ * row and split, the K_max = max n_neighbors nearest training rows sorted by (key, original row index): an exact tie
+ * goes to the lower index (scikit-learn's ArgKmin heap usually, but not always, keeps the same rows).  Every candidate
+ * votes from those lists: uniform (proba = count / k) or 1 / distance (the indicator of zero distance when a neighbour
+ * is at distance 0; sums in numpy's pairwise order), prediction = first arg-max; regressor: mean of the neighbours' y
+ * (float32 when flags has GS_TARGET_F32: numpy keeps float32 y) or sum w y / sum w in float64.  Classifier: labels from
+ * gs_set_data, up to 64 classes, every gs_set_scoring classifier scorer (roc_auc: binary, on predict_proba[:, 1]).
+ * Regressor: float64 targets from gs_set_targets_f64, r2 / GS_SCORE_NEG_MSE / GS_SCORE_NEG_RMSE.  Splits: fold ids or
+ * gs_set_splits masks; flags GS_RETURN_TRAIN also scores every split's training rows.  A task whose n_neighbors exceeds
+ * its split's training rows scores NaN (scikit-learn's kneighbors raises ValueError).  Sample and class weights are
+ * rejected.  fit_ms / score_ms (may be NULL): the call's distance + selection time and its vote time, each divided
+ * evenly over the tasks.  gs_profile: ms_gram the distances, ms_solve the selection, ms_score votes and scorers.
+ */
+enum { GS_KNN_UNIFORM = 0, GS_KNN_DISTANCE = 1 };
+enum { GS_KNN_EUCLIDEAN = 0, GS_KNN_MANHATTAN = 1 };
+enum { GS_KNN_MAX_NEIGHBORS = 256 };
+enum { GS_TARGET_F32 = 8 };          /* gs_knn flag: the regression targets are float32 */
+int gs_knn(gs_handle *h, int32_t n_cand, const int32_t *n_neighbors, const int32_t *weights, const int32_t *metric,
+           uint32_t flags, double *test_scores, double *train_scores, float *fit_ms, float *score_ms);
+
 /* ---- test hooks (used by tests/ to localise a parity failure to one kernel) ---------------- */
+/* The sorted neighbour lists gs_knn votes from, for every row (original order) against the training rows of split `split`:
+ * idx_out [n][k] original row indices (-1 past the split's training rows), dist_out [n][k] distances (+inf there); either
+ * may be NULL.  metric: GS_KNN_EUCLIDEAN or GS_KNN_MANHATTAN; 1 <= k <= GS_KNN_MAX_NEIGHBORS. */
+int gs_debug_knn_neighbors(gs_handle *h, int32_t metric, int32_t k, int32_t split, int32_t *idx_out, double *dist_out);
 /* S_out [n][n] float64 Gram X X^T and xsq_out [n] (either may be NULL), in ORIGINAL row order.  */
 int gs_debug_gram(gs_handle *h, double *S_out, double *xsq_out);
 /* K_out [n][n] float32 kernel matrix (the SMO solver's Q without the y_i*y_j sign), original order; poly / sigmoid take

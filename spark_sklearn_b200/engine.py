@@ -11,7 +11,9 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libb200gs.so")
 
-GS_RETURN_TRAIN, GS_GRAM_TENSOR, GS_NO_SHRINKING = 1, 2, 4
+GS_RETURN_TRAIN, GS_GRAM_TENSOR, GS_NO_SHRINKING, GS_TARGET_F32 = 1, 2, 4, 8
+KNN_WEIGHTS = {"uniform": 0, "distance": 1}
+KNN_METRIC = {"euclidean": 0, "manhattan": 1}
 KERNEL_ID = {"linear": 0, "rbf": 1, "poly": 2, "sigmoid": 3}
 _PARAM_KERNELS = (2, 3)            # the kernels that read degree / coef0 (gs_set_kernel_params)
 
@@ -77,6 +79,8 @@ def load_library():
     L.gs_linsvc.argtypes = [vp, i32, vp, dbl, i32, i32, dbl, u32, vp, vp, vp, vp, vp]
     L.gs_linsvc_refit.argtypes = [vp, dbl, dbl, i32, i32, dbl, vp, vp]
     L.gs_debug_gemm_f64.argtypes = [vp, vp, i32, vp, i32, i32, vp]
+    L.gs_knn.argtypes = [vp, i32, vp, vp, vp, u32, vp, vp, vp, vp]
+    L.gs_debug_knn_neighbors.argtypes = [vp, i32, i32, i32, vp, vp]
     L.gs_get_profile.argtypes = [vp, c.POINTER(GsProfile)]
     L.gs_debug_gram.argtypes = [vp, vp, vp]
     L.gs_debug_kernel_matrix.argtypes = [vp, i32, dbl, vp, vp, vp]
@@ -92,7 +96,7 @@ def load_library():
     for f in ("gs_create", "gs_set_data", "gs_svc", "gs_svc_refit", "gs_ridge", "gs_ridge_refit", "gs_enet", "gs_enet_refit", "gs_set_targets_f64",
               "gs_svr", "gs_svr_refit", "gs_logreg",
               "gs_logreg_refit", "gs_linsvc", "gs_linsvc_refit", "gs_get_profile", "gs_debug_gram", "gs_debug_kernel_matrix",
-              "gs_debug_decision", "gs_debug_score", "gs_debug_gemm_nt", "gs_debug_gemm_f64"):
+              "gs_debug_decision", "gs_debug_score", "gs_debug_gemm_nt", "gs_debug_gemm_f64", "gs_knn", "gs_debug_knn_neighbors"):
         getattr(L, f).restype = c.c_int
     _lib = L
     return L
@@ -338,7 +342,32 @@ class Engine:
                                             float(intercept_scaling), _ptr(raw), _ptr(it)))
         return raw, it
 
+    def knn(self, n_neighbors, weights, metric, return_train=True, y_f32=False):
+        """k-NN scores per (candidate, split) from one neighbour selection per metric (include/b200gs.h gs_knn); weights and
+        metric are names (KNN_WEIGHTS, KNN_METRIC) or codes.  NaN where n_neighbors exceeds the split's training rows."""
+        nn = np.ascontiguousarray(n_neighbors, np.int32)
+        w = np.ascontiguousarray([KNN_WEIGHTS[v] if isinstance(v, str) else int(v) for v in weights], np.int32)
+        m = np.ascontiguousarray([KNN_METRIC[v] if isinstance(v, str) else int(v) for v in metric], np.int32)
+        shape = (len(nn), self.n_splits)
+        out = dict(test=np.zeros(shape), train=np.zeros(shape), fit_ms=np.zeros(shape, np.float32),
+                   score_ms=np.zeros(shape, np.float32))
+        fl = (GS_RETURN_TRAIN if return_train else 0) | (GS_TARGET_F32 if y_f32 else 0)
+        self._check(self._L.gs_knn(self._h, len(nn), _ptr(nn), _ptr(w), _ptr(m), fl, _ptr(out["test"]), _ptr(out["train"]),
+                                   _ptr(out["fit_ms"]), _ptr(out["score_ms"])))
+        if not return_train:
+            out["train"] = None
+        return out
+
     # -- test hooks --
+    def debug_knn_neighbors(self, metric, k, split):
+        """-> (idx [n][k] original row indices, -1 past the split's training rows; dist [n][k]): the sorted neighbour lists
+        gs_knn votes from, every row against the training rows of split `split`"""
+        idx = np.zeros((self.n, k), np.int32)
+        dist = np.zeros((self.n, k))
+        m = KNN_METRIC[metric] if isinstance(metric, str) else int(metric)
+        self._check(self._L.gs_debug_knn_neighbors(self._h, m, int(k), int(split), _ptr(idx), _ptr(dist)))
+        return idx, dist
+
     def debug_gram(self):
         S = np.zeros((self.n, self.n))
         xsq = np.zeros(self.n)

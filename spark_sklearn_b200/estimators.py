@@ -4,7 +4,7 @@ and turn refit buffers back into genuine fitted scikit-learn estimators for ``be
 
 Only estimators with a CUDA path are accepted (SVC with the linear, rbf, poly and sigmoid kernels, SVR rbf/linear, Ridge,
 Lasso / ElasticNet, LogisticRegression, LinearSVC with the primal squared-hinge solver -- the families the reference ships
-examples for); anything else raises: no CPU fallback.
+examples for -- and KNeighborsClassifier / KNeighborsRegressor); anything else raises: no CPU fallback.
 """
 import numbers
 import warnings
@@ -94,6 +94,7 @@ class Folds:
 
 def adapter_for(estimator):
     from sklearn.linear_model import ElasticNet, Lasso, LogisticRegression, Ridge
+    from sklearn.neighbors import KNeighborsClassifier, KNeighborsRegressor
     from sklearn.pipeline import Pipeline
     from sklearn.svm import SVC, SVR, LinearSVC
     t = type(estimator)
@@ -109,13 +110,16 @@ def adapter_for(estimator):
         return ENetAdapter
     if t is LinearSVC:
         return LinearSVCAdapter
+    if t in (KNeighborsClassifier, KNeighborsRegressor):
+        return KNeighborsAdapter if t is KNeighborsClassifier else KNeighborsRegressorAdapter
     if t is Pipeline and len(estimator.steps) == 1:
         # the reference's own search tests wrap the estimator in a one-step Pipeline and search 'step__param'
         # (python/spark_sklearn/tests/test_search_2.py:69-93): the step's adapter runs, the names are translated
         return PipelineAdapter(estimator.steps[0][0], adapter_for(estimator.steps[0][1]))
     raise NotImplementedError(
-        "spark_sklearn_b200 has CUDA paths for SVC, SVR, Ridge, Lasso, ElasticNet, LogisticRegression and LinearSVC (bare or as "
-        "the only step of a Pipeline); got %s (no CPU fallback)" % t.__name__)
+        "spark_sklearn_b200 has CUDA paths for SVC, SVR, Ridge, Lasso, ElasticNet, LogisticRegression, LinearSVC, "
+        "KNeighborsClassifier and KNeighborsRegressor (bare or as the only step of a Pipeline); got %s (no CPU fallback)"
+        % t.__name__)
 
 
 def _as_matrix(X):
@@ -952,3 +956,112 @@ def materialize_linsvc(est, classes, raw, n_iter, n_features):
         from sklearn.exceptions import ConvergenceWarning
         warnings.warn("Liblinear failed to converge, increase the number of iterations.", ConvergenceWarning)
     return est
+
+
+# ------------------------------------------------------------------ k-nearest neighbours ------
+class KNeighborsAdapter:
+    # One GPU: the neighbour selection is the cost of the whole search and every candidate shares it, so dealing candidates
+    # to several GPUs would repeat it on each.  Under torchrun each rank still evaluates the candidates it is dealt.
+    multi_device = False
+    scorers = CLASSIFICATION_SCORERS
+
+    @staticmethod
+    def plan(estimator, cands, X, y, fold_id, n_splits, device=None):
+        return KNeighborsPlan(estimator, cands, X, y, fold_id, n_splits, device)
+
+
+class KNeighborsRegressorAdapter(KNeighborsAdapter):
+    scorers = REGRESSION_SCORERS
+
+
+_KNN_METRICS = {"euclidean": "euclidean", "l2": "euclidean", "manhattan": "manhattan", "l1": "manhattan",
+                "cityblock": "manhattan"}
+
+
+class KNeighborsPlan(_Plan):
+    """sklearn.neighbors.KNeighborsClassifier / KNeighborsRegressor (csrc/knn.cu).  A fit stores its training rows; every
+    (candidate, split) task's scorer queries the neighbours of its test rows (and, for the train score, of its training
+    rows).  The engine selects the max n_neighbors nearest training rows once per (split, metric) and every candidate votes
+    from those lists.  The refit is scikit-learn's own fit (it stores the data, plus a tree index when scikit-learn builds
+    one: there is no arithmetic for the device to take over)."""
+    max_neighbors = 256
+
+    def __init__(self, estimator, cands, X, y, fold_id, n_splits, device=None):
+        super().__init__(estimator, cands, X, y, fold_id, n_splits, device)
+        from sklearn.neighbors import KNeighborsClassifier
+        name = type(estimator).__name__
+        if y is None:
+            raise ValueError("%s needs y" % name)
+        self.classifier = isinstance(estimator, KNeighborsClassifier)
+        self.scorers = CLASSIFICATION_SCORERS if self.classifier else REGRESSION_SCORERS
+        y = np.asarray(y)
+        if y.ndim != 1:
+            raise NotImplementedError("multi-output %s is not supported by the CUDA path" % name)
+        if self.classifier:
+            self.classes, self.y_class = np.unique(y, return_inverse=True)
+            if len(self.classes) > 64:
+                raise NotImplementedError("%s CUDA path handles up to 64 classes (got %d)" % (name, len(self.classes)))
+            self._set_data(self.X, y_class=self.y_class.astype(np.int32))
+        else:
+            # scikit-learn keeps y's dtype: float32 y gives float32 uniform means
+            self.y_f32 = y.dtype == np.float32
+            self.y64 = y.astype(np.float64)
+            self._set_data(self.X, y_target=self.y64.astype(np.float32))
+            self.engine.set_targets_f64(self.y64)
+
+    def _check(self, p):
+        """scikit-learn's own parameter checks (ValueError), then what the CUDA path does not cover -> (n_neighbors, weights,
+        metric name)"""
+        type(self.estimator)(**p)._validate_params()
+        nn = p["n_neighbors"]
+        if nn > self.max_neighbors:
+            raise NotImplementedError("n_neighbors=%d: the CUDA path handles up to %d neighbours" % (nn, self.max_neighbors))
+        if callable(p["weights"]):
+            raise NotImplementedError("a callable weights has no CUDA path ('uniform' and 'distance' do)")
+        if p.get("metric_params") is not None:
+            raise NotImplementedError("metric_params has no CUDA path")
+        metric = p["metric"]
+        if metric == "minkowski":
+            if p["p"] not in (1, 2):
+                raise NotImplementedError("minkowski p=%r has no CUDA path (p=1 and p=2 do)" % (p["p"],))
+            metric = "manhattan" if p["p"] == 1 else "euclidean"
+        elif not isinstance(metric, str) or metric not in _KNN_METRICS:
+            raise NotImplementedError("metric=%r has no CUDA path (minkowski with p 1 or 2, %s do)"
+                                      % (metric, ", ".join(sorted(_KNN_METRICS))))
+        return int(nn), p["weights"], _KNN_METRICS[metric]
+
+    def evaluate(self, my, return_train=True, error_score='raise'):
+        ns = self.n_splits
+        shape = (len(my), ns)
+        checked = [self._check(self._base_params(self.cands[ci])) for ci in my]
+        m_train = [int(np.count_nonzero(self._train_rows(k))) for k in range(ns)]
+        too_many = np.array([[nn > m_train[k] for k in range(ns)] for nn, _, _ in checked], bool).reshape(shape)
+        if too_many.any() and error_score == 'raise':
+            j, k = map(int, np.argwhere(too_many)[0])
+            n_test = int(np.count_nonzero(self._test_rows(k)))
+            raise ValueError("Expected n_neighbors <= n_samples_fit, but n_neighbors = %d, n_samples_fit = %d, n_samples = %d"
+                             % (checked[j][0], m_train[k], n_test))
+        res = dict(test=np.full(shape, np.nan), train=np.full(shape, np.nan), fit_ms=np.zeros(shape), score_ms=np.zeros(shape))
+        if my:
+            self.engine.set_scoring(self.score_kind, self.score_pos)
+            r = self.engine.knn([c[0] for c in checked], [c[1] for c in checked], [c[2] for c in checked],
+                                return_train=return_train, y_f32=not self.classifier and self.y_f32)
+            for key in ("test", "fit_ms", "score_ms"):
+                res[key][:] = r[key]
+            if return_train:
+                res["train"][:] = r["train"]
+            self._prof = self.engine.profile()
+        res["test"][too_many] = np.nan
+        res["train"][too_many] = np.nan
+        return self._finish(res, return_train, error_score, len(my))
+
+    def _test_rows(self, k):
+        if self.folds is not None and not self.folds.partition:
+            return (self.folds.masks[0][:, k >> 6] >> np.uint64(k & 63)) & np.uint64(1) == 1
+        fold_id = self.fold_id if self.folds is None else self.folds.fold_id
+        return fold_id == k
+
+    def refit(self, best_params):
+        p = self._base_params(best_params)
+        self._check(p)
+        return clone(self.estimator).set_params(**best_params).fit(self.X, self.y)

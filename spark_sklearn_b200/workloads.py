@@ -116,6 +116,37 @@ def _linsvc(which="small"):
     return w
 
 
+def _knn(which="small"):
+    """k-nearest neighbours: config 3's recipe at 2000 x 32 (small, binary), a 4-class set (multi), the SVR recipe (reg_small),
+    config 2's data with a 200-fit grid (c2) and config 3's 50000 x 256 data with a smaller grid (c3: the row-slab case)."""
+    grid = {"n_neighbors": [1, 3, 5, 15], "weights": ["uniform", "distance"], "p": [1, 2]}
+    if which == "reg_small":
+        w = _svr(name="knn_reg_small", grid=grid)
+        w.update(estimator="KNeighborsRegressor", est_params={})
+        return w
+    if which == "multi":
+        from sklearn.datasets import make_classification
+        from sklearn.preprocessing import StandardScaler
+        X, y = make_classification(n_samples=2000, n_features=32, n_informative=12, n_redundant=0, n_classes=4,
+                                   class_sep=1.0, flip_y=0.02, random_state=0)
+        X = np.ascontiguousarray(StandardScaler().fit_transform(X).astype(np.float32))
+        return dict(name="knn_multi", X=X, y=y.astype(np.int64), estimator="KNeighborsClassifier", est_params={},
+                    param_grid=grid, cv=5, search="grid")
+    if which == "c2":
+        X, y = _svc_data()
+        return dict(name="knn_c2", X=X, y=y, estimator="KNeighborsClassifier", est_params={},
+                    param_grid={"n_neighbors": [1, 2, 3, 5, 8, 13, 21, 34, 55, 89], "weights": ["uniform", "distance"],
+                                "p": [1, 2]}, cv=5, search="grid")
+    if which == "c3":
+        w = _c3(name="knn_c3")
+        w.update(estimator="KNeighborsClassifier", est_params={}, search="grid",
+                 param_grid={"n_neighbors": [5, 21], "weights": ["uniform", "distance"], "p": [1, 2]})
+        return w
+    w = _c3(n=2000, d=32, name="knn_small")
+    w.update(estimator="KNeighborsClassifier", est_params={}, search="grid", param_grid=grid)
+    return w
+
+
 WORKLOADS = {
     "c1": _c1, "c2": _c2, "c3": _c3, "c4": _c4, "c5": _c5,
     # reduced-size variants: same recipes, sizes the CPU oracle finishes in seconds
@@ -140,6 +171,12 @@ WORKLOADS = {
     "linsvc_small": _linsvc,
     "linsvc_multi": lambda: _linsvc("multi"),
     "linsvc_c3": lambda: _linsvc("c3"),
+    # k-nearest neighbours (csrc/knn.cu): one neighbour selection per (split, metric) serves every candidate
+    "knn_small": _knn,
+    "knn_multi": lambda: _knn("multi"),
+    "knn_reg_small": lambda: _knn("reg_small"),
+    "knn_c2": lambda: _knn("c2"),
+    "knn_c3": lambda: _knn("c3"),
 }
 
 
@@ -164,6 +201,9 @@ def make_estimator(w):
     if w["estimator"] == "LinearSVC":
         from sklearn.svm import LinearSVC
         return LinearSVC(**w["est_params"])
+    if w["estimator"] in ("KNeighborsClassifier", "KNeighborsRegressor"):
+        import sklearn.neighbors as nb
+        return getattr(nb, w["estimator"])(**w["est_params"])
     if w["estimator"] in ("Lasso", "ElasticNet"):
         import sklearn.linear_model as lm
         return getattr(lm, w["estimator"])(**w["est_params"])
