@@ -287,6 +287,38 @@ enum { GS_DEBUG_SCORE_VOTE = 0, GS_DEBUG_SCORE_CLASS_COUNTS = 1, GS_DEBUG_SCORE_
 int gs_debug_score(gs_handle *h, int32_t kind, const double *dec, const double *rho, int32_t ncols, const int32_t *first_col,
                    const int32_t *fold, int32_t n_tasks, void *out);
 
+/* The stages of one gs_ridge / gs_enet search (mode GS_DEBUG_RIDGE / GS_DEBUG_ENET; refit != 0: gs_ridge_refit / gs_enet_refit
+ * on n_cand = 1 instead), on the dataset, splits, sample weights and scorer as set.  The search runs exactly as in production;
+ * its device buffers are copied out at the end.  Sizes are always filled; with sizes_only != 0 the call stops there (no device
+ * work).  Every array may be NULL and is in the caller's row order without padding; D = d + 2 (columns of Z = [X | y | 1]
+ * shifted, see csrc/linear.cu).  A block is a row list contracted into one Gram: a test fold (a trailing block holds the rows
+ * of no test fold), or the training / test rows of a general split (blocks 2k, 2k + 1), or all rows (refit); blocks
+ * n_plain .. n_blocks-1 are the sqrt(sample_weight)-scaled copies of blocks 0 .. n_plain-1.  Systems s = g * n_cand + c. */
+enum { GS_DEBUG_RIDGE = 0, GS_DEBUG_ENET = 1 };
+typedef struct gs_linear_debug {
+    int32_t sizes_only;          /* in */
+    int32_t n_blocks, n_plain, n_groups, n_sys, n_rows;   /* out: sizes (n_rows: the rows of all n_plain blocks, listed) */
+    int32_t cg_iterations;       /* out: CG iterations run (Ridge) */
+    int32_t *block_start;        /* [n_plain + 1]: rows of block b are rows[block_start[b] .. block_start[b + 1]) */
+    int32_t *rows;               /* [n_rows] caller row indices */
+    int32_t *test_block, *train_block;   /* [n_groups] the blocks each group is scored on (-1: none / T - test block) */
+    float *shift;                /* [d + 1] shift c of [X | y]: the Grams are about c */
+    float *block_shift;          /* [n_plain][d + 1] the block's own mean, about which it is contracted */
+    double *ystat;               /* [n_plain][2] float64 mean and centred sum of squares of the block's y */
+    double *G;                   /* [n_blocks][D][D] block Grams Z^T Z about c (Z = [X - c | y - c_y | 1], sqrt(w)-scaled copies) */
+    double *T, *Tw;              /* [D][D] sums of the unweighted / weighted block Grams */
+    float *A;                    /* [n_groups][d][d] centred training normal matrices */
+    float *rhs;                  /* [n_groups][d] */
+    double *means;               /* [n_groups][d + 3] training means of X - c, mean of y - c_y, rows, centred y^T y */
+    float *coef;                 /* [n_sys][d] solutions */
+    double *qk, *qt;             /* [n_sys] w^T G_test w and w^T M w, M = T or the split's training Gram (not on refit) */
+    double *scores;              /* [n_sys][2] test / training score (not on refit) */
+    int32_t *n_iter;             /* [n_sys] coordinate-descent sweeps (ElasticNet) */
+    double *gap;                 /* [n_sys] duality gap (ElasticNet) */
+} gs_linear_debug;
+int gs_debug_linear(gs_handle *h, int32_t mode, int32_t n_cand, const double *alpha, const double *l1_ratio, int32_t fit_intercept,
+                    double tol, int32_t max_iter, int32_t refit, gs_linear_debug *out);
+
 /* C[M][N] = sum_k A[M][k]*B[N][k] on the wgmma tensor-core path (3xTF32 split), host fp32 row-major in/out. */
 int gs_debug_gemm_nt(gs_handle *h, const float *A, int32_t M, const float *B, int32_t N, int32_t K, float *C);
 /* C[M][N] = sum_k A[M][k]*B[N][k] on the FP64 tensor-core path of gs_linsvc (K > 1024: split-K with the fixed-order sum of

@@ -143,8 +143,12 @@ class B200BaseSearchCV(BaseSearchCV):
             results['mean_%s' % key_name] = array_means
             array_stds = np.sqrt(np.average((array - array_means[:, np.newaxis]) ** 2, axis=1, weights=weights))
             results['std_%s' % key_name] = array_stds
-            if rank:
-                results["rank_%s" % key_name] = np.asarray(rankdata(-array_means, method='min'), dtype=np.int32)
+            if rank:                             # scikit-learn's rule: NaN means rank with the worst, all NaN are tied first
+                if np.isnan(array_means).all():
+                    results["rank_%s" % key_name] = np.ones(len(array_means), np.int32)
+                else:
+                    ranked = np.nan_to_num(array_means, nan=np.nanmin(array_means) - 1)
+                    results["rank_%s" % key_name] = np.asarray(rankdata(-ranked, method='min'), dtype=np.int32)
 
         _store('test_score', test_scores, splits=True, rank=True,
                weights=test_sample_counts if self.iid else None)

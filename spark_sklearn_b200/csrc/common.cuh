@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <cmath>
 #include <cstring>
 #include <string>
 #include <vector>
@@ -99,6 +100,14 @@ struct EvTimer {       // accumulates elapsed ms between consecutive marks on on
 struct SplitMasks {
     const unsigned long long *te, *tr;
 };
+// scikit-learn r2_score (metrics/_regression.py, force_finite=True) from the residual and total sums of squares of m rows:
+// NaN below two rows (UndefinedMetricWarning); a constant target (tss == 0) scores 1.0 when predicted exactly, else 0.0
+__host__ __device__ inline double gs_r2_score(double rss, double tss, double m)
+{
+    if (m < 2) return NAN;
+    if (tss != 0) return 1.0 - rss / tss;
+    return rss == 0 ? 1.0 : 0.0;
+}
 #ifdef __CUDACC__
 __device__ __forceinline__ bool split_test(const SplitMasks &m, int r, int k)      // k < 0 (refit): nobody is tested
 {

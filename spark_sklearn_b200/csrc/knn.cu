@@ -344,14 +344,6 @@ knn_vote_kernel(const int *__restrict__ li, const double *__restrict__ lk, int n
     }
 }
 
-// scikit-learn r2_score (force_finite=True) from the residual and total sums of squares of m rows; NaN below two rows
-double knn_r2(double rss, double tss, double m)
-{
-    if (m < 2) return NAN;
-    if (tss != 0) return 1.0 - rss / tss;
-    return rss == 0 ? 1.0 : 0.0;
-}
-
 // Slab rows per distance pass: the slab of float64 distances [rows][n] takes at most 1 GiB and a quarter of the free memory.
 int slab_rows(int n, size_t free_bytes)
 {
@@ -614,7 +606,7 @@ static int knn_run(gs_handle *h, int n_cand, const int32_t *nn, const int32_t *w
                         if (!(m > 0)) s = NAN;
                         else if (kind == GS_SCORE_NEG_MSE) s = -(rss / m);
                         else if (kind == GS_SCORE_NEG_RMSE) s = -std::sqrt(rss / m);
-                        else s = knn_r2(rss, tss[(size_t)k * 2 + sp], m);
+                        else s = gs_r2_score(rss, tss[(size_t)k * 2 + sp], m);
                     }
                     (sp == 0 ? sc_test : sc_train)[t] = s;
                 }

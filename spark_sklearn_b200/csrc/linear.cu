@@ -17,10 +17,12 @@
 // T - G_k.  Sample weights (gs_set_sample_weight): a second, sqrt(w)-scaled copy of the row blocks gives the weighted training
 // statistics; the scores stay unweighted.  Lasso / ElasticNet: steps 1, 2 and 4 as above, step 3 is scikit-learn's cyclic
 // coordinate descent restated on (A_k, rhs) -- enet_cd_kernel below.
-// With fit_intercept the Grams are formed from SHIFTED data, Z = [X - c | y - c_y | 1] with c the column means over all
-// rows (float64 sums, rounded to float32): the raw-moment subtractions X^T X - n xbar xbar^T and yy - ys^2/n then cancel
-// nothing even when a feature's mean dwarfs its spread (scikit-learn centres before forming products, _ridge.py:964).
-// w and R^2 are invariant under the shift; the intercept gets c_y - c.w added back.
+// With fit_intercept the Grams hold SHIFTED data, Z = [X - c | y - c_y | 1] with c the column means over all rows (float64
+// sums, rounded to float32); w and R^2 are invariant under the shift, the intercept gets c_y - c.w added back.  Each block is
+// contracted about its OWN mean and moved to c in float64 (sum_grams_kernel), so the raw-moment subtractions
+// X^T X - n xbar xbar^T and T - G_k cancel nothing a fold's own spread does not, however far the fold's mean lies from c
+// (scikit-learn centres before forming products, _ridge.py:964).  The total sums of squares of the scores come straight
+// from y in float64 (block_means_kernel): a constant target gives exactly 0, and r2 follows r2_score's edge rules.
 #include "common.cuh"
 #include <algorithm>
 #include <cmath>
@@ -32,37 +34,58 @@ namespace {
 constexpr int CG_MAX_ITER = 4000;
 constexpr double CG_TOL = 1e-6;          // relative residual; fp32 Cholesky (sklearn) is accurate to ~cond*6e-8
 
-// shift[j] = (float) mean over all rows of column j of [X | y]  (float64 accumulation); block = 32 columns x 32 row stripes
-__global__ void column_means_kernel(const float *__restrict__ X, const float *__restrict__ y, int n, int d, float *__restrict__ shift)
+// shift[b][j] = (float) mean of column j of [X | y] over the rows of block b (float64 accumulation; 0 for an empty block): rows
+// row0[b] .. row0[b]+cnt[b], or rowidx[...] of them when the blocks are row lists; row0 == nullptr: one block of all n_all rows.
+// ystat (may be null): [b][2] = the float64 mean and centred sum of squares of y over the block, straight from y, so a constant
+// target gives exactly 0.  Grid ((d + 32) / 32, blocks), block = 32 columns x 32 row stripes.
+__global__ void block_means_kernel(const float *__restrict__ X, const float *__restrict__ y, int d, const int *__restrict__ row0,
+                                   const int *__restrict__ cnt, int n_all, const int *__restrict__ rowidx, float *__restrict__ shift,
+                                   double *__restrict__ ystat)
 {
     __shared__ double acc[32][33];
-    const int j = blockIdx.x * 32 + threadIdx.x;
+    const int b = blockIdx.y, j = blockIdx.x * 32 + threadIdx.x;
+    const int r0 = row0 ? row0[b] : 0, m = row0 ? cnt[b] : n_all;
+    auto row = [&](int r) { return rowidx ? rowidx[r0 + r] : r0 + r; };
     double s = 0;
     if (j <= d)
-        for (int r = threadIdx.y; r < n; r += 32) s += (double)(j < d ? X[(size_t)r * d + j] : y[r]);
+        for (int r = threadIdx.y; r < m; r += 32) { const int q = row(r); s += (double)(j < d ? X[(size_t)q * d + j] : y[q]); }
     acc[threadIdx.y][threadIdx.x] = s;
     __syncthreads();
-    if (threadIdx.y == 0 && j <= d) {
-        double t = 0;
-        for (int q = 0; q < 32; q++) t += acc[q][threadIdx.x];
-        shift[j] = (float)(t / (double)n);
+    double t = 0;
+    for (int q = 0; q < 32; q++) t += acc[q][threadIdx.x];
+    const double mean = m > 0 ? t / (double)m : 0.0;
+    if (threadIdx.y == 0 && j <= d) shift[(size_t)b * (d + 1) + j] = (float)mean;
+    if (ystat && (int)blockIdx.x == d >> 5) {                 // the CTA that holds column d (uniform over the CTA)
+        __syncthreads();
+        double c = 0;
+        if (j == d)
+            for (int r = threadIdx.y; r < m; r += 32) { const double e = (double)y[row(r)] - mean; c += e * e; }
+        acc[threadIdx.y][threadIdx.x] = c;
+        __syncthreads();
+        if (threadIdx.y == 0 && j == d) {
+            double c2 = 0;
+            for (int q = 0; q < 32; q++) c2 += acc[q][threadIdx.x];
+            ystat[(size_t)b * 2] = mean; ystat[(size_t)b * 2 + 1] = c2;
+        }
     }
 }
 
 // (sample weights: the chunk list is doubled; chunks >= first_weighted build sqrt(w)-scaled rows, whose Grams are the weighted
 // training statistics sum w z z^T, while the unweighted copy keeps serving the scores -- _fit_and_score weights the fit only)
-// Zt[j][poff[b] + r] = X[row][j] - shift[j] (j<d) | y[row] - shift[d] (j==d) | 1 (j==d+1); rows of block b are row0[b] .. row0[b]+cnt[b],
-// or rowidx[row0[b] .. row0[b]+cnt[b]) when the blocks are row lists (general splits: the training / test rows of a split)
-__global__ void build_zt_kernel(const float *__restrict__ X, const float *__restrict__ y, const float *__restrict__ shift, int d, int n_blocks,
-                                const int *__restrict__ row0, const int *__restrict__ cnt, const int *__restrict__ poff,
-                                const int *__restrict__ rowidx, const float *__restrict__ sw, int first_weighted,
-                                float *__restrict__ Zt, int64_t ldz)
+// Zt[j][poff[q] + r] = X[row][j] - m[j] (j<d) | y[row] - m[d] (j==d) | 1 (j==d+1), m = the shift of the chunk's block
+// (bshift + cblk[q] (d + 1)); rows of chunk q are row0[q] .. row0[q]+cnt[q], or rowidx[row0[q] .. row0[q]+cnt[q]) when the
+// blocks are row lists (general splits: the training / test rows of a split)
+__global__ void build_zt_kernel(const float *__restrict__ X, const float *__restrict__ y, const float *__restrict__ bshift,
+                                const int *__restrict__ cblk, int d, int n_blocks, const int *__restrict__ row0,
+                                const int *__restrict__ cnt, const int *__restrict__ poff, const int *__restrict__ rowidx,
+                                const float *__restrict__ sw, int first_weighted, float *__restrict__ Zt, int64_t ldz)
 {
     __shared__ float tile[32][33];
     const int b = blockIdx.z;
     if (b >= n_blocks) return;
     const int r0 = blockIdx.x * 32, j0 = blockIdx.y * 32;
     if (r0 >= cnt[b]) return;
+    const float *shift = bshift + (size_t)cblk[b] * (d + 1);
     {   // coalesced read along j
         const int r = r0 + threadIdx.y, j = j0 + threadIdx.x;
         float v = 0.f;
@@ -82,18 +105,42 @@ __global__ void build_zt_kernel(const float *__restrict__ X, const float *__rest
     }
 }
 
-// The Gram of a row block is contracted in chunks of <= TC_KCHUNK rows (the tensor-core accumulator does not round to nearest); the chunk
-// partials Gq are added here in float64: G_b = sum of the chunks of block b (chunks qs[b] .. qs[b+1]), T = sum_b G_b.
-__global__ void sum_grams_kernel(const float *__restrict__ Gq, const int *__restrict__ qs, int n_blocks, int n_plain, int64_t per,
-                                 float *__restrict__ G, double *__restrict__ T, double *__restrict__ Tw)
+// The Gram of a row block is contracted in chunks of <= TC_KCHUNK rows (the tensor-core accumulator does not round to nearest),
+// about the block's own mean m_b; the chunk partials Gq are added here in float64 and moved to the common shift c: with
+// delta = m_b - c (0 in column d + 1) the rows about c are z + delta z_{d+1}, so G_b = L^T (sum of the chunks) L with
+// L = I + e_{d+1} delta^T.  The moments a fold's statistics subtract from one another are then no larger than its own
+// spread makes them, however far its mean lies from c; the (d+1)-terms are added symmetrically, G_b stays bitwise symmetric.
+// Blocks: chunks qs[b] .. qs[b+1]; T = sum_b G_b over the unweighted blocks [0, n_plain), Tw over the weighted copy.
+// E[b][c]: the ones row of block b about its mean (sum of the chunks' row d + 1, ones_row_kernel).
+__global__ void ones_row_kernel(const float *__restrict__ Gq, const int *__restrict__ qs, int n_blocks, int Dp, int d, double *__restrict__ E)
 {
+    const int64_t per = (int64_t)Dp * Dp;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n_blocks * Dp; i += gridDim.x * blockDim.x) {
+        const int b = i / Dp, c = i % Dp;
+        double s = 0;
+        for (int q = qs[b]; q < qs[b + 1]; q++) s += (double)Gq[(size_t)q * per + (size_t)(d + 1) * Dp + c];
+        E[i] = s;
+    }
+}
+
+__global__ void sum_grams_kernel(const float *__restrict__ Gq, const int *__restrict__ qs, int n_blocks, int n_plain, int Dp, int d,
+                                 const float *__restrict__ bshift, const float *__restrict__ shift, const double *__restrict__ E,
+                                 double *__restrict__ G, double *__restrict__ T, double *__restrict__ Tw)
+{
+    const int64_t per = (int64_t)Dp * Dp;
     for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < per; i += (int64_t)gridDim.x * blockDim.x) {
-        double tot = 0, totw = 0;                                   // blocks [0, n_plain): unweighted; [n_plain, n_blocks): weighted copy
+        const int a = (int)(i / Dp), c = (int)(i % Dp);
+        double tot = 0, totw = 0;
         for (int b = 0; b < n_blocks; b++) {
+            const float *m = bshift + (size_t)(b < n_plain ? b : b - n_plain) * (d + 1);
+            const double da = a <= d ? (double)m[a] - (double)shift[a] : 0.0, dc = c <= d ? (double)m[c] - (double)shift[c] : 0.0;
+            const double sa = E[(size_t)b * Dp + a], sc = E[(size_t)b * Dp + c], nn = E[(size_t)b * Dp + d + 1];
             double s = 0;
             for (int q = qs[b]; q < qs[b + 1]; q++) s += (double)Gq[(size_t)q * per + i];
-            G[(size_t)b * per + i] = (float)s;
-            if (b < n_plain) tot += s; else totw += s;
+            // no contraction into FMAs: fma(da, sc, dc * sa) would not be symmetric in (a, c)
+            const double v = __dadd_rn(__dadd_rn(s, __dadd_rn(__dmul_rn(da, sc), __dmul_rn(dc, sa))), __dmul_rn(__dmul_rn(da, dc), nn));
+            G[(size_t)b * per + i] = v;
+            if (b < n_plain) tot += v; else totw += v;
         }
         T[i] = tot;
         if (Tw) Tw[i] = totw;
@@ -103,18 +150,18 @@ __global__ void sum_grams_kernel(const float *__restrict__ Gq, const int *__rest
 // Per system-group g (a split, or "all rows" for the refit): training statistics S = T - G_test (test folds that
 // partition the rows) or S = G_train (general splits: the split's own training block), centred normal matrix
 // A (float32, [dp][dp], zero padded) and rhs (float32 [dp]); means kept in float64 for the intercept.
-__global__ void build_systems_kernel(const double *__restrict__ T, const float *__restrict__ G, const int *__restrict__ test_block,
+__global__ void build_systems_kernel(const double *__restrict__ T, const double *__restrict__ G, const int *__restrict__ test_block,
                                      const int *__restrict__ train_block, int wofs /* block offset of the weighted copy */,
                                      int d, int Dp, int dp, int fit_intercept, float *__restrict__ A, float *__restrict__ rhs,
                                      double *__restrict__ means /* [groups][dp + 3]: xbar[0..d), ybar, n_train, centred y^T y */)
 {
     const int g = blockIdx.z;
     const int tb = test_block[g], trb = train_block[g];
-    const float *Gt = tb >= 0 ? G + (size_t)(tb + wofs) * Dp * Dp : nullptr;
-    const float *Gtr = trb >= 0 ? G + (size_t)(trb + wofs) * Dp * Dp : nullptr;
+    const double *Gt = tb >= 0 ? G + (size_t)(tb + wofs) * Dp * Dp : nullptr;
+    const double *Gtr = trb >= 0 ? G + (size_t)(trb + wofs) * Dp * Dp : nullptr;
     auto S = [&](int a, int b) -> double {
-        if (Gtr) return (double)Gtr[(size_t)a * Dp + b];
-        return T[(size_t)a * Dp + b] - (Gt ? (double)Gt[(size_t)a * Dp + b] : 0.0);
+        if (Gtr) return Gtr[(size_t)a * Dp + b];
+        return T[(size_t)a * Dp + b] - (Gt ? Gt[(size_t)a * Dp + b] : 0.0);
     };
     const double ntr = S(d + 1, d + 1);
     const double ybar = fit_intercept ? S(d, d + 1) / ntr : 0.0;
@@ -425,7 +472,7 @@ cudaError_t launch_enet_cd(const float *A, const float *rhs, const double *means
 // goes to part[s][z][jt] and is summed in a fixed order by ridge_r2_kernel (deterministic, no atomics).
 constexpr int QT = 64, QL = 16;
 __global__ void __launch_bounds__(256) ridge_quad_kernel(const float *__restrict__ Xs, const double *__restrict__ T,
-                                                         const float *__restrict__ G, const int *__restrict__ test_block,
+                                                         const double *__restrict__ G, const int *__restrict__ test_block,
                                                          const int *__restrict__ train_block, int n_cand, int d, int Dp, int dp,
                                                          int njt, double *__restrict__ part)
 {
@@ -433,7 +480,7 @@ __global__ void __launch_bounds__(256) ridge_quad_kernel(const float *__restrict
     const int g = blockIdx.y, z = blockIdx.z;
     const int s0 = (blockIdx.x / njt) * QT, jt = blockIdx.x % njt, j0 = jt * QT;
     const int tb = test_block[g], trb = train_block[g];
-    const float *Mf = z == 0 ? G + (size_t)tb * Dp * Dp : (trb >= 0 ? G + (size_t)trb * Dp * Dp : nullptr);   // else T (float64)
+    const double *M = z == 0 ? G + (size_t)tb * Dp * Dp : (trb >= 0 ? G + (size_t)trb * Dp * Dp : T);
     const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
     const int mj = threadIdx.x & 63, ml = threadIdx.x >> 6;
     const float *Wg = Xs + (size_t)g * n_cand * dp;
@@ -449,7 +496,7 @@ __global__ void __launch_bounds__(256) ridge_quad_kernel(const float *__restrict
             Ws[tx][sl] = (c < n_cand && l < d) ? (double)Wg[(size_t)c * dp + l] : 0.0;
             const int lm = l0 + ml + 4 * q, j = j0 + mj;                     // lm < Dp: d + 2 <= Dp and QL | Dp
             double v = 0.0;
-            if (j < d && lm < d) v = Mf ? (double)Mf[(size_t)lm * Dp + j] : T[(size_t)lm * Dp + j];
+            if (j < d && lm < d) v = M[(size_t)lm * Dp + j];
             Ms[ml + 4 * q][mj] = v;
         }
         __syncthreads();
@@ -483,23 +530,25 @@ __global__ void __launch_bounds__(256) ridge_quad_kernel(const float *__restrict
 }
 
 // R^2 (or -MSE / -RMSE) of system s on its test block and on its training rows, from Gram statistics in float64: the
-// quadratic forms come from ridge_quad_kernel, the linear terms (rows d and d+1 of the symmetric Grams) are read here.
-__global__ void ridge_r2_kernel(const float *__restrict__ Xs, const double *__restrict__ T, const float *__restrict__ G,
-                                const int *__restrict__ test_block, const int *__restrict__ train_block,
-                                const double *__restrict__ means, const double *__restrict__ part, int njt, int n_cand, int d, int Dp,
-                                int dp, int fit_intercept, int kind, double *__restrict__ out /* [systems][2] */)
+// quadratic forms come from ridge_quad_kernel, the linear terms (rows d and d+1 of the symmetric Grams) are read here.  The
+// total sums of squares come from ystat (block_means_kernel), exact for a constant target; the training rows of a partition
+// combine the other plain blocks [0, n_plain) by the parallel-axis rule.
+__global__ void ridge_r2_kernel(const float *__restrict__ Xs, const double *__restrict__ T, const double *__restrict__ G,
+                                const double *__restrict__ ystat, int n_plain, const int *__restrict__ test_block,
+                                const int *__restrict__ train_block, const double *__restrict__ means, const double *__restrict__ part,
+                                int njt, int n_cand, int d, int Dp, int dp, int fit_intercept, int kind, double *__restrict__ out /* [systems][2] */)
 {
     __shared__ double sh[32];
     const int s = blockIdx.x, g = s / n_cand;
     const int tb = test_block[g], trb = train_block[g];
-    const float *Gk = G + (size_t)tb * Dp * Dp;
-    const float *Gtr = trb >= 0 ? G + (size_t)trb * Dp * Dp : nullptr;      // general splits: own training block; else T - Gk
-    auto Tr = [&](int a, int b) -> double { return Gtr ? (double)Gtr[(size_t)a * Dp + b] : T[(size_t)a * Dp + b]; };
+    const double *Gk = G + (size_t)tb * Dp * Dp;
+    const double *Gtr = trb >= 0 ? G + (size_t)trb * Dp * Dp : nullptr;    // general splits: own training block; else T - Gk
+    auto Tr = [&](int a, int b) -> double { return Gtr ? Gtr[(size_t)a * Dp + b] : T[(size_t)a * Dp + b]; };
     double wxy_k = 0, wxy_t = 0, ws_k = 0, ws_t = 0, xbw = 0;
     for (int j = threadIdx.x; j < d; j += blockDim.x) {
         const double w = (double)Xs[(size_t)s * dp + j];
-        wxy_k += w * (double)Gk[(size_t)d * Dp + j]; wxy_t += w * Tr(d, j);
-        ws_k += w * (double)Gk[(size_t)(d + 1) * Dp + j]; ws_t += w * Tr(d + 1, j);
+        wxy_k += w * Gk[(size_t)d * Dp + j]; wxy_t += w * Tr(d, j);
+        ws_k += w * Gk[(size_t)(d + 1) * Dp + j]; ws_t += w * Tr(d + 1, j);
         xbw += w * means[(size_t)g * (dp + 3) + j];
     }
     wxy_k = block_sum(wxy_k, sh); wxy_t = block_sum(wxy_t, sh);
@@ -509,18 +558,31 @@ __global__ void ridge_r2_kernel(const float *__restrict__ Xs, const double *__re
         double qk = 0, qt = 0;
         for (int t = 0; t < njt; t++) { qk += part[((size_t)s * 2) * njt + t]; qt += part[((size_t)s * 2 + 1) * njt + t]; }
         const double b0 = fit_intercept ? means[(size_t)g * (dp + 3) + dp] - xbw : 0.0;
-        auto r2 = [&](double yy, double ys, double nn, double q, double wxy, double ws) {
+        auto score = [&](double yy, double ys, double nn, double q, double wxy, double ws, double tss) {
             const double res = yy - 2 * wxy - 2 * b0 * ys + q + 2 * b0 * ws + nn * b0 * b0;
-            const double tot = yy - ys * ys / nn;
             if (kind == GS_SCORE_NEG_MSE) return -res / nn;              // sklearn.metrics.mean_squared_error, negated by the scorer
             if (kind == GS_SCORE_NEG_RMSE) return -sqrt(fmax(res, 0.0) / nn);
-            return 1.0 - res / tot;
+            return gs_r2_score(res, tss, nn);
         };
         const double yy_k = Gk[(size_t)d * Dp + d], ys_k = Gk[(size_t)d * Dp + d + 1], n_k = Gk[(size_t)(d + 1) * Dp + d + 1];
         const double yy_t = Tr(d, d), ys_t = Tr(d, d + 1), n_t = Tr(d + 1, d + 1);
-        out[(size_t)s * 2] = r2(yy_k, ys_k, n_k, qk, wxy_k, ws_k);
-        out[(size_t)s * 2 + 1] = Gtr ? r2(yy_t, ys_t, n_t, qt, wxy_t, ws_t)
-                                     : r2(yy_t - yy_k, ys_t - ys_k, n_t - n_k, qt - qk, wxy_t - wxy_k, ws_t - ws_k);
+        double tss_t;
+        if (Gtr) tss_t = ystat[(size_t)trb * 2 + 1];
+        else {                                                          // parallel-axis sum over the training blocks
+            double nt = 0, st = 0;
+            for (int b = 0; b < n_plain; b++)
+                if (b != tb) { const double nb = G[((size_t)b * Dp + d + 1) * Dp + d + 1]; nt += nb; st += nb * ystat[(size_t)b * 2]; }
+            const double mt = nt > 0 ? st / nt : 0.0;
+            tss_t = 0;
+            for (int b = 0; b < n_plain; b++)
+                if (b != tb) {
+                    const double nb = G[((size_t)b * Dp + d + 1) * Dp + d + 1], dm = ystat[(size_t)b * 2] - mt;
+                    tss_t += ystat[(size_t)b * 2 + 1] + nb * dm * dm;
+                }
+        }
+        out[(size_t)s * 2] = score(yy_k, ys_k, n_k, qk, wxy_k, ws_k, ystat[(size_t)tb * 2 + 1]);
+        out[(size_t)s * 2 + 1] = Gtr ? score(yy_t, ys_t, n_t, qt, wxy_t, ws_t, tss_t)
+                                     : score(yy_t - yy_k, ys_t - ys_k, n_t - n_k, qt - qk, wxy_t - wxy_k, ws_t - ws_k, tss_t);
     }
 }
 
@@ -529,8 +591,10 @@ struct RidgeTimers { float gram = 0, solve = 0, score = 0, total = 0; };
 struct EnetSpec { const double *l1_ratio; double tol; int max_iter; int32_t *n_iter; double *dual_gap; };
 
 // groups: fold k (test block k) for the search; one group with test block -1 for the refit
+// dbg (test hook gs_debug_linear, null in production): sizes, then every stage's device buffers copied out at the end
 int ridge_run(gs_handle *h, int n_cand, const double *alpha, int fit_intercept, bool refit,
-              double *test_scores, double *train_scores, double *coef_out, RidgeTimers *tmr, const EnetSpec *en = nullptr)
+              double *test_scores, double *train_scores, double *coef_out, RidgeTimers *tmr, const EnetSpec *en = nullptr,
+              gs_linear_debug *dbg = nullptr)
 {
     if (!h) return GS_ERR_ARG;
     if (h->n == 0) { gs_set_error(h, "gs_ridge: no dataset (call gs_set_data first)"); return GS_ERR_NO_DATA; }
@@ -588,9 +652,11 @@ int ridge_run(gs_handle *h, int n_cand, const double *alpha, int fit_intercept, 
         for (int b = 0; b < nb_plain; b++) { row0.push_back(row0[b]); cnt.push_back(cnt[b]); }
     const int nb = (int)row0.size();
     // contraction chunks: <= TC_KCHUNK rows each, zero-padded to a multiple of 32 columns of Z^T
-    std::vector<int> crow0, ccnt, qs(nb + 1, 0);
+    std::vector<int> crow0, ccnt, cblk, qs(nb + 1, 0);
     for (int b = 0; b < nb; b++) {
-        for (int r = 0; r < cnt[b]; r += TC_KCHUNK) { crow0.push_back(row0[b] + r); ccnt.push_back(std::min(TC_KCHUNK, cnt[b] - r)); }
+        for (int r = 0; r < cnt[b]; r += TC_KCHUNK) {
+            crow0.push_back(row0[b] + r); ccnt.push_back(std::min(TC_KCHUNK, cnt[b] - r)); cblk.push_back(b % nb_plain);
+        }
         qs[b + 1] = (int)crow0.size();
     }
     const int nq = (int)crow0.size();
@@ -600,6 +666,12 @@ int ridge_run(gs_handle *h, int n_cand, const double *alpha, int fit_intercept, 
     const int64_t ldz = poff[nq];
     const int groups = refit ? 1 : ns;
     const int nsys = groups * n_cand;
+    if (dbg) {
+        dbg->n_blocks = nb; dbg->n_plain = nb_plain; dbg->n_groups = groups; dbg->n_sys = nsys;
+        dbg->n_rows = 0;
+        for (int b = 0; b < nb_plain; b++) dbg->n_rows += cnt[b];
+        if (dbg->sizes_only) return GS_OK;
+    }
 
     h->evp.reset(); h->tt.reset();
     cudaEvent_t ev[5];
@@ -610,25 +682,30 @@ int ridge_run(gs_handle *h, int n_cand, const double *alpha, int fit_intercept, 
     DevBuf &bZ = h->dWork[0], &bZh = h->dWork[1], &bZl = h->dWork[2], &bG = h->dWork[3], &bMisc = h->dWork[4],
            &bA = h->dWork[5], &bV = h->dWork[6], &bMeta = h->dWork[7];
     GS_CUDA(bZ.reserve((size_t)Dp * ldz * 4)); GS_CUDA(bZh.reserve((size_t)Dp * ldz * 4)); GS_CUDA(bZl.reserve((size_t)Dp * ldz * 4));
-    GS_CUDA(bG.reserve((size_t)(nb + nq) * Dp * Dp * 4));                   // per-block Grams, then the chunk partials
+    GS_CUDA(bG.reserve((size_t)(nb * 8 + nq * 4) * Dp * Dp));               // float64 block Grams, then the float32 chunk partials
     const size_t tBytes = (size_t)Dp * Dp * 8 * 2, meansBytes = (size_t)groups * (dp + 3) * 8;
-    GS_CUDA(bMisc.reserve(tBytes + meansBytes + (size_t)nsys * (8 + 8 + 16) + (size_t)n_cand * 8 + (size_t)(d + 1) * 4 + 256));
+    GS_CUDA(bMisc.reserve(tBytes + meansBytes + (size_t)nsys * (8 + 8 + 16) + (size_t)n_cand * 8 + (size_t)nb_plain * 16 +
+                          (size_t)(nb_plain + 1) * (d + 1) * 4 + (size_t)nb * Dp * 8 + 256));
     GS_CUDA(bA.reserve((size_t)groups * dp * dp * 4 * 3 + (size_t)groups * dp * 4));
     GS_CUDA(bV.reserve((size_t)nsys * dp * 4 * (6 + (size_t)((dp + TC_KCHUNK - 1) / TC_KCHUNK))));
     const int nkc = (dp + TC_KCHUNK - 1) / TC_KCHUNK;                          // K-chunks of the CG product
-    GS_CUDA(bMeta.reserve((size_t)(nq * 3 + nb + 1 + 2 * groups) * 4 + (size_t)(nq + groups * nkc) * sizeof(TcBatch) + (size_t)nsys * 4 + rowidx.size() * 4 + 128));
+    GS_CUDA(bMeta.reserve((size_t)(nq * 4 + nb + 1 + 2 * groups + 2 * nb_plain) * 4 + (size_t)(nq + groups * nkc) * sizeof(TcBatch) + (size_t)nsys * 4 + rowidx.size() * 4 + 128));
     double *dT = bMisc.as<double>(), *dTw = dT + (size_t)Dp * Dp;          // totals of the unweighted / weighted block Grams
     double *dMeans = dTw + (size_t)Dp * Dp;
     double *dRR = dMeans + (size_t)groups * (dp + 3), *dBB = dRR + nsys, *dOut = dBB + nsys, *dAlpha = dOut + 2 * (size_t)nsys;
-    float *dShift = reinterpret_cast<float *>(dAlpha + n_cand);               // [d + 1] column shifts of [X | y]
+    double *dYstat = dAlpha + n_cand;                                         // [nb_plain][2] mean and centred y^T y per block
+    float *dShift = reinterpret_cast<float *>(dYstat + (size_t)nb_plain * 2); // [d + 1] column shifts c of [X | y]
+    float *dBshift = dShift + (d + 1);                                        // [nb_plain][d + 1] block means
+    double *dE = reinterpret_cast<double *>(((uintptr_t)(dBshift + (size_t)nb_plain * (d + 1)) + 7) & ~(uintptr_t)7);   // [nb][Dp]
     float *dA = bA.as<float>(), *dAh = dA + (size_t)groups * dp * dp, *dAl = dAh + (size_t)groups * dp * dp,
           *dRhs = dAl + (size_t)groups * dp * dp;
     float *dX = bV.as<float>(), *dR = dX + (size_t)nsys * dp, *dP = dR + (size_t)nsys * dp, *dPh = dP + (size_t)nsys * dp,
           *dPl = dPh + (size_t)nsys * dp, *dQ = dPl + (size_t)nsys * dp, *dQp = dQ + (size_t)nsys * dp;
-    float *dGq = bG.as<float>() + (size_t)nb * Dp * Dp;
-    int *dRow0 = bMeta.as<int>(), *dCnt = dRow0 + nq, *dPoff = dCnt + nq, *dQs = dPoff + nq, *dTestBlock = dQs + nb + 1,
-        *dTrainBlock = dTestBlock + groups;
-    int *dDone = dTrainBlock + groups;
+    double *dG = bG.as<double>();
+    float *dGq = reinterpret_cast<float *>(dG + (size_t)nb * Dp * Dp);
+    int *dRow0 = bMeta.as<int>(), *dCnt = dRow0 + nq, *dPoff = dCnt + nq, *dCblk = dPoff + nq, *dQs = dCblk + nq,
+        *dTestBlock = dQs + nb + 1, *dTrainBlock = dTestBlock + groups, *dBrow0 = dTrainBlock + groups, *dBcnt = dBrow0 + nb_plain;
+    int *dDone = dBcnt + nb_plain;
     int *dOpen = dDone + nsys;
     TcBatch *dBatchG = reinterpret_cast<TcBatch *>(((uintptr_t)(dOpen + 4) + 15) & ~(uintptr_t)15);
     TcBatch *dBatchCG = dBatchG + nq;
@@ -642,6 +719,9 @@ int ridge_run(gs_handle *h, int n_cand, const double *alpha, int fit_intercept, 
     GS_CUDA(cudaMemcpyAsync(dRow0, crow0.data(), nq * 4, cudaMemcpyHostToDevice, st));
     GS_CUDA(cudaMemcpyAsync(dCnt, ccnt.data(), nq * 4, cudaMemcpyHostToDevice, st));
     GS_CUDA(cudaMemcpyAsync(dPoff, poff.data(), nq * 4, cudaMemcpyHostToDevice, st));
+    GS_CUDA(cudaMemcpyAsync(dCblk, cblk.data(), nq * 4, cudaMemcpyHostToDevice, st));
+    GS_CUDA(cudaMemcpyAsync(dBrow0, row0.data(), nb_plain * 4, cudaMemcpyHostToDevice, st));
+    GS_CUDA(cudaMemcpyAsync(dBcnt, cnt.data(), nb_plain * 4, cudaMemcpyHostToDevice, st));
     GS_CUDA(cudaMemcpyAsync(dQs, qs.data(), (nb + 1) * 4, cudaMemcpyHostToDevice, st));
     GS_CUDA(cudaMemcpyAsync(dTestBlock, testBlock.data(), groups * 4, cudaMemcpyHostToDevice, st));
     GS_CUDA(cudaMemcpyAsync(dTrainBlock, trainBlock.data(), groups * 4, cudaMemcpyHostToDevice, st));
@@ -661,10 +741,13 @@ int ridge_run(gs_handle *h, int n_cand, const double *alpha, int fit_intercept, 
     GS_CUDA(cudaMemsetAsync(bZ.p, 0, (size_t)Dp * ldz * 4, st));
     {
         dim3 grid((TC_KCHUNK + 31) / 32, (D + 31) / 32, nq), block(32, 32);
-        if (fit_intercept) column_means_kernel<<<(d + 1 + 31) / 32, dim3(32, 32), 0, st>>>(h->dX.as<float>(), h->dYt.as<float>(), n, d, dShift);
+        const float *X = h->dX.as<float>(), *y = h->dYt.as<float>();
+        if (fit_intercept) block_means_kernel<<<(d + 32) / 32, dim3(32, 32), 0, st>>>(X, y, d, nullptr, nullptr, n, nullptr, dShift, nullptr);
         else GS_CUDA(cudaMemsetAsync(dShift, 0, (size_t)(d + 1) * 4, st));
         GS_CUDA(cudaGetLastError());
-        build_zt_kernel<<<grid, block, 0, st>>>(h->dX.as<float>(), h->dYt.as<float>(), dShift, d, nq, dRow0, dCnt, dPoff, dRowIdx,
+        block_means_kernel<<<dim3((d + 32) / 32, nb_plain), dim3(32, 32), 0, st>>>(X, y, d, dBrow0, dBcnt, 0, dRowIdx, dBshift, dYstat);
+        GS_CUDA(cudaGetLastError());
+        build_zt_kernel<<<grid, block, 0, st>>>(X, y, dBshift, dCblk, d, nq, dRow0, dCnt, dPoff, dRowIdx,
                                                 weighted ? h->dSw.as<float>() : nullptr, first_weighted, bZ.as<float>(), ldz);
         GS_CUDA(cudaGetLastError());
     }
@@ -675,15 +758,16 @@ int ridge_run(gs_handle *h, int n_cand, const double *alpha, int fit_intercept, 
     h->tt.begin(h->evp, st);
     GS_CUDA(launch_gemm_nt_tf32x3(mzh, mzl, mzh, mzl, dBatchG, nq, D, D, 1.0f, false, st, true));   // Gram: upper tiles + mirror
     h->tt.end(h->evp, st, 3.0 * 2.0 * (double)D * D * (double)ldz * (((D + 127) / 128 + 1) / (2.0 * ((D + 127) / 128))));   // tiles on/above the diagonal
-    sum_grams_kernel<<<528, 256, 0, st>>>(dGq, dQs, nb, nb_plain, (int64_t)Dp * Dp, bG.as<float>(), dT, weighted ? dTw : nullptr);
+    ones_row_kernel<<<(nb * Dp + 255) / 256, 256, 0, st>>>(dGq, dQs, nb, Dp, d, dE);
+    sum_grams_kernel<<<528, 256, 0, st>>>(dGq, dQs, nb, nb_plain, Dp, d, dBshift, dShift, dE, dG, dT, weighted ? dTw : nullptr);
     GS_CUDA(cudaGetLastError());
-    launches += 5;
+    launches += 7;
     cudaEventRecord(ev[1], st);
 
     // ---- 2. per-group centred systems ----
     {
         dim3 block(32, 8), grid((dp + 31) / 32, (dp + 7) / 8, groups);
-        build_systems_kernel<<<grid, block, 0, st>>>(weighted ? dTw : dT, bG.as<float>(), dTestBlock, dTrainBlock, weighted ? nb_plain : 0, d, Dp, dp,
+        build_systems_kernel<<<grid, block, 0, st>>>(weighted ? dTw : dT, dG, dTestBlock, dTrainBlock, weighted ? nb_plain : 0, d, Dp, dp,
                                                      fit_intercept, dA, dRhs, dMeans);
         GS_CUDA(cudaGetLastError());
     }
@@ -739,11 +823,11 @@ int ridge_run(gs_handle *h, int n_cand, const double *alpha, int fit_intercept, 
         const int njt = (d + QT - 1) / QT;
         GS_CUDA(h->dWork[8].reserve((size_t)nsys * 2 * njt * 8));
         double *dPart = h->dWork[8].as<double>();
-        ridge_quad_kernel<<<dim3(((n_cand + QT - 1) / QT) * njt, groups, 2), 256, 0, st>>>(dX, dT, bG.as<float>(), dTestBlock, dTrainBlock,
+        ridge_quad_kernel<<<dim3(((n_cand + QT - 1) / QT) * njt, groups, 2), 256, 0, st>>>(dX, dT, dG, dTestBlock, dTrainBlock,
                                                                                           n_cand, d, Dp, dp, njt, dPart);
         GS_CUDA(cudaGetLastError());
-        ridge_r2_kernel<<<nsys, 128, 0, st>>>(dX, dT, bG.as<float>(), dTestBlock, dTrainBlock, dMeans, dPart, njt, n_cand, d, Dp, dp,
-                                              fit_intercept, h->score_kind, dOut);
+        ridge_r2_kernel<<<nsys, 128, 0, st>>>(dX, dT, dG, dYstat, nb_plain, dTestBlock, dTrainBlock, dMeans, dPart, njt, n_cand, d, Dp,
+                                              dp, fit_intercept, h->score_kind, dOut);
         GS_CUDA(cudaGetLastError());
         launches++;
         launches++;
@@ -787,6 +871,61 @@ int ridge_run(gs_handle *h, int n_cand, const double *alpha, int fit_intercept, 
                 if (en->dual_gap) en->dual_gap[o] = gp[s];
                 it = std::max(it, ni[s]);
             }
+    }
+    if (dbg) {
+        GS_CUDA(cudaStreamSynchronize(st));
+        dbg->cg_iterations = en ? 0 : it;
+        auto get = [&](void *dst, const void *src, size_t bytes) -> cudaError_t {
+            return dst ? cudaMemcpy(dst, src, bytes, cudaMemcpyDeviceToHost) : cudaSuccess;
+        };
+        auto unpad = [](auto *dst, const auto *src, int m, int rows, int cols, int ld) {   // [m][ld][ld] -> [m][rows][cols]
+            if (dst)
+                for (size_t i = 0; i < (size_t)m * rows; i++) {
+                    const auto *s = src + ((i / rows) * ld + i % rows) * ld;
+                    std::copy(s, s + cols, dst + i * cols);
+                }
+        };
+        if (dbg->block_start) {
+            dbg->block_start[0] = 0;
+            for (int b = 0; b < nb_plain; b++) dbg->block_start[b + 1] = dbg->block_start[b] + cnt[b];
+        }
+        if (dbg->rows)
+            for (int b = 0, o = 0; b < nb_plain; b++)
+                for (int r = 0; r < cnt[b]; r++) dbg->rows[o++] = h->perm[dRowIdx ? rowidx[row0[b] + r] : row0[b] + r];
+        if (dbg->test_block) std::copy(testBlock.begin(), testBlock.end(), dbg->test_block);
+        if (dbg->train_block) std::copy(trainBlock.begin(), trainBlock.end(), dbg->train_block);
+        GS_CUDA(get(dbg->shift, dShift, (size_t)(d + 1) * 4));
+        GS_CUDA(get(dbg->block_shift, dBshift, (size_t)nb_plain * (d + 1) * 4));
+        GS_CUDA(get(dbg->ystat, dYstat, (size_t)nb_plain * 16));
+        std::vector<double> hd((size_t)std::max(nb, groups) * Dp * Dp);
+        std::vector<float> hf((size_t)std::max(groups * dp, nsys) * dp);
+        if (dbg->G) { GS_CUDA(cudaMemcpy(hd.data(), dG, (size_t)nb * Dp * Dp * 8, cudaMemcpyDeviceToHost)); unpad(dbg->G, hd.data(), nb, D, D, Dp); }
+        if (dbg->T) { GS_CUDA(cudaMemcpy(hd.data(), dT, (size_t)Dp * Dp * 8, cudaMemcpyDeviceToHost)); unpad(dbg->T, hd.data(), 1, D, D, Dp); }
+        if (dbg->Tw && weighted) { GS_CUDA(cudaMemcpy(hd.data(), dTw, (size_t)Dp * Dp * 8, cudaMemcpyDeviceToHost)); unpad(dbg->Tw, hd.data(), 1, D, D, Dp); }
+        if (dbg->A) { GS_CUDA(cudaMemcpy(hf.data(), dA, (size_t)groups * dp * dp * 4, cudaMemcpyDeviceToHost)); unpad(dbg->A, hf.data(), groups, d, d, dp); }
+        if (dbg->rhs) { GS_CUDA(cudaMemcpy(hf.data(), dRhs, (size_t)groups * dp * 4, cudaMemcpyDeviceToHost)); for (int g = 0; g < groups; g++) std::copy(hf.data() + (size_t)g * dp, hf.data() + (size_t)g * dp + d, dbg->rhs + (size_t)g * d); }
+        if (dbg->means) {
+            GS_CUDA(cudaMemcpy(hd.data(), dMeans, (size_t)groups * (dp + 3) * 8, cudaMemcpyDeviceToHost));
+            for (int g = 0; g < groups; g++) {
+                const double *m = hd.data() + (size_t)g * (dp + 3);
+                std::copy(m, m + d, dbg->means + (size_t)g * (d + 3));
+                std::copy(m + dp, m + dp + 3, dbg->means + (size_t)g * (d + 3) + d);
+            }
+        }
+        if (dbg->coef) { GS_CUDA(cudaMemcpy(hf.data(), dX, (size_t)nsys * dp * 4, cudaMemcpyDeviceToHost)); for (int q = 0; q < nsys; q++) std::copy(hf.data() + (size_t)q * dp, hf.data() + (size_t)q * dp + d, dbg->coef + (size_t)q * d); }
+        if (!refit && (dbg->qk || dbg->qt)) {                       // summed over the column tiles in ridge_r2_kernel's order
+            const int njt = (d + QT - 1) / QT;
+            std::vector<double> part((size_t)nsys * 2 * njt);
+            GS_CUDA(cudaMemcpy(part.data(), h->dWork[8].p, part.size() * 8, cudaMemcpyDeviceToHost));
+            for (int q = 0; q < nsys; q++) {
+                double qk = 0, qt = 0;
+                for (int t = 0; t < njt; t++) { qk += part[((size_t)q * 2) * njt + t]; qt += part[((size_t)q * 2 + 1) * njt + t]; }
+                if (dbg->qk) dbg->qk[q] = qk;
+                if (dbg->qt) dbg->qt[q] = qt;
+            }
+        }
+        if (!refit) GS_CUDA(get(dbg->scores, dOut, (size_t)nsys * 16));
+        if (en) { GS_CUDA(get(dbg->n_iter, dDone, (size_t)nsys * 4)); GS_CUDA(get(dbg->gap, dRR, (size_t)nsys * 8)); }
     }
     cudaEventRecord(ev[4], st);
     GS_CUDA(cudaStreamSynchronize(st));
@@ -858,6 +997,22 @@ int gs_enet_refit(gs_handle *h, double alpha, double l1_ratio, int32_t fit_inter
     RidgeTimers t;
     EnetSpec en{&l1_ratio, tol, max_iter, n_iter, dual_gap};
     return ridge_run(h, 1, &alpha, fit_intercept, true, nullptr, nullptr, coef_out, &t, &en);
+}
+
+// ---- test hook: the stages of one Ridge / ElasticNet search (include/b200gs.h) ----
+int gs_debug_linear(gs_handle *h, int32_t mode, int32_t n_cand, const double *alpha, const double *l1_ratio, int32_t fit_intercept,
+                    double tol, int32_t max_iter, int32_t refit, gs_linear_debug *out)
+{
+    if (!h) return GS_ERR_ARG;
+    if (!out || (mode != GS_DEBUG_RIDGE && mode != GS_DEBUG_ENET) || (refit && n_cand != 1) || (mode == GS_DEBUG_ENET && !l1_ratio)) {
+        gs_set_error(h, "gs_debug_linear: bad arguments"); return GS_ERR_ARG;
+    }
+    RidgeTimers t;
+    EnetSpec en{l1_ratio, tol, max_iter, nullptr, nullptr};
+    const int ns = std::max(h->n_splits, 1);
+    std::vector<double> te((size_t)n_cand * ns), tr((size_t)n_cand * ns), coef((size_t)h->d + 1);
+    return ridge_run(h, n_cand, alpha, fit_intercept, refit != 0, te.data(), tr.data(), coef.data(), &t,
+                     mode == GS_DEBUG_ENET ? &en : nullptr, out);
 }
 
 // ---- test hook: one tensor-core GEMM with host buffers ----

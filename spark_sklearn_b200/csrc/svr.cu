@@ -46,15 +46,6 @@ rss_kernel(const double *__restrict__ dec, const double *__restrict__ rho, int n
     if (threadIdx.x < 2) rss[(size_t)blockIdx.x * 2 + threadIdx.x] = red[threadIdx.x][0];
 }
 
-// scikit-learn r2_score (metrics/_regression.py, force_finite=True) from the residual and total sums of squares of m rows;
-// NaN for fewer than two rows (scikit-learn: UndefinedMetricWarning)
-double r2_from(double rss, double tss, double m)
-{
-    if (m < 2) return NAN;
-    if (tss != 0) return 1.0 - rss / tss;
-    return rss == 0 ? 1.0 : 0.0;
-}
-
 }  // namespace
 
 cudaError_t launch_rss(const double *dec, const double *rho, int n, const double *z, SplitMasks sm, const VoteTask *tasks,
@@ -276,7 +267,7 @@ static int svr_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
                 if (!(m > 0)) { sc[sp] = NAN; continue; }
                 if (kind == GS_SCORE_NEG_MSE) sc[sp] = -(r / m);                         // mean_squared_error
                 else if (kind == GS_SCORE_NEG_RMSE) sc[sp] = -std::sqrt(r / m);          // root_mean_squared_error
-                else sc[sp] = r2_from(r, tss[(size_t)k * 2 + sp], m);
+                else sc[sp] = gs_r2_score(r, tss[(size_t)k * 2 + sp], m);
             }
             test_scores[t] = task_bad[t] ? NAN : sc[0];
             if (train_scores) train_scores[t] = task_bad[t] ? NAN : sc[1];

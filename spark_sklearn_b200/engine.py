@@ -29,6 +29,16 @@ class GsProfile(ctypes.Structure):
                 ("ms_tensor", ctypes.c_float), ("tensor_flops", ctypes.c_double)]
 
 
+class GsLinearDebug(ctypes.Structure):
+    """include/b200gs.h gs_linear_debug"""
+    _I32 = ("block_start", "rows", "test_block", "train_block", "n_iter")
+    _F32 = ("shift", "block_shift", "A", "rhs", "coef")
+    _F64 = ("ystat", "G", "T", "Tw", "means", "qk", "qt", "scores", "gap")
+    _fields_ = [(k, ctypes.c_int32) for k in ("sizes_only", "n_blocks", "n_plain", "n_groups", "n_sys", "n_rows", "cg_iterations")] + \
+               [(k, ctypes.c_void_p) for k in ("block_start", "rows", "test_block", "train_block", "shift", "block_shift", "ystat",
+                                               "G", "T", "Tw", "A", "rhs", "means", "coef", "qk", "qt", "scores", "n_iter", "gap")]
+
+
 class EngineError(RuntimeError):
     def __init__(self, status, msg):
         super().__init__("libb200gs status %d: %s" % (status, msg))
@@ -87,6 +97,7 @@ def load_library():
     L.gs_debug_decision.argtypes = [vp, i32, dbl, i32, dbl, vp, i32, i32, vp, vp]
     L.gs_debug_score.argtypes = [vp, i32, vp, vp, i32, vp, vp, i32, vp]
     L.gs_debug_gemm_nt.argtypes = [vp, vp, i32, vp, i32, i32, vp]
+    L.gs_debug_linear.argtypes = [vp, i32, i32, vp, vp, i32, dbl, i32, i32, vp]
     L.gs_svc_predicted_iterations.argtypes = [i32, dbl, dbl, i32]
     L.gs_svc_predicted_iterations.restype = dbl
     L.gs_svc_cluster_count.argtypes = [vp, i32, i32]
@@ -96,7 +107,7 @@ def load_library():
     for f in ("gs_create", "gs_set_data", "gs_svc", "gs_svc_refit", "gs_ridge", "gs_ridge_refit", "gs_enet", "gs_enet_refit", "gs_set_targets_f64",
               "gs_svr", "gs_svr_refit", "gs_logreg",
               "gs_logreg_refit", "gs_linsvc", "gs_linsvc_refit", "gs_get_profile", "gs_debug_gram", "gs_debug_kernel_matrix",
-              "gs_debug_decision", "gs_debug_score", "gs_debug_gemm_nt", "gs_debug_gemm_f64", "gs_knn", "gs_debug_knn_neighbors"):
+              "gs_debug_decision", "gs_debug_score", "gs_debug_linear", "gs_debug_gemm_nt", "gs_debug_gemm_f64", "gs_knn", "gs_debug_knn_neighbors"):
         getattr(L, f).restype = c.c_int
     _lib = L
     return L
@@ -421,6 +432,44 @@ class Engine:
             out = np.zeros((t, 4), np.uint64)
         self._check(self._L.gs_debug_score(self._h, k, _ptr(dec), _ptr(rho), dec.shape[0], _ptr(first_col), _ptr(fold), t,
                                            _ptr(out)))
+        return out
+
+    def debug_linear(self, alpha, l1_ratio=None, fit_intercept=True, tol=1e-4, max_iter=1000, refit=False):
+        """The stages of one Ridge search (l1_ratio None) or ElasticNet search (include/b200gs.h gs_debug_linear) -> dict:
+        blocks (list of caller row-index arrays, the unweighted blocks), weighted_copies (bool), shift [d+1],
+        block_shift [n_plain][d+1], ystat [n_plain][2], G [n_blocks][D][D] (D = d + 2; blocks n_plain.. are the weighted
+        copies), T, Tw [D][D], test_block / train_block [groups], A [groups][d][d], rhs [groups][d], means [groups][d+3],
+        coef [groups][n_cand][d], qk, qt [groups][n_cand], scores [groups][n_cand][2], cg_iterations; ElasticNet: n_iter and
+        gap [groups][n_cand].  refit: one candidate on all rows, no qk / qt / scores."""
+        alpha = np.ascontiguousarray(np.atleast_1d(alpha), np.float64)
+        n_cand = len(alpha)
+        enet = l1_ratio is not None
+        l1 = np.ascontiguousarray(np.broadcast_to(np.asarray(l1_ratio, np.float64), alpha.shape)) if enet else None
+        args = lambda rec: (self._h, int(enet), n_cand, _ptr(alpha), _ptr(l1), int(bool(fit_intercept)), float(tol), int(max_iter),
+                            int(bool(refit)), ctypes.byref(rec))
+        rec = GsLinearDebug(sizes_only=1)
+        self._check(self._L.gs_debug_linear(*args(rec)))
+        nb, npl, ng, nsys, nrows = rec.n_blocks, rec.n_plain, rec.n_groups, rec.n_sys, rec.n_rows
+        d, D = self.d, self.d + 2
+        shapes = dict(block_start=(npl + 1,), rows=(nrows,), test_block=(ng,), train_block=(ng,), shift=(d + 1,),
+                      block_shift=(npl, d + 1), ystat=(npl, 2), G=(nb, D, D), T=(D, D), Tw=(D, D), A=(ng, d, d), rhs=(ng, d),
+                      means=(ng, d + 3), coef=(ng, n_cand, d))
+        if not refit:
+            shapes.update(qk=(ng, n_cand), qt=(ng, n_cand), scores=(ng, n_cand, 2))
+        if enet:
+            shapes.update(n_iter=(ng, n_cand), gap=(ng, n_cand))
+        out = {}
+        rec = GsLinearDebug(sizes_only=0)
+        for k, shape in shapes.items():
+            dt = np.int32 if k in GsLinearDebug._I32 else np.float32 if k in GsLinearDebug._F32 else np.float64
+            out[k] = np.zeros(shape, dt)
+            setattr(rec, k, out[k].ctypes.data)
+        self._check(self._L.gs_debug_linear(*args(rec)))
+        bs = out.pop("block_start")
+        rows = out.pop("rows")
+        out["blocks"] = [rows[bs[b]:bs[b + 1]] for b in range(npl)]
+        out["weighted_copies"] = nb > npl
+        out["cg_iterations"] = rec.cg_iterations
         return out
 
     def debug_gemm_nt(self, A, B):

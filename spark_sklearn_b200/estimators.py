@@ -251,9 +251,12 @@ class _Plan:
         p.update(cand)
         return p
 
-    def _finish(self, res, return_train, error_score, n_my):
+    def _finish(self, res, return_train, error_score, n_my, undefined=None):
+        """undefined: [n_splits] bool, the splits whose test score scikit-learn itself leaves NaN (kept, not an error)"""
         test, train = res["test"], res.get("train")
         bad = ~np.isfinite(test)
+        if undefined is not None:
+            bad &= ~undefined[None, :]
         if bad.any():
             if error_score == 'raise':
                 raise FloatingPointError("non-finite score from the CUDA path")
@@ -598,6 +601,18 @@ class RidgePlan(_Plan):
                           % type(estimator).__name__, UserWarning)
         self._set_data(self.X.astype(np.float32, copy=False), y_target=y.astype(np.float32))
 
+    def _undefined(self):
+        """r2 of a test set of fewer than two rows is NaN (r2_score: UndefinedMetricWarning), as in scikit-learn's search"""
+        if self.score_kind != 0:
+            return None
+        f = self.folds
+        if f is None or f.partition:
+            fid = np.asarray(self.fold_id)
+            n_test = np.bincount(fid[fid >= 0], minlength=self.n_splits)
+        else:
+            n_test = np.array([((f.masks[0][:, k >> 6] >> np.uint64(k & 63)) & np.uint64(1)).sum() for k in range(f.n_splits)])
+        return n_test < 2
+
     def _check(self, p):
         if p.get("solver", "auto") not in ("auto", "cholesky"):
             raise NotImplementedError("Ridge solver=%r has no CUDA path (auto/cholesky do)" % (p["solver"],))
@@ -626,7 +641,7 @@ class RidgePlan(_Plan):
             for k, v in self.engine.profile().items():
                 prof[k] = prof.get(k, 0) + v
         self._prof = prof
-        return self._finish(res, return_train, error_score, len(my))
+        return self._finish(res, return_train, error_score, len(my), self._undefined())
 
     def refit(self, best_params):
         p = self._base_params(best_params)
@@ -704,7 +719,7 @@ class ENetPlan(RidgePlan):
                 prof[k] = prof.get(k, 0) + v
         self._prof = prof
         self.n_iter_ = res["n_iter"]
-        return self._finish(res, return_train, error_score, len(my))
+        return self._finish(res, return_train, error_score, len(my), self._undefined())
 
     def refit(self, best_params):
         p = self._base_params(best_params)
