@@ -147,6 +147,20 @@ int gs_svc_refit(gs_handle *h, int32_t kernel, double C, double gamma, double to
                  uint32_t flags, double *pair_coef, double *rho, int32_t *n_iter);
 
 /*
+ * nu-SVC (replaces NuSVC.fit/score: sklearn libsvm svm.cpp solve_nu_svc, Solver_NU).  Arguments, outputs, kernels, scorers and
+ * splits as gs_svc / gs_svc_refit, with nu[n_cand] (0 < nu <= 1) in place of C.  Class weights do not enter a nu-SVC solve
+ * (libsvm gives every row C = 1) and are ignored; sample weights are rejected.  pair_coef and rho are the model's: alpha y / r
+ * and rho / r.  A (candidate, split) whose training class counts make some class pair infeasible (svm_check_parameter:
+ * nu (n1 + n2) / 2 > min(n1, n2)) is not solved: its scores are NaN and its n_iter is -1.  gs_nusvc_refit returns GS_ERR_ARG
+ * ("specified nu is infeasible") in that case.  Sub-problems of at most 16384 rows.
+ */
+int gs_nusvc(gs_handle *h, int32_t n_cand, const int32_t *kernel, const double *nu, const double *gamma, double tol,
+             int32_t max_iter, uint32_t flags, double *test_scores, double *train_scores, int32_t *n_iter,
+             int32_t *n_sv, float *fit_ms, float *score_ms);
+int gs_nusvc_refit(gs_handle *h, int32_t kernel, double nu, double gamma, double tol, int32_t max_iter, uint32_t flags,
+                   double *pair_coef, double *rho, int32_t *n_iter);
+
+/*
  * Ridge (replaces Ridge.fit/score: sklearn linear_model/_ridge.py:919, _solve_cholesky :215-227,
  * r2 base.py:716).  alpha[n_cand].  Scores are R^2.  coef_out (may be NULL): refit on all rows of
  * candidate refit_cand -> [d] weights + intercept at [d].
@@ -204,6 +218,16 @@ int gs_svr(gs_handle *h, int32_t n_cand, const int32_t *kernel, const double *C,
            int32_t *n_sv, float *fit_ms, float *score_ms);
 int gs_svr_refit(gs_handle *h, int32_t kernel, double C, double epsilon, double gamma, double tol, int32_t max_iter,
                  uint32_t flags, double *coef, double *rho, int32_t *n_iter);
+
+/*
+ * nu-SVR (replaces NuSVR.fit/score: sklearn libsvm svm.cpp solve_nu_svr, Solver_NU on 2l variables).  Arguments, outputs,
+ * limits and scorers as gs_svr / gs_svr_refit, with nu[n_cand] (0 < nu <= 1) in place of epsilon.
+ */
+int gs_nusvr(gs_handle *h, int32_t n_cand, const int32_t *kernel, const double *C, const double *nu, const double *gamma,
+             double tol, int32_t max_iter, uint32_t flags, double *test_scores, double *train_scores, int32_t *n_iter,
+             int32_t *n_sv, float *fit_ms, float *score_ms);
+int gs_nusvr_refit(gs_handle *h, int32_t kernel, double C, double nu, double gamma, double tol, int32_t max_iter,
+                   uint32_t flags, double *coef, double *rho, int32_t *n_iter);
 
 /*
  * LinearSVC (penalty='l2', loss='squared_hinge', primal: replaces LinearSVC.fit/score = sklearn liblinear linear.cpp train /

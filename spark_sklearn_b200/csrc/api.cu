@@ -77,7 +77,7 @@ __global__ void gather_rows_kernel(const T *__restrict__ src, const int *__restr
 
 extern "C" {
 
-int gs_version(void) { return 105; }
+int gs_version(void) { return 106; }
 
 int gs_set_class_weight(gs_handle *h, const double *w, int32_t n_sets)
 {
@@ -388,22 +388,26 @@ extern "C" void gs_svc_schedule(const double *cost_desc, int32_t n, int32_t sm_c
     if (n_exclusive) *n_exclusive = be;
 }
 
+// nu == false: C-SVC, Cv[c] is C.  nu == true: nu-SVC (libsvm's Solver_NU, svm.cpp solve_nu_svc), Cv[c] is nu; class weights
+// do not enter a nu-SVC solve (its C is 1 per row), and a task whose training set makes some class pair infeasible for its nu
+// is not solved: it scores NaN with n_iter = -1 (a refit returns GS_ERR_ARG).
 static int svc_run(gs_handle *h, int n_cand, const int32_t *kernel, const double *Cv, const double *gamma,
-                   double tol, int max_iter, uint32_t flags, bool refit,
+                   double tol, int max_iter, uint32_t flags, bool refit, bool nu,
                    double *test_scores, double *train_scores, int32_t *n_iter, int32_t *n_sv,
                    float *fit_ms, float *score_ms, double *pair_coef, double *rho_out, int32_t *pair_iter)
 {
+    const char *who = nu ? "gs_nusvc" : "gs_svc";
     if (!h) return GS_ERR_ARG;
-    if (h->n == 0) { gs_set_error(h, "gs_svc: no dataset (call gs_set_data first)"); return GS_ERR_NO_DATA; }
-    if (!h->classification) { gs_set_error(h, "gs_svc: dataset has no class labels"); return GS_ERR_ARG; }
-    if (h->n_classes < 2 || h->n_classes > 32) { gs_set_error(h, "gs_svc: need 2..32 classes"); return GS_ERR_UNSUPPORTED; }
-    if (n_cand <= 0 || !kernel || !Cv || !gamma) { gs_set_error(h, "gs_svc: bad arguments"); return GS_ERR_ARG; }
+    if (h->n == 0) { gs_set_error(h, std::string(who) + ": no dataset (call gs_set_data first)"); return GS_ERR_NO_DATA; }
+    if (!h->classification) { gs_set_error(h, std::string(who) + ": dataset has no class labels"); return GS_ERR_ARG; }
+    if (h->n_classes < 2 || h->n_classes > 32) { gs_set_error(h, std::string(who) + ": need 2..32 classes"); return GS_ERR_UNSUPPORTED; }
+    if (n_cand <= 0 || !kernel || !Cv || !gamma) { gs_set_error(h, std::string(who) + ": bad arguments"); return GS_ERR_ARG; }
     if (!h->sample_w.empty()) {
-        gs_set_error(h, "gs_svc: sample weights (a C per row) are not supported by the SMO kernels; class weights are (gs_set_class_weight)");
+        gs_set_error(h, std::string(who) + ": sample weights (a C per row) are not supported by the SMO kernels; class weights are (gs_set_class_weight)");
         return GS_ERR_UNSUPPORTED;
     }
     if (h->class_w_sets > 1 && h->class_w_sets != (refit ? 1 : h->n_splits)) {
-        gs_set_error(h, "gs_svc: gs_set_class_weight was given a weight set per split, but not for this number of splits"); return GS_ERR_ARG;
+        gs_set_error(h, std::string(who) + ": gs_set_class_weight was given a weight set per split, but not for this number of splits"); return GS_ERR_ARG;
     }
     GS_CUDA(cudaSetDevice(h->device));
     cudaStream_t st = h->stream;
@@ -413,11 +417,12 @@ static int svc_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
     const int n_tasks = n_cand * n_splits;
     const int64_t ldk = ((int64_t)n + 31) & ~31LL;
     for (int c = 0; c < n_cand; c++) {
-        if (kernel[c] < GS_KERNEL_LINEAR || kernel[c] > GS_KERNEL_SIGMOID) { gs_set_error(h, "gs_svc: unsupported kernel id"); return GS_ERR_UNSUPPORTED; }
-        if (!(Cv[c] > 0)) { gs_set_error(h, "gs_svc: C must be > 0"); return GS_ERR_ARG; }
+        if (kernel[c] < GS_KERNEL_LINEAR || kernel[c] > GS_KERNEL_SIGMOID) { gs_set_error(h, std::string(who) + ": unsupported kernel id"); return GS_ERR_UNSUPPORTED; }
+        if (nu && !(Cv[c] > 0 && Cv[c] <= 1)) { gs_set_error(h, "gs_nusvc: nu must be in (0, 1]"); return GS_ERR_ARG; }
+        if (!(Cv[c] > 0)) { gs_set_error(h, std::string(who) + ": C must be > 0"); return GS_ERR_ARG; }
     }
     if (!h->kp_degree.empty() && (int)h->kp_degree.size() != n_cand) {
-        gs_set_error(h, "gs_svc: gs_set_kernel_params was given " + std::to_string(h->kp_degree.size()) + " candidates, this call has " +
+        gs_set_error(h, std::string(who) + ": gs_set_kernel_params was given " + std::to_string(h->kp_degree.size()) + " candidates, this call has " +
                             std::to_string(n_cand));
         return GS_ERR_ARG;
     }
@@ -449,7 +454,7 @@ static int svc_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
                     if (refit || h->is_train(r, k)) rows_all.push_back(r);
                 const int l = (int)rows_all.size() - sp_off[s];
                 if (sp_npos[s] == 0 || sp_npos[s] == l) {
-                    gs_set_error(h, "gs_svc: a training fold lacks one of the classes"); return GS_ERR_ARG;
+                    gs_set_error(h, std::string(who) + ": a training fold lacks one of the classes"); return GS_ERR_ARG;
                 }
                 lmax = std::max(lmax, l);
             }
@@ -474,14 +479,33 @@ static int svc_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
             sp_seg[s * 8 + 4 + e] = std::min(runs[e].second, (int)ldk) - runs[e].first;
         }
     }
+    if (nu && lmax > smo_max_rows()) {
+        gs_set_error(h, "gs_nusvc: sub-problem with " + std::to_string(lmax) + " rows exceeds the resident-state SMO kernel limit of " +
+                            std::to_string(smo_max_rows()));
+        return GS_ERR_UNSUPPORTED;
+    }
     if (lmax > smo_max_rows() && lmax > smo_colown_max_rows(4) && lmax >= 16383) {
-        gs_set_error(h, "gs_svc: sub-problem with " + std::to_string(lmax) + " rows exceeds the resident-state SMO kernel limit of " +
+        gs_set_error(h, std::string(who) + ": sub-problem with " + std::to_string(lmax) + " rows exceeds the resident-state SMO kernel limit of " +
                             std::to_string(smo_max_rows()));
         return GS_ERR_UNSUPPORTED;
     }
 
+    // nu-SVC feasibility of every (candidate, split) over its class pairs (svm.cpp svm_check_parameter: nu (n1 + n2) / 2 >
+    // min(n1, n2) for the class counts n1, n2 of the training rows)
+    std::vector<char> infeasible(n_tasks, 0);
+    if (nu)
+        for (int t = 0; t < n_tasks; t++) {
+            const int k = t % n_splits;
+            for (int p = 0; p < n_pairs; p++) {
+                const size_t s = (size_t)k * n_pairs + p;
+                const double n1 = sp_npos[s], n2 = sp_off[s + 1] - sp_off[s] - sp_npos[s];
+                if (Cv[t / n_splits] * (n1 + n2) / 2 > std::min(n1, n2)) infeasible[t] = 1;
+            }
+            if (refit && infeasible[t]) { gs_set_error(h, "gs_nusvc_refit: specified nu is infeasible"); return GS_ERR_ARG; }
+        }
+
     // ---- 3. group tasks by kernel matrix (kernel, gamma, degree, coef0); 4. memory plan: batches of kernel matrices that fit in free HBM ----
-    if (const int rc = search.group("gs_svc", n_cand, n_splits, kernel, gamma, degree, coef0)) return rc;
+    if (const int rc = search.group(who, n_cand, n_splits, kernel, gamma, degree, coef0)) return rc;
     if (const int rc = search.plan_batches()) return rc;
     const int n_groups = (int)search.groups.size(), gpb = search.per_batch;
 
@@ -499,11 +523,11 @@ static int svc_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
     std::vector<unsigned long long> score_raw;
     if (!refit && h->score_kind != GS_SCORE_DEFAULT) {
         const int kd = h->score_kind;
-        if (kd == GS_SCORE_NEG_MSE || kd == GS_SCORE_NEG_RMSE) { gs_set_error(h, "gs_svc: regression scorer on a classifier"); return GS_ERR_ARG; }
+        if (kd == GS_SCORE_NEG_MSE || kd == GS_SCORE_NEG_RMSE) { gs_set_error(h, std::string(who) + ": regression scorer on a classifier"); return GS_ERR_ARG; }
         if ((kd == GS_SCORE_ROC_AUC || kd == GS_SCORE_F1 || kd == GS_SCORE_PRECISION || kd == GS_SCORE_RECALL) && nc != 2) {
-            gs_set_error(h, "gs_svc: this scorer is defined for binary problems only"); return GS_ERR_UNSUPPORTED;
+            gs_set_error(h, std::string(who) + ": this scorer is defined for binary problems only"); return GS_ERR_UNSUPPORTED;
         }
-        if (h->score_pos >= nc) { gs_set_error(h, "gs_svc: positive class out of range"); return GS_ERR_ARG; }
+        if (h->score_pos >= nc) { gs_set_error(h, std::string(who) + ": positive class out of range"); return GS_ERR_ARG; }
     }
     int64_t total_iter = 0;
     double solve_bytes = 0;
@@ -514,6 +538,7 @@ static int svc_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
         if (const int rc = search.kernel_matrices(g0, g1)) return rc;
         // -- problems: ordered by (group, task, pair); column index == problem index --
         std::vector<SmoProblem> probs;
+        std::vector<NuData> nud;
         std::vector<int> prob_task, group_first(g1 - g0 + 1, 0);
         std::vector<VoteTask> vtasks;
         std::vector<int> vtask_id;
@@ -521,6 +546,7 @@ static int svc_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
             group_first[g - g0] = (int)probs.size();
             for (int t : search.group_tasks[g]) {
                 const int c = t / n_splits, k = t % n_splits;
+                if (infeasible[t]) continue;
                 vtasks.push_back(VoteTask{(int)probs.size(), refit ? -100 : k});
                 vtask_id.push_back(t);
                 for (int p = 0; p < n_pairs; p++) {
@@ -545,6 +571,12 @@ static int svc_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
                     P.guard = search.d_guard;
                     P.nslots = 0;
                     for (int e = 0; e < P.nseg; e++) P.nslots += P.seg_len[e];
+                    if (nu) {                                  // svm.cpp:1660-1673: C = 1 per row, nu_l = sum of nu x C in row order
+                        P.C = P.Cn = 1.0;
+                        double nu_l = 0;
+                        for (int r = 0; r < P.l; r++) nu_l += Cv[c] * 1.0;
+                        nud.push_back(NuData{nu_l / 2, nu_l / 2});
+                    }
                     probs.push_back(P);
                     prob_task.push_back(t);
                 }
@@ -552,15 +584,18 @@ static int svc_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
         }
         group_first[g1 - g0] = (int)probs.size();
         const int np = (int)probs.size();
+        if (np == 0) continue;                                // every task of the batch is infeasible for its nu
         if (const int rc = search.workspaces(probs)) return rc;
-        GS_CUDA(h->dWork[6].reserve((size_t)np * sizeof(SmoProblem) + (size_t)np * 4 + vtasks.size() * (sizeof(VoteTask) + 16) + 256));
+        GS_CUDA(h->dWork[6].reserve((size_t)np * sizeof(SmoProblem) + (size_t)np * 4 + vtasks.size() * (sizeof(VoteTask) + 16) +
+                                    nud.size() * sizeof(NuData) + 256));
         // Predicted cost = rows x predicted SMO iterations (gs_svc_predicted_iterations): the predicted-longest problems lead
         // the launch order and the cluster policy below works on cost ratios.
         std::vector<double> cost(np);
         for (int q = 0; q < np; q++) {
             const int t = prob_task[q];
             const auto &grp = search.groups[search.task_group[t]];
-            cost[q] = gs_svc_predicted_iterations(grp.kernel, Cv[t / n_splits], grp.gamma, (int32_t)d) * (double)probs[q].l;
+            // no iteration model for nu-SVC yet: rows alone order its problems
+            cost[q] = (nu ? 1.0 : gs_svc_predicted_iterations(grp.kernel, Cv[t / n_splits], grp.gamma, (int32_t)d)) * (double)probs[q].l;
         }
         std::vector<int> order(np);
         std::iota(order.begin(), order.end(), 0);
@@ -574,6 +609,12 @@ static int svc_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
         off += vtasks.size() * sizeof(VoteTask);
         off = (off + 15) & ~(size_t)15;
         int *d_counts = (int *)(dmeta + off);
+        off += vtasks.size() * 16;
+        NuData *d_nu = (NuData *)(dmeta + off);
+        if (nu) {
+            GS_CUDA(cudaMemcpyAsync(d_nu, nud.data(), nud.size() * sizeof(NuData), cudaMemcpyHostToDevice, st));
+            pf.h2d_bytes += nud.size() * sizeof(NuData);
+        }
         GS_CUDA(cudaMemcpyAsync(d_probs, probs.data(), (size_t)np * sizeof(SmoProblem), cudaMemcpyHostToDevice, st));
         GS_CUDA(cudaMemcpyAsync(d_order, order.data(), (size_t)np * 4, cudaMemcpyHostToDevice, st));
         GS_CUDA(cudaMemcpyAsync(d_vt, vtasks.data(), vtasks.size() * sizeof(VoteTask), cudaMemcpyHostToDevice, st));
@@ -612,7 +653,7 @@ static int svc_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
         //     two-tier schedule of the position-owned kernel (gs_svc_cluster_count).
         // B200GS_SMO_CLUSTER (0/2/4/8) and B200GS_SMO_CLUSTER_N force the cluster size and the number of clustered problems.
         int cl = 0, n_cl = 0, n_ex = 0;
-        if (lmax > 2048) {
+        if (!nu && lmax > 2048) {
             if (np * 8 <= h->sm_count) { cl = 8; n_cl = np; }
             else if (np * 4 <= h->sm_count) { cl = 4; n_cl = np; }
             else if (np * 2 <= h->sm_count) { cl = 2; n_cl = np; }
@@ -628,7 +669,13 @@ static int svc_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
         if (const char *e = getenv("B200GS_SMO_CLUSTER_N")) n_cl = std::min(np, atoi(e));
         if (!(cl == 2 || cl == 4 || cl == 8) || lmax > smo_colown_max_rows(cl) || lmax <= 2048) n_cl = 0;
         n_ex = std::max(0, std::min(n_ex, np - n_cl));
-        if (n_cl > 0 || n_ex > 0) {
+        if (nu) {                                            // Solver_NU has only the position-owned instance (smo.cu)
+            for (int inst = search.fast ? 1 : 0; inst >= 0; inst--) {
+                const cudaError_t ce = launch_smo_nu(d_probs, nullptr, d_nu, d_order, np, lmax, inst == 1, st, &why);
+                if (ce != cudaSuccess) { gs_set_error(h, why.empty() ? std::string("launch_smo_nu: ") + cudaGetErrorString(ce) : why); return why.empty() ? GS_ERR_CUDA : GS_ERR_UNSUPPORTED; }
+                pf.launches++;
+            }
+        } else if (n_cl > 0 || n_ex > 0) {
             // The latency tiers must get their SMs before the shared-SM launch floods the GPU (a late start of the critical
             // path costs the makespan that much).  So the cluster
             // kernel goes on the engine stream itself, in order behind the uploads; the exclusive and the shared launches go
@@ -715,7 +762,7 @@ static int svc_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
             solve_bytes += (double)info[(size_t)q * 4] * 2.0 * probs[q].l * 4.0;
             // a task whose solve went non-finite scores NaN; the caller applies error_score to THAT task only
             // (reference base_search.py:69,87: _fit_and_score(..., error_score) fills per task)
-            if (!std::isfinite(rho[q])) { if (refit) { gs_set_error(h, "gs_svc_refit: non-finite intercept"); return GS_ERR_NUMERIC; } task_bad[t] = 1; }
+            if (!std::isfinite(rho[q])) { if (refit) { gs_set_error(h, std::string(who) + "_refit: non-finite intercept"); return GS_ERR_NUMERIC; } task_bad[t] = 1; }
         }
         if (getenv("B200GS_SMO_TIMELINE") && atoi(getenv("B200GS_SMO_TIMELINE"))) {
             // development aid: when each tier starts and ends (globaltimer of the sub-problems, ms after the first start)
@@ -795,8 +842,8 @@ static int svc_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
                 test_scores[t] = task_score[(size_t)t * 2];
                 if (train_scores) train_scores[t] = task_score[(size_t)t * 2 + 1];
             }
-            if (task_bad[t]) { test_scores[t] = NAN; if (train_scores) train_scores[t] = NAN; }
-            if (n_iter) n_iter[t] = task_iter[t];
+            if (task_bad[t] || infeasible[t]) { test_scores[t] = NAN; if (train_scores) train_scores[t] = NAN; }
+            if (n_iter) n_iter[t] = infeasible[t] ? -1 : task_iter[t];
             if (n_sv) n_sv[t] = task_sv[t];
             if (fit_ms) fit_ms[t] = (float)task_fit_ms[t];
             if (score_ms) score_ms[t] = pf.ms_score / (float)n_tasks;
@@ -810,7 +857,7 @@ int gs_svc(gs_handle *h, int32_t n_cand, const int32_t *kernel, const double *C,
            int32_t *n_sv, float *fit_ms, float *score_ms)
 {
     if (h && !test_scores) { gs_set_error(h, "gs_svc: test_scores is NULL"); return GS_ERR_ARG; }
-    return svc_run(h, n_cand, kernel, C, gamma, tol, max_iter, flags, false, test_scores,
+    return svc_run(h, n_cand, kernel, C, gamma, tol, max_iter, flags, false, false, test_scores,
                    (flags & GS_RETURN_TRAIN) ? train_scores : nullptr, n_iter, n_sv, fit_ms, score_ms, nullptr, nullptr, nullptr);
 }
 
@@ -818,7 +865,24 @@ int gs_svc_refit(gs_handle *h, int32_t kernel, double C, double gamma, double to
                  double *pair_coef, double *rho, int32_t *n_iter)
 {
     const int32_t k = kernel;
-    return svc_run(h, 1, &k, &C, &gamma, tol, max_iter, flags, true, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
+    return svc_run(h, 1, &k, &C, &gamma, tol, max_iter, flags, true, false, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
+                   pair_coef, rho, n_iter);
+}
+
+int gs_nusvc(gs_handle *h, int32_t n_cand, const int32_t *kernel, const double *nu, const double *gamma, double tol,
+             int32_t max_iter, uint32_t flags, double *test_scores, double *train_scores, int32_t *n_iter,
+             int32_t *n_sv, float *fit_ms, float *score_ms)
+{
+    if (h && !test_scores) { gs_set_error(h, "gs_nusvc: test_scores is NULL"); return GS_ERR_ARG; }
+    return svc_run(h, n_cand, kernel, nu, gamma, tol, max_iter, flags, false, true, test_scores,
+                   (flags & GS_RETURN_TRAIN) ? train_scores : nullptr, n_iter, n_sv, fit_ms, score_ms, nullptr, nullptr, nullptr);
+}
+
+int gs_nusvc_refit(gs_handle *h, int32_t kernel, double nu, double gamma, double tol, int32_t max_iter, uint32_t flags,
+                   double *pair_coef, double *rho, int32_t *n_iter)
+{
+    const int32_t k = kernel;
+    return svc_run(h, 1, &k, &nu, &gamma, tol, max_iter, flags, true, true, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
                    pair_coef, rho, n_iter);
 }
 

@@ -225,6 +225,15 @@ struct SvrData {
 // (ascending original index) twice, n_pos = l / 2; svr[q] holds its targets and epsilon.  coef gets alpha+ - alpha- by row.
 cudaError_t launch_smo_svr(const SmoProblem *d_probs, const SvrData *d_svr, const int *d_order, int n_prob, int lmax, bool fast,
                            int rowcap, cudaStream_t st, std::string *why);
+// nu-SVC / nu-SVR starting point of one problem (parallel to SmoProblem; only the nu instances read it): the sums that
+// libsvm hands out greedily, min(C, remaining) in position order, to the +1 positions and to the -1 positions
+struct NuData {
+    double sum_pos, sum_neg;
+};
+// libsvm's Solver_NU on the position-owned kernel.  d_svr == nullptr: nu-SVC (C = Cn = 1, coef = alpha y / r, rho / r);
+// otherwise nu-SVR on the SVR layout of launch_smo_svr with svr[q].eps = 0 (linear term -/+ z).
+cudaError_t launch_smo_nu(const SmoProblem *d_probs, const SvrData *d_svr, const NuData *d_nu, const int *d_order, int n_prob,
+                          int lmax, bool fast, cudaStream_t st, std::string *why);
 // smo_lean.cu: the throughput instance (static slots = the problem's column runs, two or more sub-problems per SM).  Every
 // problem of the launch needs a slot layout: nseg > 0, nslots <= smo_lean_max_slots(), l < 16383; alpha and Gbar hold nslots doubles.
 int smo_lean_max_slots();

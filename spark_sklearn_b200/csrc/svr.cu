@@ -1,4 +1,5 @@
-// svr.cu -- epsilon-SVR search and refit (gs_svr / gs_svr_refit) and the regression scorer over SVR decision values.
+// svr.cu -- epsilon-SVR and nu-SVR searches and refits (gs_svr / gs_svr_refit, gs_nusvr / gs_nusvr_refit) and the regression
+// scorer over SVR decision values.
 //
 // An SVR fit on l training rows is libsvm's C-SVC Solver on 2l variables (svm.cpp solve_epsilon_svr): positions 0..l-1 are
 // the rows with y = +1 and linear term eps - z, positions l..2l-1 the same rows with y = -1 and linear term eps + z.  The
@@ -56,26 +57,29 @@ cudaError_t launch_rss(const double *dec, const double *rho, int n, const double
     return cudaGetLastError();
 }
 
+// nu == false: epsilon-SVR, epsv[c] is epsilon.  nu == true: nu-SVR (svm.cpp solve_nu_svr on Solver_NU), epsv[c] is nu.
 static int svr_run(gs_handle *h, int n_cand, const int32_t *kernel, const double *Cv, const double *epsv, const double *gamma,
-                   double tol, int max_iter, uint32_t flags, bool refit,
+                   double tol, int max_iter, uint32_t flags, bool refit, bool nu,
                    double *test_scores, double *train_scores, int32_t *n_iter, int32_t *n_sv, float *fit_ms, float *score_ms,
                    double *coef_out, double *rho_out)
 {
+    const char *who = nu ? "gs_nusvr" : "gs_svr";
     if (!h) return GS_ERR_ARG;
-    if (h->n == 0) { gs_set_error(h, "gs_svr: no dataset (call gs_set_data first)"); return GS_ERR_NO_DATA; }
-    if (h->classification) { gs_set_error(h, "gs_svr: the dataset has class labels (SVR needs a regression gs_set_data)"); return GS_ERR_ARG; }
-    if (h->z64.empty()) { gs_set_error(h, "gs_svr: no float64 targets (call gs_set_targets_f64 after gs_set_data)"); return GS_ERR_NO_DATA; }
-    if (n_cand <= 0 || !kernel || !Cv || !epsv || !gamma) { gs_set_error(h, "gs_svr: bad arguments"); return GS_ERR_ARG; }
-    if (!h->sample_w.empty()) { gs_set_error(h, "gs_svr: sample weights are not supported by the SVR kernels"); return GS_ERR_UNSUPPORTED; }
-    if (h->class_w_sets > 0) { gs_set_error(h, "gs_svr: class weights do not apply to a regressor"); return GS_ERR_ARG; }
+    if (h->n == 0) { gs_set_error(h, std::string(who) + ": no dataset (call gs_set_data first)"); return GS_ERR_NO_DATA; }
+    if (h->classification) { gs_set_error(h, std::string(who) + ": the dataset has class labels (SVR needs a regression gs_set_data)"); return GS_ERR_ARG; }
+    if (h->z64.empty()) { gs_set_error(h, std::string(who) + ": no float64 targets (call gs_set_targets_f64 after gs_set_data)"); return GS_ERR_NO_DATA; }
+    if (n_cand <= 0 || !kernel || !Cv || !epsv || !gamma) { gs_set_error(h, std::string(who) + ": bad arguments"); return GS_ERR_ARG; }
+    if (!h->sample_w.empty()) { gs_set_error(h, std::string(who) + ": sample weights are not supported by the SVR kernels"); return GS_ERR_UNSUPPORTED; }
+    if (h->class_w_sets > 0) { gs_set_error(h, std::string(who) + ": class weights do not apply to a regressor"); return GS_ERR_ARG; }
     const int kind = refit ? GS_SCORE_DEFAULT : h->score_kind;
     if (kind != GS_SCORE_DEFAULT && kind != GS_SCORE_NEG_MSE && kind != GS_SCORE_NEG_RMSE) {
-        gs_set_error(h, "gs_svr: classification scorer on a regressor"); return GS_ERR_ARG;
+        gs_set_error(h, std::string(who) + ": classification scorer on a regressor"); return GS_ERR_ARG;
     }
     for (int c = 0; c < n_cand; c++) {
-        if (kernel[c] != GS_KERNEL_LINEAR && kernel[c] != GS_KERNEL_RBF) { gs_set_error(h, "gs_svr: unsupported kernel id"); return GS_ERR_UNSUPPORTED; }
-        if (!(Cv[c] > 0) || !std::isfinite(Cv[c])) { gs_set_error(h, "gs_svr: C must be > 0"); return GS_ERR_ARG; }
-        if (!(epsv[c] >= 0) || !std::isfinite(epsv[c])) { gs_set_error(h, "gs_svr: epsilon must be >= 0"); return GS_ERR_ARG; }
+        if (kernel[c] != GS_KERNEL_LINEAR && kernel[c] != GS_KERNEL_RBF) { gs_set_error(h, std::string(who) + ": unsupported kernel id"); return GS_ERR_UNSUPPORTED; }
+        if (!(Cv[c] > 0) || !std::isfinite(Cv[c])) { gs_set_error(h, std::string(who) + ": C must be > 0"); return GS_ERR_ARG; }
+        if (nu && !(epsv[c] > 0 && epsv[c] <= 1)) { gs_set_error(h, "gs_nusvr: nu must be in (0, 1]"); return GS_ERR_ARG; }
+        if (!(epsv[c] >= 0) || !std::isfinite(epsv[c])) { gs_set_error(h, std::string(who) + ": epsilon must be >= 0"); return GS_ERR_ARG; }
     }
     GS_CUDA(cudaSetDevice(h->device));
     cudaStream_t st = h->stream;
@@ -99,9 +103,9 @@ static int svr_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
             if (refit || h->is_train(r, k)) rs.push_back(r);
         }
         const int l = (int)rs.size();
-        if (l == 0) { gs_set_error(h, "gs_svr: a split has no training rows"); return GS_ERR_ARG; }
+        if (l == 0) { gs_set_error(h, std::string(who) + ": a split has no training rows"); return GS_ERR_ARG; }
         if (2 * l > smo_max_rows()) {
-            gs_set_error(h, "gs_svr: a fit on " + std::to_string(l) + " training rows exceeds the SVR kernel limit of " +
+            gs_set_error(h, std::string(who) + ": a fit on " + std::to_string(l) + " training rows exceeds the SVR kernel limit of " +
                                 std::to_string(smo_max_rows() / 2));
             return GS_ERR_UNSUPPORTED;
         }
@@ -110,7 +114,7 @@ static int svr_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
         lmax = std::max(lmax, 2 * l);
     }
     sp_off[n_splits] = (int)rows_all.size();
-    if (const int rc = search.group("gs_svr", n_cand, n_splits, kernel, gamma, nullptr, nullptr)) return rc;   // groups by kernel matrix (kernel, gamma)
+    if (const int rc = search.group(who, n_cand, n_splits, kernel, gamma, nullptr, nullptr)) return rc;   // groups by kernel matrix (kernel, gamma)
 
     // ---- per-split sizes and r2 denominators (they depend on the split only) ----
     std::vector<double> tss((size_t)n_splits * 2, 0.0), cnt((size_t)n_splits * 2, 0.0);
@@ -161,6 +165,7 @@ static int svr_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
         // ---- 3. one problem per (candidate, split), ordered by group: column index == problem index ----
         std::vector<SmoProblem> probs;
         std::vector<SvrData> svr;
+        std::vector<NuData> nud;
         std::vector<int> prob_task, group_first(g1 - g0 + 1, 0);
         std::vector<VoteTask> vtasks;
         for (int g = g0; g < g1; g++) {
@@ -180,14 +185,20 @@ static int svr_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
                 P.shrinking = (flags & GS_NO_SHRINKING) ? 0 : 1;
                 P.guard = search.d_guard;
                 probs.push_back(P);
-                svr.push_back(SvrData{h->dZ64.as<double>(), epsv[c]});
+                if (nu) {                                     // svm.cpp:1809-1815: linear term -/+ z, sum of C x nu in row order, halved
+                    double sum = 0;
+                    for (int r = 0; r < P.l / 2; r++) sum += Cv[c] * epsv[c];
+                    sum /= 2;
+                    nud.push_back(NuData{sum, sum});
+                    svr.push_back(SvrData{h->dZ64.as<double>(), 0.0});
+                } else svr.push_back(SvrData{h->dZ64.as<double>(), epsv[c]});
                 prob_task.push_back(t);
             }
         }
         group_first[g1 - g0] = (int)probs.size();
         const int np = (int)probs.size();
         if (const int rc = search.workspaces(probs)) return rc;
-        const size_t meta_bytes = (size_t)np * (sizeof(SmoProblem) + sizeof(SvrData) + 4) + vtasks.size() * sizeof(VoteTask) + 256;
+        const size_t meta_bytes = (size_t)np * (sizeof(SmoProblem) + sizeof(SvrData) + sizeof(NuData) + 4) + vtasks.size() * sizeof(VoteTask) + 256;
         GS_CUDA(h->dWork[6].reserve(meta_bytes));
         GS_CUDA(h->dScore.reserve((size_t)np * 2 * 8));                   // rss[np][2]
         // ---- 4. launch order: longest predicted first.  There is no iteration model for SVR yet; C x l orders the
@@ -205,6 +216,12 @@ static int svr_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
         int *d_order = (int *)(dmeta + off);
         off = (off + (size_t)np * 4 + 15) & ~(size_t)15;
         VoteTask *d_vt = (VoteTask *)(dmeta + off);
+        off = (off + vtasks.size() * sizeof(VoteTask) + 15) & ~(size_t)15;
+        NuData *d_nu = (NuData *)(dmeta + off);
+        if (nu) {
+            GS_CUDA(cudaMemcpyAsync(d_nu, nud.data(), nud.size() * sizeof(NuData), cudaMemcpyHostToDevice, st));
+            pf.h2d_bytes += nud.size() * sizeof(NuData);
+        }
         GS_CUDA(cudaMemcpyAsync(d_probs, probs.data(), (size_t)np * sizeof(SmoProblem), cudaMemcpyHostToDevice, st));
         GS_CUDA(cudaMemcpyAsync(d_svr, svr.data(), (size_t)np * sizeof(SvrData), cudaMemcpyHostToDevice, st));
         GS_CUDA(cudaMemcpyAsync(d_order, order.data(), (size_t)np * 4, cudaMemcpyHostToDevice, st));
@@ -215,9 +232,10 @@ static int svr_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
         // ---- 5. solve: one launch per instance (branch-free first, then the guarded general one) ----
         for (int inst = search.fast ? 1 : 0; inst >= 0; inst--) {
             std::string why;
-            const cudaError_t ce = launch_smo_svr(d_probs, d_svr, d_order, np, lmax, inst == 1, (int)ldk, st, &why);
+            const cudaError_t ce = nu ? launch_smo_nu(d_probs, d_svr, d_nu, d_order, np, lmax, inst == 1, st, &why)
+                                      : launch_smo_svr(d_probs, d_svr, d_order, np, lmax, inst == 1, (int)ldk, st, &why);
             if (ce != cudaSuccess) {
-                gs_set_error(h, why.empty() ? std::string("launch_smo_svr: ") + cudaGetErrorString(ce) : why);
+                gs_set_error(h, why.empty() ? std::string(nu ? "launch_smo_nu: " : "launch_smo_svr: ") + cudaGetErrorString(ce) : why);
                 return why.empty() ? GS_ERR_CUDA : GS_ERR_UNSUPPORTED;
             }
             pf.launches++;
@@ -247,7 +265,7 @@ static int svr_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
             total_iter += info[(size_t)q * 4];
             // two gathered K rows per iteration, over the problem's l / 2 distinct columns
             solve_bytes += (double)info[(size_t)q * 4] * 2.0 * (probs[q].l / 2) * 4.0;
-            if (!std::isfinite(rho[q])) { if (refit) { gs_set_error(h, "gs_svr_refit: non-finite intercept"); return GS_ERR_NUMERIC; } task_bad[t] = 1; }
+            if (!std::isfinite(rho[q])) { if (refit) { gs_set_error(h, std::string(who) + "_refit: non-finite intercept"); return GS_ERR_NUMERIC; } task_bad[t] = 1; }
         }
         if (refit) {
             if (rho_out) *rho_out = rho[0];
@@ -307,7 +325,7 @@ int gs_svr(gs_handle *h, int32_t n_cand, const int32_t *kernel, const double *C,
            int32_t *n_sv, float *fit_ms, float *score_ms)
 {
     if (h && !test_scores) { gs_set_error(h, "gs_svr: test_scores is NULL"); return GS_ERR_ARG; }
-    return svr_run(h, n_cand, kernel, C, epsilon, gamma, tol, max_iter, flags, false, test_scores,
+    return svr_run(h, n_cand, kernel, C, epsilon, gamma, tol, max_iter, flags, false, false, test_scores,
                    (flags & GS_RETURN_TRAIN) ? train_scores : nullptr, n_iter, n_sv, fit_ms, score_ms, nullptr, nullptr);
 }
 
@@ -315,7 +333,24 @@ int gs_svr_refit(gs_handle *h, int32_t kernel, double C, double epsilon, double 
                  uint32_t flags, double *coef, double *rho, int32_t *n_iter)
 {
     const int32_t k = kernel;
-    return svr_run(h, 1, &k, &C, &epsilon, &gamma, tol, max_iter, flags, true, nullptr, nullptr, n_iter, nullptr, nullptr,
+    return svr_run(h, 1, &k, &C, &epsilon, &gamma, tol, max_iter, flags, true, false, nullptr, nullptr, n_iter, nullptr, nullptr,
+                   nullptr, coef, rho);
+}
+
+int gs_nusvr(gs_handle *h, int32_t n_cand, const int32_t *kernel, const double *C, const double *nu, const double *gamma,
+             double tol, int32_t max_iter, uint32_t flags, double *test_scores, double *train_scores, int32_t *n_iter,
+             int32_t *n_sv, float *fit_ms, float *score_ms)
+{
+    if (h && !test_scores) { gs_set_error(h, "gs_nusvr: test_scores is NULL"); return GS_ERR_ARG; }
+    return svr_run(h, n_cand, kernel, C, nu, gamma, tol, max_iter, flags, false, true, test_scores,
+                   (flags & GS_RETURN_TRAIN) ? train_scores : nullptr, n_iter, n_sv, fit_ms, score_ms, nullptr, nullptr);
+}
+
+int gs_nusvr_refit(gs_handle *h, int32_t kernel, double C, double nu, double gamma, double tol, int32_t max_iter,
+                   uint32_t flags, double *coef, double *rho, int32_t *n_iter)
+{
+    const int32_t k = kernel;
+    return svr_run(h, 1, &k, &C, &nu, &gamma, tol, max_iter, flags, true, true, nullptr, nullptr, n_iter, nullptr, nullptr,
                    nullptr, coef, rho);
 }
 

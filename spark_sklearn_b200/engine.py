@@ -77,6 +77,8 @@ def load_library():
     L.gs_set_data.argtypes = [vp, vp, i32, i64, i64, vp, vp, vp, i32]
     L.gs_svc.argtypes = [vp, i32, vp, vp, vp, dbl, i32, u32, vp, vp, vp, vp, vp, vp]
     L.gs_svc_refit.argtypes = [vp, i32, dbl, dbl, dbl, i32, u32, vp, vp, vp]
+    L.gs_nusvc.argtypes = L.gs_svc.argtypes
+    L.gs_nusvc_refit.argtypes = L.gs_svc_refit.argtypes
     L.gs_ridge.argtypes = [vp, i32, vp, i32, u32, vp, vp, vp, vp]
     L.gs_ridge_refit.argtypes = [vp, dbl, i32, vp]
     L.gs_enet.argtypes = [vp, i32, vp, vp, i32, dbl, i32, u32, vp, vp, vp, vp, vp]
@@ -84,6 +86,8 @@ def load_library():
     L.gs_set_targets_f64.argtypes = [vp, vp]
     L.gs_svr.argtypes = [vp, i32, vp, vp, vp, vp, dbl, i32, u32, vp, vp, vp, vp, vp, vp]
     L.gs_svr_refit.argtypes = [vp, i32, dbl, dbl, dbl, dbl, i32, u32, vp, vp, vp]
+    L.gs_nusvr.argtypes = L.gs_svr.argtypes
+    L.gs_nusvr_refit.argtypes = L.gs_svr_refit.argtypes
     L.gs_logreg.argtypes = [vp, i32, vp, dbl, i32, i32, u32, vp, vp, vp, vp, vp]
     L.gs_logreg_refit.argtypes = [vp, dbl, dbl, i32, i32, vp, vp]
     L.gs_linsvc.argtypes = [vp, i32, vp, dbl, i32, i32, dbl, u32, vp, vp, vp, vp, vp]
@@ -105,7 +109,7 @@ def load_library():
     L.gs_svc_schedule.argtypes = [vp, i32, i32, vp, vp]
     L.gs_svc_schedule.restype = None
     for f in ("gs_create", "gs_set_data", "gs_svc", "gs_svc_refit", "gs_ridge", "gs_ridge_refit", "gs_enet", "gs_enet_refit", "gs_set_targets_f64",
-              "gs_svr", "gs_svr_refit", "gs_logreg",
+              "gs_svr", "gs_svr_refit", "gs_nusvc", "gs_nusvc_refit", "gs_nusvr", "gs_nusvr_refit", "gs_logreg",
               "gs_logreg_refit", "gs_linsvc", "gs_linsvc_refit", "gs_get_profile", "gs_debug_gram", "gs_debug_kernel_matrix",
               "gs_debug_decision", "gs_debug_score", "gs_debug_linear", "gs_debug_gemm_nt", "gs_debug_gemm_f64", "gs_knn", "gs_debug_knn_neighbors"):
         getattr(L, f).restype = c.c_int
@@ -231,19 +235,23 @@ class Engine:
         finally:
             self._L.gs_set_kernel_params(self._h, None, None, 0)
 
-    def svc(self, kernel, C, gamma, tol=1e-3, max_iter=-1, shrinking=True, return_train=True, flags=0, degree=None, coef0=None):
-        """degree / coef0: scalars or one per candidate, read by the poly and sigmoid candidates (defaults 3 / 0.0)"""
+    def svc(self, kernel, C, gamma, tol=1e-3, max_iter=-1, shrinking=True, return_train=True, flags=0, degree=None, coef0=None,
+            nu=False):
+        """degree / coef0: scalars or one per candidate, read by the poly and sigmoid candidates (defaults 3 / 0.0).
+        nu=True: NuSVC (gs_nusvc), C holds nu; a fit that is infeasible for its nu scores NaN with n_iter -1."""
         ids = [KERNEL_ID[k] if isinstance(k, str) else int(k) for k in kernel]
         return self._with_kernel_params(ids, degree, coef0, lambda: self._kernel_svm(
-            self._L.gs_svc, ids, C, [], gamma, tol, max_iter, shrinking, return_train, flags))
+            self._L.gs_nusvc if nu else self._L.gs_svc, ids, C, [], gamma, tol, max_iter, shrinking, return_train, flags))
 
-    def svc_refit(self, kernel, C, gamma, n_classes, tol=1e-3, max_iter=-1, shrinking=True, degree=3, coef0=0.0):
+    def svc_refit(self, kernel, C, gamma, n_classes, tol=1e-3, max_iter=-1, shrinking=True, degree=3, coef0=0.0, nu=False):
+        """nu=True: NuSVC (gs_nusvc_refit), C holds nu"""
         n_pairs = n_classes * (n_classes - 1) // 2
         coef = np.zeros((n_pairs, self.n))
         rho = np.zeros(n_pairs)
         it = np.zeros(n_pairs, np.int32)
         k = KERNEL_ID[kernel] if isinstance(kernel, str) else int(kernel)
-        self._with_kernel_params([k], degree, coef0, lambda: self._check(self._L.gs_svc_refit(
+        fn = self._L.gs_nusvc_refit if nu else self._L.gs_svc_refit
+        self._with_kernel_params([k], degree, coef0, lambda: self._check(fn(
             self._h, k, float(C), float(gamma), float(tol), int(max_iter), 0 if shrinking else GS_NO_SHRINKING, _ptr(coef),
             _ptr(rho), _ptr(it))))
         return coef, rho, it
@@ -255,18 +263,21 @@ class Engine:
             raise ValueError("y has shape %r; expected (%d,)" % (y.shape, self.n))
         self._check(self._L.gs_set_targets_f64(self._h, _ptr(y)))
 
-    def svr(self, kernel, C, epsilon, gamma, tol=1e-3, max_iter=-1, shrinking=True, return_train=True, flags=0):
+    def svr(self, kernel, C, epsilon, gamma, tol=1e-3, max_iter=-1, shrinking=True, return_train=True, flags=0, nu=False):
+        """nu=True: NuSVR (gs_nusvr), epsilon holds nu"""
         epsilon = np.ascontiguousarray(np.broadcast_to(np.asarray(epsilon, np.float64), (len(C),)))
-        return self._kernel_svm(self._L.gs_svr, kernel, C, [epsilon], gamma, tol, max_iter, shrinking, return_train, flags)
+        return self._kernel_svm(self._L.gs_nusvr if nu else self._L.gs_svr, kernel, C, [epsilon], gamma, tol, max_iter, shrinking,
+                                return_train, flags)
 
-    def svr_refit(self, kernel, C, epsilon, gamma, tol=1e-3, max_iter=-1, shrinking=True, flags=0):
-        """-> (coef [n] by row: alpha+ - alpha-, rho, n_iter); prediction = sum coef k(x, x_row) - rho"""
+    def svr_refit(self, kernel, C, epsilon, gamma, tol=1e-3, max_iter=-1, shrinking=True, flags=0, nu=False):
+        """-> (coef [n] by row: alpha+ - alpha-, rho, n_iter); prediction = sum coef k(x, x_row) - rho.  nu=True: NuSVR,
+        epsilon holds nu."""
         coef = np.zeros(self.n)
         rho = np.zeros(1)
         it = np.zeros(1, np.int32)
         k = KERNEL_ID[kernel] if isinstance(kernel, str) else int(kernel)
         fl = int(flags) | (0 if shrinking else GS_NO_SHRINKING)
-        self._check(self._L.gs_svr_refit(self._h, k, float(C), float(epsilon), float(gamma), float(tol), int(max_iter),
+        self._check((self._L.gs_nusvr_refit if nu else self._L.gs_svr_refit)(self._h, k, float(C), float(epsilon), float(gamma), float(tol), int(max_iter),
                                          fl, _ptr(coef), _ptr(rho), _ptr(it)))
         return coef, float(rho[0]), int(it[0])
 

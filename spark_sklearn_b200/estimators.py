@@ -96,12 +96,16 @@ def adapter_for(estimator):
     from sklearn.linear_model import ElasticNet, Lasso, LogisticRegression, Ridge
     from sklearn.neighbors import KNeighborsClassifier, KNeighborsRegressor
     from sklearn.pipeline import Pipeline
-    from sklearn.svm import SVC, SVR, LinearSVC
+    from sklearn.svm import SVC, SVR, LinearSVC, NuSVC, NuSVR
     t = type(estimator)
     if t is SVC:
         return SVCAdapter
     if t is SVR:
         return SVRAdapter
+    if t is NuSVC:
+        return NuSVCAdapter
+    if t is NuSVR:
+        return NuSVRAdapter
     if t is Ridge:
         return RidgeAdapter
     if t is LogisticRegression:
@@ -117,7 +121,7 @@ def adapter_for(estimator):
         # (python/spark_sklearn/tests/test_search_2.py:69-93): the step's adapter runs, the names are translated
         return PipelineAdapter(estimator.steps[0][0], adapter_for(estimator.steps[0][1]))
     raise NotImplementedError(
-        "spark_sklearn_b200 has CUDA paths for SVC, SVR, Ridge, Lasso, ElasticNet, LogisticRegression, LinearSVC, "
+        "spark_sklearn_b200 has CUDA paths for SVC, SVR, NuSVC, NuSVR, Ridge, Lasso, ElasticNet, LogisticRegression, LinearSVC, "
         "KNeighborsClassifier and KNeighborsRegressor (bare or as the only step of a Pipeline); got %s (no CPU fallback)"
         % t.__name__)
 
@@ -297,6 +301,10 @@ class _KernelGamma:
             raise ValueError("gamma must be >= 0 or 'scale'/'auto'; got %r" % (g,))
         return float(g)
 
+    def _nu_kw(self):
+        """engine keyword of the nu solvers (NuSVCPlan / NuSVRPlan set nu = True)"""
+        return {"nu": True} if self.nu else {}
+
     def _flags(self):
         import os
         # B200GS_GRAM=tensor: opt-in wgmma Gram (fp32-faithful; scores match to solver tolerance, not bit for bit)
@@ -318,6 +326,9 @@ class SVCPlan(_KernelGamma, _Plan):
         self._set_data(self.X, y_class=self.y_class.astype(np.int32))
         self._var_cache = {}
 
+    nu = False                 # NuSVCPlan: the nu-SVC solver, with nu where SVC has C
+    penalty = "C"
+
     def _check(self, p):
         if p["kernel"] not in ("rbf", "linear", "poly", "sigmoid"):
             raise NotImplementedError("SVC kernel=%r has no CUDA path (linear, rbf, poly and sigmoid do)" % (p["kernel"],))
@@ -332,6 +343,9 @@ class SVCPlan(_KernelGamma, _Plan):
             raise NotImplementedError("SVC probability=True is not supported by the CUDA path")
         if p.get("break_ties"):
             raise NotImplementedError("SVC break_ties=True is not supported by the CUDA path")
+        self._check_penalty(p)
+
+    def _check_penalty(self, p):
         if not (isinstance(p["C"], numbers.Real) and p["C"] > 0):
             raise ValueError("C must be a positive number; got %r" % (p["C"],))
 
@@ -369,13 +383,14 @@ class SVCPlan(_KernelGamma, _Plan):
         for (tol, max_iter, shrinking, _cwk), idx in groups.items():
             self._set_class_weight(params[idx[0]].get("class_weight"))
             kern = [params[j]["kernel"] for j in idx]
-            C = [float(params[j]["C"]) for j in idx]
+            C = [float(params[j][self.penalty]) for j in idx]
             gam = np.array([[self._gamma(params[j]["gamma"], k) if params[j]["kernel"] != "linear" else 0.0
                              for k in range(ns)] for j in idx])
             self.engine.set_scoring(self.score_kind, self.score_pos)
             r = self.engine.svc(kern, C, gam, tol=tol, max_iter=max_iter, shrinking=shrinking,
                                 return_train=return_train, flags=self._flags(),
-                                degree=[int(params[j]["degree"]) for j in idx], coef0=[float(params[j]["coef0"]) for j in idx])
+                                degree=[int(params[j]["degree"]) for j in idx], coef0=[float(params[j]["coef0"]) for j in idx],
+                                **self._nu_kw())
             for key in ("test", "fit_ms", "score_ms", "n_iter"):
                 res[key][idx] = r[key]
             if return_train:
@@ -392,9 +407,10 @@ class SVCPlan(_KernelGamma, _Plan):
         self._check(p)
         gamma = self._gamma(p["gamma"], -1)          # all rows train (svm/_base.py:278-286)
         cw_ = self._set_class_weight(p.get("class_weight"), refit=True)
-        coef, rho, n_iter = self.engine.svc_refit(p["kernel"], p["C"], gamma if p["kernel"] != "linear" else 0.0,
+        coef, rho, n_iter = self.engine.svc_refit(p["kernel"], p[self.penalty], gamma if p["kernel"] != "linear" else 0.0,
                                                   len(self.classes), tol=p["tol"], max_iter=p["max_iter"],
-                                                  shrinking=p["shrinking"], degree=int(p["degree"]), coef0=float(p["coef0"]))
+                                                  shrinking=p["shrinking"], degree=int(p["degree"]), coef0=float(p["coef0"]),
+                                                  **self._nu_kw())
         self.engine.set_class_weight(None)
         est = clone(self.estimator).set_params(**best_params)
         est = materialize_svc(est, self.X, self.y_class, self.classes, coef, rho, n_iter, gamma)
@@ -445,6 +461,49 @@ def materialize_svc(est, X, y_class, classes, pair_coef, rho, n_iter, gamma):
     return est
 
 
+# ------------------------------------------------------------------ NuSVC ---------------------
+class NuSVCAdapter(SVCAdapter):
+    @staticmethod
+    def plan(estimator, cands, X, y, fold_id, n_splits, device=None):
+        return NuSVCPlan(estimator, cands, X, y, fold_id, n_splits, device)
+
+
+class NuSVCPlan(SVCPlan):
+    """sklearn.svm.NuSVC (libsvm's nu-SVC): SVCPlan with nu in place of C.  class_weight is accepted and reported in
+    class_weight_ but, as in libsvm, does not change a nu-SVC fit."""
+    nu = True
+    penalty = "nu"
+
+    def _check_penalty(self, p):
+        type(self.estimator)(**p)._validate_params()          # scikit-learn's own ValueError, e.g. nu outside (0, 1]
+
+    def _infeasible(self, nu, k):
+        """libsvm svm_check_parameter: nu is infeasible for the training rows of split k (k < 0: all rows) when some class
+        pair has nu (n1 + n2) / 2 > min(n1, n2)"""
+        n = np.bincount(self.y_class[self._train_rows(k)], minlength=len(self.classes)).astype(np.float64)
+        n = n[n > 0]
+        return any(nu * (n[a] + n[b]) / 2 > min(n[a], n[b]) for a in range(len(n)) for b in range(a + 1, len(n)))
+
+    def costs(self):
+        return None                                           # no iteration model for nu-SVC: candidates are dealt uniformly
+
+    def evaluate(self, my, return_train=True, error_score='raise'):
+        if error_score == 'raise':                            # scikit-learn's fit raises before any solve
+            for ci in my:
+                p = self._base_params(self.cands[ci])
+                self._check(p)
+                if any(self._infeasible(float(p["nu"]), k) for k in range(self.n_splits)):
+                    raise ValueError("specified nu is infeasible")
+        return super().evaluate(my, return_train, error_score)
+
+    def refit(self, best_params):
+        p = self._base_params(best_params)
+        self._check(p)
+        if self._infeasible(float(p["nu"]), -1):
+            raise ValueError("specified nu is infeasible")
+        return super().refit(best_params)
+
+
 # ------------------------------------------------------------------ SVR -----------------------
 class SVRAdapter:
     multi_device = True        # plan(..., device=d): one plan per GPU of the in-process scheduler
@@ -476,9 +535,15 @@ class SVRPlan(_KernelGamma, _Plan):
         self._set_data(self.X, y_target=self.y.astype(np.float32))
         self.engine.set_targets_f64(self.y)
 
+    nu = False                 # NuSVRPlan: the nu-SVR solver, with nu where SVR has epsilon
+    tube = "epsilon"
+
     def _check(self, p):
         if p["kernel"] not in ("rbf", "linear"):
-            raise NotImplementedError("SVR kernel=%r has no CUDA path (rbf and linear do)" % (p["kernel"],))
+            raise NotImplementedError("%s kernel=%r has no CUDA path (rbf and linear do)" % (type(self.estimator).__name__, p["kernel"]))
+        self._check_tube(p)
+
+    def _check_tube(self, p):
         if not (isinstance(p["C"], numbers.Real) and p["C"] > 0):
             raise ValueError("C must be a positive number; got %r" % (p["C"],))
         if not (isinstance(p["epsilon"], numbers.Real) and p["epsilon"] >= 0):
@@ -489,7 +554,8 @@ class SVRPlan(_KernelGamma, _Plan):
     def _check_rows(self, k):
         m = int(np.count_nonzero(self._train_rows(k)))
         if m > self.max_rows:
-            raise NotImplementedError("SVR fit on %d training rows: the CUDA solver handles up to %d" % (m, self.max_rows))
+            raise NotImplementedError("%s fit on %d training rows: the CUDA solver handles up to %d"
+                                      % (type(self.estimator).__name__, m, self.max_rows))
 
     def check_refit(self):
         """the refit trains on every row: raise before the search when that fit is too large"""
@@ -513,12 +579,12 @@ class SVRPlan(_KernelGamma, _Plan):
         for (tol, max_iter, shrinking), idx in groups.items():
             kern = [params[j]["kernel"] for j in idx]
             C = [float(params[j]["C"]) for j in idx]
-            eps = [float(params[j]["epsilon"]) for j in idx]
+            eps = [float(params[j][self.tube]) for j in idx]
             gam = np.array([[self._gamma(params[j]["gamma"], k) if params[j]["kernel"] == "rbf" else 0.0
                              for k in range(ns)] for j in idx])
             self.engine.set_scoring(self.score_kind, self.score_pos)
             r = self.engine.svr(kern, C, eps, gam, tol=tol, max_iter=max_iter, shrinking=shrinking,
-                                return_train=return_train, flags=self._flags())
+                                return_train=return_train, flags=self._flags(), **self._nu_kw())
             for key in ("test", "fit_ms", "score_ms", "n_iter"):
                 res[key][idx] = r[key]
             if return_train:
@@ -534,9 +600,9 @@ class SVRPlan(_KernelGamma, _Plan):
         self._check(p)
         self._check_rows(-1)
         gamma = self._gamma(p["gamma"], -1)          # all rows train (svm/_base.py:278-286)
-        coef, rho, n_iter = self.engine.svr_refit(p["kernel"], p["C"], p["epsilon"], gamma if p["kernel"] == "rbf" else 0.0,
+        coef, rho, n_iter = self.engine.svr_refit(p["kernel"], p["C"], p[self.tube], gamma if p["kernel"] == "rbf" else 0.0,
                                                   tol=p["tol"], max_iter=p["max_iter"], shrinking=p["shrinking"],
-                                                  flags=self._flags())
+                                                  flags=self._flags(), **self._nu_kw())
         est = clone(self.estimator).set_params(**best_params)
         est = materialize_svr(est, self.X, coef, rho, n_iter, gamma)
         if p["max_iter"] != -1 and n_iter >= p["max_iter"]:        # svm/_base.py: fit_status_ 1 and its warning
@@ -572,6 +638,22 @@ def materialize_svr(est, X, coef, rho, n_iter, gamma):
     est.shape_fit_ = X.shape
     est.n_features_in_ = X.shape[1]
     return est
+
+
+# ------------------------------------------------------------------ NuSVR ---------------------
+class NuSVRAdapter(SVRAdapter):
+    @staticmethod
+    def plan(estimator, cands, X, y, fold_id, n_splits, device=None):
+        return NuSVRPlan(estimator, cands, X, y, fold_id, n_splits, device)
+
+
+class NuSVRPlan(SVRPlan):
+    """sklearn.svm.NuSVR (libsvm's nu-SVR): SVRPlan with nu in place of epsilon; materialize_svr builds the fitted NuSVR."""
+    nu = True
+    tube = "nu"
+
+    def _check_tube(self, p):
+        type(self.estimator)(**p)._validate_params()          # scikit-learn's own ValueError, e.g. nu outside (0, 1]
 
 
 # ------------------------------------------------------------------ Ridge ---------------------

@@ -95,6 +95,14 @@ def _svc_kernels(n=3000, d=128, cv=5, name="svc_kernels_mid"):
     return dict(name=name, X=X, y=y, estimator="SVC", est_params={}, param_grid=grid, cv=cv, search="grid")
 
 
+def _nusvc(n=1000, d=64, grid=None, cv=5, name="nusvc_small"):
+    """NuSVC on the config-2 data recipe; nusvc_c2 is config 2's data with an 8 x 8 nu x gamma grid."""
+    X, y = _svc_data(n, d)
+    if grid is None:
+        grid = {"nu": [0.1, 0.3, 0.5, 0.7], "gamma": [8.0 / (d * 64), 8.0 / (d * 4), "scale"]}
+    return dict(name=name, X=X, y=y, estimator="NuSVC", est_params={"kernel": "rbf"}, param_grid=grid, cv=cv, search="grid")
+
+
 def _linsvc(which="small"):
     """LinearSVC (primal TRON): the config-3 data with 8 C values (small), a 3-class set (multi), and config 3's own
     search shape on its data (c3: 256 random C candidates x 5 folds = 1280 fits of 40000 x 256, all primal)."""
@@ -164,6 +172,19 @@ WORKLOADS = {
                                                  "epsilon": [0.1]}, name="svr_mid"),
     "svr_c6": lambda: _svr(n=10000, d=512, grid={"C": np.logspace(-1, 2.5, 8), "gamma": np.geomspace(1.0 / 4096, 1.0 / 256, 8),
                                                  "epsilon": [0.1]}, name="svr_c6"),
+    # NuSVC / NuSVR (libsvm's Solver_NU on the position-owned SMO kernel): nusvc_c2 is the measurement config (tools/bench_nu.py)
+    "nusvc_small": _nusvc,
+    "nusvc_mid": lambda: _nusvc(n=3000, d=128, grid=[{"nu": [0.2, 0.5], "gamma": [1.0 / 512, "scale"]},
+                                                     {"kernel": ["poly"], "nu": [0.3], "degree": [2, 3], "coef0": [1.0]},
+                                                     {"kernel": ["sigmoid"], "nu": [0.3], "gamma": [1.0 / 1024], "coef0": [0.0]},
+                                                     {"kernel": ["linear"], "nu": [0.4]},
+                                                     {"nu": [1.0]}], name="nusvc_mid"),   # nu = 1: infeasible on unequal folds
+    "nusvc_c2": lambda: _nusvc(n=10000, d=512, grid={"nu": np.linspace(0.1, 0.8, 8), "gamma": np.geomspace(1.0 / 4096, 1.0 / 256, 8)},
+                               name="nusvc_c2"),
+    "nusvr_small": lambda: dict(_svr(grid={"nu": [0.1, 0.5, 0.9], "C": [1.0, 10.0], "gamma": [1.0 / 32, "scale"]},
+                                     name="nusvr_small"), estimator="NuSVR"),
+    "nusvr_mid": lambda: dict(_svr(n=5000, d=128, grid={"nu": [0.2, 0.5, 0.8], "C": [0.3, 3.0, 30.0], "gamma": [1.0 / 1024, "scale"]},
+                                   name="nusvr_mid"), estimator="NuSVR"),
     # SVC poly / sigmoid: the golden-sized grid and the same grid on config-2 data (tools/bench_kernels.py)
     "svc_kernels_mid": _svc_kernels,
     "svc_kernels_c2": lambda: _svc_kernels(n=10000, d=512, name="svc_kernels_c2"),
@@ -198,6 +219,9 @@ def make_estimator(w):
     if w["estimator"] == "SVR":
         from sklearn.svm import SVR
         return SVR(**w["est_params"])
+    if w["estimator"] in ("NuSVC", "NuSVR"):
+        import sklearn.svm as svm
+        return getattr(svm, w["estimator"])(**w["est_params"])
     if w["estimator"] == "LinearSVC":
         from sklearn.svm import LinearSVC
         return LinearSVC(**w["est_params"])
