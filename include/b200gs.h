@@ -345,6 +345,37 @@ int gs_debug_linear(gs_handle *h, int32_t mode, int32_t n_cand, const double *al
 
 /* C[M][N] = sum_k A[M][k]*B[N][k] on the wgmma tensor-core path (3xTF32 split), host fp32 row-major in/out. */
 int gs_debug_gemm_nt(gs_handle *h, const float *A, int32_t M, const float *B, int32_t N, int32_t K, float *C);
+/*
+ * LinearSVR (csrc/linsvr.cu).  Replaces: sklearn.svm.LinearSVR.fit / score per (candidate, split) (reference
+ * base_search.py:83-87) with liblinear's three SVR solvers, chosen per fit by solver[c * n_splits + k]:
+ *   11 L2R_L2LOSS_SVR       TRON on the FP64 tensor-core contractions (gs_linsvc's rounds), eps = tol
+ *   12 L2R_L2LOSS_SVR_DUAL  dual coordinate descent, lambda_i = 0.5 / C_i, no bound          } one warp per fit, w in
+ *   13 L2R_L1LOSS_SVR_DUAL  dual coordinate descent, lambda 0, |beta_i| <= C_i               } registers (d <= 512)
+ * C_i = C x sample weight (gs_set_sample_weight); rows of zero weight are dropped in order.  seed[c * n_splits + k]: the
+ * seed of the fit's std::mt19937 (scikit-learn's check_random_state(random_state).randint(INT_MAX)), which shuffles the
+ * CD's training positions every epoch.  The positions are the split's training rows in gs_set_train_order's order
+ * (default: ascending).  The bias is a feature of value intercept_scaling when fit_intercept.  Needs a regression
+ * gs_set_data and gs_set_targets_f64.  Scores: GS_SCORE_DEFAULT (r2), GS_SCORE_NEG_MSE, GS_SCORE_NEG_RMSE on the float64
+ * decision values of one forward contraction.  n_iter [n_cand][n_splits]: LinearSVR.n_iter_ of each fit.
+ * Test hooks: coef_out (may be NULL) [n_cand][n_splits][d + 1] every fit's raw weights (the bias feature's last, 0 without
+ * an intercept); cd_stats (may be NULL) [n_cand][n_splits][3] = coordinate steps, clock cycles in the per-epoch shuffles,
+ * clock cycles of the whole CD fit (0 for TRON fits).
+ * gs_linsvr_refit: one fit on every row (in row order): coef_out [d + 1] raw weights, n_iter [1].
+ */
+#define GS_LINSVR_MAX_FEATURES 512
+int gs_linsvr(gs_handle *h, int32_t n_cand, const double *C, const double *epsilon, const int32_t *solver, const uint32_t *seed,
+              double tol, int32_t max_iter, int32_t fit_intercept, double intercept_scaling, uint32_t flags, double *test_scores,
+              double *train_scores, int32_t *n_iter, float *fit_ms, float *score_ms, double *coef_out, int64_t *cd_stats);
+int gs_linsvr_refit(gs_handle *h, double C, double epsilon, int32_t solver, uint32_t seed, double tol, int32_t max_iter,
+                    int32_t fit_intercept, double intercept_scaling, double *coef_out, int32_t *n_iter);
+/* The order in which every split's training rows enter a fit that depends on it (LinearSVR's CD: liblinear shuffles
+ * positions 0..l-1 of X[train], so the order of the splitter's train indices is part of the result).  rows: original row
+ * indices, split k's at rows[offsets[k] .. offsets[k + 1]); each list must hold exactly the split's training rows.  Call
+ * after gs_set_data / gs_set_splits, which reset it; NULL resets it to ascending order. */
+int gs_set_train_order(gs_handle *h, const int32_t *rows, const int64_t *offsets, int32_t n_splits);
+/* Test hook: the first k outputs of the device std::mt19937(seed) that gs_linsvr's shuffles draw from. */
+int gs_debug_mt19937(gs_handle *h, uint32_t seed, int32_t k, uint32_t *out);
+
 /* C[M][N] = sum_k A[M][k]*B[N][k] on the FP64 tensor-core path of gs_linsvc (K > 1024: split-K with the fixed-order sum of
  * the partials), host float64 row-major in/out. */
 int gs_debug_gemm_f64(gs_handle *h, const double *A, int32_t M, const double *B, int32_t N, int32_t K, double *C);

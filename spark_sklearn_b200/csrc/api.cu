@@ -77,7 +77,7 @@ __global__ void gather_rows_kernel(const T *__restrict__ src, const int *__restr
 
 extern "C" {
 
-int gs_version(void) { return 106; }
+int gs_version(void) { return 107; }
 
 int gs_set_class_weight(gs_handle *h, const double *w, int32_t n_sets)
 {
@@ -218,6 +218,7 @@ int gs_set_data(gs_handle *h, const void *X, int32_t x_dtype, int64_t n, int64_t
     h->class_w.clear(); h->class_w_sets = 0;
     h->sample_w.clear();
     h->z64.clear();
+    h->train_order.clear(); h->train_off.clear();
     h->kp_degree.clear(); h->kp_coef0.clear();
     h->perm.resize(n);
     std::iota(h->perm.begin(), h->perm.end(), 0);
@@ -308,6 +309,7 @@ int gs_set_splits(gs_handle *h, const uint64_t *test_mask, const uint64_t *train
         }
     }
     h->n_splits = n_splits;
+    h->train_order.clear(); h->train_off.clear();            // a training order belongs to the splits it was given for
     h->partition = false;                                    // fold-block algorithms (Ridge) need gs_set_data's fold ids
     GS_CUDA(cudaMemcpyAsync(h->dTe.p, h->te_mask.data(), (size_t)n * 16, cudaMemcpyHostToDevice, h->stream));
     GS_CUDA(cudaMemcpyAsync(h->dTr.p, h->tr_mask.data(), (size_t)n * 16, cudaMemcpyHostToDevice, h->stream));

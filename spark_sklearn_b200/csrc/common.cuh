@@ -170,6 +170,8 @@ struct gs_handle {
     std::vector<double> kp_coef0;
     std::vector<double> z64;             // gs_set_targets_f64: [n] float64 regression targets, internal order; empty = not set
     DevBuf dZ64;                         // their device copy
+    std::vector<int32_t> train_order;    // gs_set_train_order: training rows (original indices) of every split, in fit order;
+    std::vector<int64_t> train_off;      // split k's are train_order[train_off[k] .. train_off[k + 1]); empty = ascending
     gs_profile prof;
     EventPool evp;                    // timing events of the current call
     TensorTimer tt;
@@ -278,6 +280,11 @@ double gs_score_from_counts(int kind, int pos_class, int n_classes, const int *c
 // (z_r - (dec[first_col][r] - rho[first_col]))^2, float64, fixed-order block reduction (deterministic, no atomics).
 cudaError_t launch_rss(const double *dec, const double *rho, int n, const double *z, SplitMasks sm, const VoteTask *tasks,
                        int n_tasks, double *rss, cudaStream_t st);
+// Per split (0 test, 1 train): row count and total sum of squares of the float64 targets about their mean, in ascending
+// original row order as scikit-learn's y[test] / y[train]
+void regression_split_stats(const gs_handle *h, int n_splits, std::vector<double> &tss, std::vector<double> &cnt);
+// The regression score (r2 / neg MSE / neg RMSE) of one split from its residual sum of squares; NaN for an empty split
+double regression_score(int kind, double rss, double tss, double m);
 
 // ---- kernel_svm.cu: the host steps the SVC and SVR searches share (an int return is a GS_* status) ----
 int build_gram(gs_handle *h, uint32_t flags, cudaStream_t st);   // S = X X^T -> h->dS, diag(S) -> h->dXsq
@@ -335,6 +342,22 @@ struct SvmSearch {                                 // the state of one svc_run /
     int results(int np, bool with_coef);           // downloads the batch's outputs, syncs, collects its phase times
     int finish(int64_t smo_iterations, double solve_bytes);   // end event, sync, the profile's times and totals
 };
+
+// ---- linsvc.cu: liblinear's TRON, one column per fit (LinearSVC, and LinearSVR's primal solver in linsvr.cu) ----
+enum { M_FUN = 0, M_HV = 1, M_DONE = 2 };
+constexpr int PW_BLOCKS = 64;          // row blocks of the element-wise pass: the loss partials of a column, summed in order
+constexpr int NVEC = 5;                // per-column vectors: w, g, s, r, d
+struct TrState {                       // per column
+    int mode, iter, cg_iter, init, cur, fold, pos, n_iter;
+    double Cp, Cn, eps, f, delta, gnorm1, rTr, cgtol;
+};
+// One TRON step of every open column from the gradient contraction Gp ([nchunk] split-K partials) and the loss partials
+// fpart[col][PW_BLOCKS]; the next submission goes to V[col]; *n_open counts the columns still running.
+cudaError_t launch_tron_advance(TrState *St, double *Vec, double *V, const double *Gp, int nchunk, int64_t gp_stride,
+                                const double *fpart, int ncol, int nvp, int max_iter, int *n_open, cudaStream_t st);
+// Xa = [X | bias | 0 ...] in float64 ([npad][nvp], rows >= n zero) and its transpose [nvp][npad]
+cudaError_t launch_build_xa64(const float *X32, const double *X64, int n, int d, double bias, int nvp, int64_t npad, double *Xa,
+                              double *Xat, cudaStream_t st);
 
 // ---- gemm_tc.cu: wgmma + TMA contraction  C[M][N] = sum_k A[M][k] B[N][k]  (3xTF32 split, fp32 accumulate) ----
 struct alignas(64) TcMap { unsigned char bytes[128]; };            // CUtensorMap

@@ -30,15 +30,8 @@
 
 namespace {
 
-enum { M_FUN = 0, M_HV = 1, M_DONE = 2 };
 constexpr double ETA0 = 1e-4, ETA1 = 0.25, ETA2 = 0.75, SIGMA1 = 0.25, SIGMA2 = 0.5, SIGMA3 = 4;
-constexpr int PW_BLOCKS = 64;          // row blocks of the element-wise pass: the loss partials of a column, summed in order
-constexpr int NVEC = 5;                // per-column vectors: w, g, s, r, d
-
-struct TrState {                       // per column
-    int mode, iter, cg_iter, init, cur, fold, pos, n_iter;
-    double Cp, Cn, eps, f, delta, gnorm1, rTr, cgtol;
-};
+// M_FUN / M_HV / M_DONE, PW_BLOCKS, NVEC and TrState are in common.cuh: linsvr.cu drives the same TRON
 
 __device__ __forceinline__ double warp_sum(double v)
 {
@@ -498,6 +491,22 @@ int linsvc_run(gs_handle *h, int n_cand, const double *Cv, double tol, int max_i
 }
 
 }  // namespace
+
+// ---- the TRON pieces linsvr.cu shares (LinearSVR's primal solver, L2R_L2LOSS_SVR) ----
+cudaError_t launch_tron_advance(TrState *St, double *Vec, double *V, const double *Gp, int nchunk, int64_t gp_stride,
+                                const double *fpart, int ncol, int nvp, int max_iter, int *n_open, cudaStream_t st)
+{
+    tron_advance_kernel<<<(ncol + 3) / 4, 128, 0, st>>>(St, Vec, V, Gp, nchunk, gp_stride, fpart, ncol, nvp, max_iter, n_open);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_build_xa64(const float *X32, const double *X64, int n, int d, double bias, int nvp, int64_t npad, double *Xa,
+                              double *Xat, cudaStream_t st)
+{
+    dim3 grid((unsigned)((npad + 31) / 32), (nvp + 31) / 32), block(32, 32);
+    build_xa64_kernel<<<grid, block, 0, st>>>(X32, X64, n, d, bias, nvp, npad, Xa, Xat);
+    return cudaGetLastError();
+}
 
 extern "C" {
 

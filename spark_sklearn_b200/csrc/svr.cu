@@ -57,6 +57,38 @@ cudaError_t launch_rss(const double *dec, const double *rho, int n, const double
     return cudaGetLastError();
 }
 
+void regression_split_stats(const gs_handle *h, int n_splits, std::vector<double> &tss, std::vector<double> &cnt)
+{
+    const int n = (int)h->n;
+    std::vector<int> by_orig(n);
+    for (int r = 0; r < n; r++) by_orig[h->perm[r]] = r;
+    tss.assign((size_t)n_splits * 2, 0.0); cnt.assign((size_t)n_splits * 2, 0.0);
+    for (int k = 0; k < n_splits; k++)
+        for (int sp = 0; sp < 2; sp++) {
+            // np.average then sum of squared deviations, ascending original row order as scikit-learn's y[test] / y[train]
+            double sum = 0, m = 0;
+            for (int o = 0; o < n; o++) {
+                const int r = by_orig[o];
+                if (sp == 0 ? h->is_test(r, k) : (!h->is_test(r, k) && h->is_train(r, k))) { sum += h->z64[r]; m += 1; }
+            }
+            const double mean = m > 0 ? sum / m : 0.0;
+            double s = 0;
+            for (int o = 0; o < n; o++) {
+                const int r = by_orig[o];
+                if (sp == 0 ? h->is_test(r, k) : (!h->is_test(r, k) && h->is_train(r, k))) { const double e = h->z64[r] - mean; s += e * e; }
+            }
+            tss[(size_t)k * 2 + sp] = s; cnt[(size_t)k * 2 + sp] = m;
+        }
+}
+
+double regression_score(int kind, double rss, double tss, double m)
+{
+    if (!(m > 0)) return NAN;
+    if (kind == GS_SCORE_NEG_MSE) return -(rss / m);                       // mean_squared_error
+    if (kind == GS_SCORE_NEG_RMSE) return -std::sqrt(rss / m);             // root_mean_squared_error
+    return gs_r2_score(rss, tss, m);
+}
+
 // nu == false: epsilon-SVR, epsv[c] is epsilon.  nu == true: nu-SVR (svm.cpp solve_nu_svr on Solver_NU), epsv[c] is nu.
 static int svr_run(gs_handle *h, int n_cand, const int32_t *kernel, const double *Cv, const double *epsv, const double *gamma,
                    double tol, int max_iter, uint32_t flags, bool refit, bool nu,
@@ -118,24 +150,7 @@ static int svr_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
 
     // ---- per-split sizes and r2 denominators (they depend on the split only) ----
     std::vector<double> tss((size_t)n_splits * 2, 0.0), cnt((size_t)n_splits * 2, 0.0);
-    if (!refit) {
-        for (int k = 0; k < n_splits; k++)
-            for (int sp = 0; sp < 2; sp++) {
-                // np.average then sum of squared deviations, ascending original row order as scikit-learn's y[test] / y[train]
-                double sum = 0, m = 0;
-                for (int o = 0; o < n; o++) {
-                    const int r = by_orig[o];
-                    if (sp == 0 ? h->is_test(r, k) : (!h->is_test(r, k) && h->is_train(r, k))) { sum += h->z64[r]; m += 1; }
-                }
-                const double mean = m > 0 ? sum / m : 0.0;
-                double s = 0;
-                for (int o = 0; o < n; o++) {
-                    const int r = by_orig[o];
-                    if (sp == 0 ? h->is_test(r, k) : (!h->is_test(r, k) && h->is_train(r, k))) { const double e = h->z64[r] - mean; s += e * e; }
-                }
-                tss[(size_t)k * 2 + sp] = s; cnt[(size_t)k * 2 + sp] = m;
-            }
-    }
+    if (!refit) regression_split_stats(h, n_splits, tss, cnt);
 
     gs_profile &pf = h->prof;
     search.begin();
@@ -280,13 +295,8 @@ static int svr_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
         for (int t = 0; t < n_tasks; t++) {
             const int k = t % n_splits;
             double sc[2];
-            for (int sp = 0; sp < 2; sp++) {
-                const double r = task_rss[(size_t)t * 2 + sp], m = cnt[(size_t)k * 2 + sp];
-                if (!(m > 0)) { sc[sp] = NAN; continue; }
-                if (kind == GS_SCORE_NEG_MSE) sc[sp] = -(r / m);                         // mean_squared_error
-                else if (kind == GS_SCORE_NEG_RMSE) sc[sp] = -std::sqrt(r / m);          // root_mean_squared_error
-                else sc[sp] = gs_r2_score(r, tss[(size_t)k * 2 + sp], m);
-            }
+            for (int sp = 0; sp < 2; sp++)
+                sc[sp] = regression_score(kind, task_rss[(size_t)t * 2 + sp], tss[(size_t)k * 2 + sp], cnt[(size_t)k * 2 + sp]);
             test_scores[t] = task_bad[t] ? NAN : sc[0];
             if (train_scores) train_scores[t] = task_bad[t] ? NAN : sc[1];
             if (n_iter) n_iter[t] = task_iter[t];

@@ -93,6 +93,10 @@ def load_library():
     L.gs_linsvc.argtypes = [vp, i32, vp, dbl, i32, i32, dbl, u32, vp, vp, vp, vp, vp]
     L.gs_linsvc_refit.argtypes = [vp, dbl, dbl, i32, i32, dbl, vp, vp]
     L.gs_debug_gemm_f64.argtypes = [vp, vp, i32, vp, i32, i32, vp]
+    L.gs_linsvr.argtypes = [vp, i32, vp, vp, vp, vp, dbl, i32, i32, dbl, u32, vp, vp, vp, vp, vp, vp, vp]
+    L.gs_linsvr_refit.argtypes = [vp, dbl, dbl, i32, u32, dbl, i32, i32, dbl, vp, vp]
+    L.gs_set_train_order.argtypes = [vp, vp, vp, i32]
+    L.gs_debug_mt19937.argtypes = [vp, u32, i32, vp]
     L.gs_knn.argtypes = [vp, i32, vp, vp, vp, u32, vp, vp, vp, vp]
     L.gs_debug_knn_neighbors.argtypes = [vp, i32, i32, i32, vp, vp]
     L.gs_get_profile.argtypes = [vp, c.POINTER(GsProfile)]
@@ -111,7 +115,8 @@ def load_library():
     for f in ("gs_create", "gs_set_data", "gs_svc", "gs_svc_refit", "gs_ridge", "gs_ridge_refit", "gs_enet", "gs_enet_refit", "gs_set_targets_f64",
               "gs_svr", "gs_svr_refit", "gs_nusvc", "gs_nusvc_refit", "gs_nusvr", "gs_nusvr_refit", "gs_logreg",
               "gs_logreg_refit", "gs_linsvc", "gs_linsvc_refit", "gs_get_profile", "gs_debug_gram", "gs_debug_kernel_matrix",
-              "gs_debug_decision", "gs_debug_score", "gs_debug_linear", "gs_debug_gemm_nt", "gs_debug_gemm_f64", "gs_knn", "gs_debug_knn_neighbors"):
+              "gs_debug_decision", "gs_debug_score", "gs_debug_linear", "gs_debug_gemm_nt", "gs_debug_gemm_f64", "gs_knn", "gs_debug_knn_neighbors",
+              "gs_linsvr", "gs_linsvr_refit", "gs_set_train_order", "gs_debug_mt19937"):
         getattr(L, f).restype = c.c_int
     _lib = L
     return L
@@ -363,6 +368,57 @@ class Engine:
         self._check(self._L.gs_linsvc_refit(self._h, float(C), float(tol), int(max_iter), int(bool(fit_intercept)),
                                             float(intercept_scaling), _ptr(raw), _ptr(it)))
         return raw, it
+
+    def set_train_order(self, rows=None):
+        """rows: one array of original row indices per split, the split's training rows in the order a fit sees them
+        (include/b200gs.h gs_set_train_order); None: ascending"""
+        if rows is None:
+            self._check(self._L.gs_set_train_order(self._h, None, None, 0))
+            return
+        flat = np.ascontiguousarray(np.concatenate([np.asarray(r, np.int64) for r in rows]) if len(rows) else np.zeros(0), np.int32)
+        off = np.ascontiguousarray(np.concatenate([[0], np.cumsum([len(r) for r in rows])]), np.int64)
+        self._check(self._L.gs_set_train_order(self._h, _ptr(flat), _ptr(off), len(rows)))
+
+    def linsvr(self, C, epsilon, solver, seed, tol=1e-4, max_iter=1000, fit_intercept=True, intercept_scaling=1.0,
+               return_train=True, return_coef=False, return_stats=False):
+        """LinearSVR per (candidate, split): solver and seed [n_cand][n_splits] (liblinear's 11 / 12 / 13 and the fit's
+        std::mt19937 seed); n_iter = LinearSVR.n_iter_ of each fit.  return_coef: coef [n_cand][n_splits][d + 1] raw weights;
+        return_stats: cd_stats [n_cand][n_splits][3] (coordinate steps, shuffle cycles, fit cycles)"""
+        C = np.ascontiguousarray(C, np.float64)
+        n_cand = len(C)
+        shape = (n_cand, self.n_splits)
+        epsilon = np.ascontiguousarray(np.broadcast_to(np.asarray(epsilon, np.float64), (n_cand,)))
+        solver = np.ascontiguousarray(np.broadcast_to(np.asarray(solver, np.int64), shape), np.int32)
+        seed = np.ascontiguousarray(np.broadcast_to(np.asarray(seed, np.int64), shape), np.uint32)
+        out = dict(test=np.zeros(shape), train=np.zeros(shape), n_iter=np.zeros(shape, np.int32),
+                   fit_ms=np.zeros(shape, np.float32), score_ms=np.zeros(shape, np.float32))
+        coef = np.zeros(shape + (self.d + 1,)) if return_coef else None
+        stats = np.zeros(shape + (3,), np.int64) if return_stats else None
+        self._check(self._L.gs_linsvr(self._h, n_cand, _ptr(C), _ptr(epsilon), _ptr(solver), _ptr(seed), float(tol), int(max_iter),
+                                      int(bool(fit_intercept)), float(intercept_scaling), GS_RETURN_TRAIN if return_train else 0,
+                                      _ptr(out["test"]), _ptr(out["train"]), _ptr(out["n_iter"]), _ptr(out["fit_ms"]),
+                                      _ptr(out["score_ms"]), _ptr(coef), _ptr(stats)))
+        if not return_train:
+            out["train"] = None
+        if return_coef:
+            out["coef"] = coef
+        if return_stats:
+            out["cd_stats"] = stats
+        return out
+
+    def linsvr_refit(self, C, epsilon, solver, seed, tol=1e-4, max_iter=1000, fit_intercept=True, intercept_scaling=1.0):
+        """-> (raw [d + 1]: liblinear's weights, the bias feature's last; n_iter)"""
+        raw = np.zeros(self.d + 1)
+        it = np.zeros(1, np.int32)
+        self._check(self._L.gs_linsvr_refit(self._h, float(C), float(epsilon), int(solver), int(seed), float(tol), int(max_iter),
+                                            int(bool(fit_intercept)), float(intercept_scaling), _ptr(raw), _ptr(it)))
+        return raw, int(it[0])
+
+    def debug_mt19937(self, seed, k):
+        """the first k outputs of the device std::mt19937(seed) that the LinearSVR shuffles draw from"""
+        out = np.zeros(int(k), np.uint32)
+        self._check(self._L.gs_debug_mt19937(self._h, int(seed), int(k), _ptr(out)))
+        return out
 
     def knn(self, n_neighbors, weights, metric, return_train=True, y_f32=False):
         """k-NN scores per (candidate, split) from one neighbour selection per metric (include/b200gs.h gs_knn); weights and

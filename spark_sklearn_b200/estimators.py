@@ -4,9 +4,11 @@ and turn refit buffers back into genuine fitted scikit-learn estimators for ``be
 
 Only estimators with a CUDA path are accepted (SVC with the linear, rbf, poly and sigmoid kernels, SVR rbf/linear, Ridge,
 Lasso / ElasticNet, LogisticRegression, LinearSVC with the primal squared-hinge solver -- the families the reference ships
-examples for -- and KNeighborsClassifier / KNeighborsRegressor); anything else raises: no CPU fallback.
+examples for -- LinearSVR, and KNeighborsClassifier / KNeighborsRegressor); anything else raises: no CPU fallback.
 """
+import copy
 import numbers
+import threading
 import warnings
 
 import numpy as np
@@ -72,6 +74,9 @@ class Folds:
     def __init__(self, splits, n):
         self.n_splits = len(splits)
         self.n = n
+        # every split's training indices as the splitter yields them: a fit whose result depends on the order of X[train]
+        # (LinearSVR's coordinate descent) sees its rows in this order
+        self.train_order = [np.asarray(tr, np.int64) for tr, _ in splits]
         try:
             self.fold_id = fold_ids_from_splits(splits, n)
             self.masks = None
@@ -96,7 +101,7 @@ def adapter_for(estimator):
     from sklearn.linear_model import ElasticNet, Lasso, LogisticRegression, Ridge
     from sklearn.neighbors import KNeighborsClassifier, KNeighborsRegressor
     from sklearn.pipeline import Pipeline
-    from sklearn.svm import SVC, SVR, LinearSVC, NuSVC, NuSVR
+    from sklearn.svm import SVC, SVR, LinearSVC, LinearSVR, NuSVC, NuSVR
     t = type(estimator)
     if t is SVC:
         return SVCAdapter
@@ -114,6 +119,8 @@ def adapter_for(estimator):
         return ENetAdapter
     if t is LinearSVC:
         return LinearSVCAdapter
+    if t is LinearSVR:
+        return LinearSVRAdapter
     if t in (KNeighborsClassifier, KNeighborsRegressor):
         return KNeighborsAdapter if t is KNeighborsClassifier else KNeighborsRegressorAdapter
     if t is Pipeline and len(estimator.steps) == 1:
@@ -122,7 +129,7 @@ def adapter_for(estimator):
         return PipelineAdapter(estimator.steps[0][0], adapter_for(estimator.steps[0][1]))
     raise NotImplementedError(
         "spark_sklearn_b200 has CUDA paths for SVC, SVR, NuSVC, NuSVR, Ridge, Lasso, ElasticNet, LogisticRegression, LinearSVC, "
-        "KNeighborsClassifier and KNeighborsRegressor (bare or as the only step of a Pipeline); got %s (no CPU fallback)"
+        "LinearSVR, KNeighborsClassifier and KNeighborsRegressor (bare or as the only step of a Pipeline); got %s (no CPU fallback)"
         % t.__name__)
 
 
@@ -1048,6 +1055,164 @@ def materialize_linsvc(est, classes, raw, n_iter, n_features):
         est.coef_ = raw[:, :n_features].copy()
         est.intercept_ = 0.0
     est.n_iter_ = int(np.max(n_iter))
+    est.n_features_in_ = int(n_features)
+    if est.n_iter_ >= est.max_iter:
+        from sklearn.exceptions import ConvergenceWarning
+        warnings.warn("Liblinear failed to converge, increase the number of iterations.", ConvergenceWarning)
+    return est
+
+
+# ------------------------------------------------------------------ LinearSVR -----------------
+class LinearSVRAdapter:
+    multi_device = True        # plan(..., device=d): one plan per GPU of the in-process scheduler
+    scorers = REGRESSION_SCORERS
+
+    @staticmethod
+    def plan(estimator, cands, X, y, fold_id, n_splits, device=None):
+        return LinearSVRPlan(estimator, cands, X, y, fold_id, n_splits, device)
+
+
+_INT_MAX = int(np.iinfo("i").max)
+_SEED_LOCK = threading.Lock()
+
+
+def liblinear_seed(random_state):
+    """The seed _fit_liblinear hands to liblinear: check_random_state(random_state).randint(np.iinfo('i').max).  An int or a
+    RandomState gives the same seed to every fit (clone deep-copies the parameter, so the caller's RandomState is not
+    advanced); None draws from numpy's global RandomState."""
+    from sklearn.utils import check_random_state
+    if random_state is not None and not isinstance(random_state, (numbers.Integral, np.random.RandomState)):
+        raise ValueError("%r cannot be used to seed a numpy.random.RandomState instance" % (random_state,))
+    rs = copy.deepcopy(random_state) if isinstance(random_state, np.random.RandomState) else random_state
+    return int(check_random_state(rs).randint(_INT_MAX))
+
+
+class LinearSVRPlan(_Plan):
+    """sklearn.svm.LinearSVR with liblinear's solvers (csrc/linsvr.cu): the dual coordinate descent for
+    loss='epsilon_insensitive' (13) and for the squared loss when dual resolves to True (12), TRON otherwise (11).  dual='auto'
+    is resolved per training set, as LinearSVR.fit does, so one search can mix 11 and 12.  X reaches the device in float32 or
+    float64 and is widened exactly; y is float64.  The CD shuffles the positions of X[train], so every split's training rows
+    reach the device in the splitter's order."""
+    scorers = REGRESSION_SCORERS
+    supports_sample_weight = True
+    max_features = 512         # the CD keeps w in registers (include/b200gs.h GS_LINSVR_MAX_FEATURES)
+
+    def __init__(self, estimator, cands, X, y, fold_id, n_splits, device=None):
+        super().__init__(estimator, cands, X, y, fold_id, n_splits, device)
+        if y is None:
+            raise ValueError("LinearSVR needs y")
+        y = np.asarray(y)
+        if y.ndim == 2 and y.shape[1] == 1:               # scikit-learn: column_or_1d(y, warn=True)
+            from sklearn.exceptions import DataConversionWarning
+            warnings.warn("A column-vector y was passed when a 1d array was expected. Please change the shape of y to "
+                          "(n_samples, ), for example using ravel().", DataConversionWarning, stacklevel=2)
+            y = y[:, 0]
+        if y.ndim != 1:
+            raise ValueError("LinearSVR needs a 1d target; got y of shape %r" % (y.shape,))
+        if self.X.shape[1] > self.max_features:
+            raise NotImplementedError("LinearSVR on %d features: the CUDA path handles up to %d"
+                                      % (self.X.shape[1], self.max_features))
+        self.y = y.astype(np.float64)
+        self._set_data(self.X, y_target=self.y.astype(np.float32))
+        self.engine.set_targets_f64(self.y)
+        if self.folds is not None:
+            self.engine.set_train_order(self.folds.train_order)
+        self._seeds = None
+
+    def _check(self, p, n_rows):
+        """scikit-learn's own checks in LinearSVR.fit's order (parameter constraints, dual resolution on a training set of
+        n_rows rows, the liblinear solver of (loss, dual), _fit_liblinear's intercept_scaling test: ValueError), then the
+        values without a CUDA path.  Returns the liblinear solver (11, 12 or 13)."""
+        from sklearn.svm import LinearSVR
+        from sklearn.svm._base import _get_liblinear_solver_type
+        from sklearn.svm._classes import _validate_dual_parameter
+        LinearSVR(**p)._validate_params()
+        dual = _validate_dual_parameter(p["dual"], p["loss"], "l2", "ovr", np.empty((n_rows, self.X.shape[1]), np.bool_))
+        solver = _get_liblinear_solver_type("ovr", "l2", p["loss"], dual)
+        if p["fit_intercept"] and p["intercept_scaling"] <= 0:
+            raise ValueError("Intercept scaling is %r but needs to be greater than 0. To disable fitting an intercept, set "
+                             "fit_intercept=False." % p["intercept_scaling"])
+        if p["epsilon"] < 0:
+            raise NotImplementedError("LinearSVR epsilon=%r has no CUDA path (epsilon >= 0 does)" % (p["epsilon"],))
+        return int(solver)
+
+    def _seed_table(self):
+        """[n_cand][n_splits] liblinear seeds of every fit of the search, drawn as scikit-learn's GridSearchCV draws them:
+        candidate-major, split-minor, random_state=None from numpy's global RandomState.  A search whose candidates draw
+        from the global RandomState computes the table once for all of its per-GPU plans (they share the Folds)."""
+        if self._seeds is not None:
+            return self._seeds
+        states = [self._base_params(c)["random_state"] for c in self.cands]
+        if any(rs is None for rs in states) and self.folds is not None:
+            with _SEED_LOCK:
+                table = getattr(self.folds, "_liblinear_seeds", None)
+                if table is None:
+                    table = self.folds._liblinear_seeds = self._draw_seeds(states)
+        else:
+            table = self._draw_seeds(states)
+        self._seeds = table
+        return table
+
+    def _draw_seeds(self, states):
+        table = np.zeros((len(states), self.n_splits), np.int64)
+        for c, rs in enumerate(states):
+            if rs is None:
+                for k in range(self.n_splits):
+                    table[c, k] = liblinear_seed(None)
+            else:
+                table[c, :] = liblinear_seed(rs)
+        return table
+
+    def evaluate(self, my, return_train=True, error_score='raise'):
+        ns = self.n_splits
+        shape = (len(my), ns)
+        res = dict(test=np.zeros(shape), train=np.zeros(shape), fit_ms=np.zeros(shape), score_ms=np.zeros(shape),
+                   n_iter=np.zeros(shape, np.int64))
+        rows = [int(np.count_nonzero(self._train_rows(k))) for k in range(ns)]
+        params = [self._base_params(self.cands[ci]) for ci in my]
+        solvers = [[self._check(p, rows[k]) for k in range(ns)] for p in params]
+        seeds = self._seed_table()
+        groups = {}
+        for j, (ci, p) in enumerate(zip(my, params)):
+            key = (float(p["tol"]), int(p["max_iter"]), bool(p["fit_intercept"]), float(p["intercept_scaling"]))
+            groups.setdefault(key, []).append(j)
+        prof = {}
+        self.cd_stats_ = np.zeros(shape + (3,), np.int64)
+        for (tol, mi, fi, isc), idx in groups.items():
+            self.engine.set_scoring(self.score_kind, self.score_pos)
+            r = self.engine.linsvr([float(params[j]["C"]) for j in idx], [float(params[j]["epsilon"]) for j in idx],
+                                   [solvers[j] for j in idx], seeds[[my[j] for j in idx]], tol=tol, max_iter=mi,
+                                   fit_intercept=fi, intercept_scaling=isc, return_train=return_train, return_stats=True)
+            for key in ("test", "fit_ms", "score_ms", "n_iter"):
+                res[key][idx] = r[key]
+            if return_train:
+                res["train"][idx] = r["train"]
+            self.cd_stats_[idx] = r["cd_stats"]
+            for k, v in self.engine.profile().items():
+                prof[k] = prof.get(k, 0) + v
+        self._prof = prof
+        self.n_iter_ = res["n_iter"]
+        return self._finish(res, return_train, error_score, len(my))
+
+    def refit(self, best_params):
+        p = self._base_params(best_params)
+        solver = self._check(p, len(self.X))
+        seed = liblinear_seed(p["random_state"])            # the refit's own draw, after every search fit's
+        raw, n_iter = self.engine.linsvr_refit(p["C"], p["epsilon"], solver, seed, p["tol"], p["max_iter"], p["fit_intercept"],
+                                               p["intercept_scaling"])
+        est = clone(self.estimator).set_params(**best_params)
+        return materialize_linsvr(est, raw, n_iter, self.X.shape[1])
+
+
+def materialize_linsvr(est, raw, n_iter, n_features):
+    """Fill a (cloned, parametrised) sklearn.svm.LinearSVR with the fitted state of liblinear's raw weights raw [n_features + 1]
+    (the bias feature's weight last) and the fit's iteration count (svm/_base.py _fit_liblinear, svm/_classes.py
+    LinearSVR.fit: coef_ raveled, intercept_ = intercept_scaling x the bias weight as a 1-element array, or 0.0; n_iter_ an
+    int), with scikit-learn's ConvergenceWarning."""
+    raw = np.asarray(raw, np.float64)
+    est.coef_ = raw[:n_features].copy()
+    est.intercept_ = est.intercept_scaling * raw[n_features:n_features + 1] if est.fit_intercept else 0.0
+    est.n_iter_ = int(n_iter)
     est.n_features_in_ = int(n_features)
     if est.n_iter_ >= est.max_iter:
         from sklearn.exceptions import ConvergenceWarning

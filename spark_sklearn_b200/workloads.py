@@ -124,6 +124,24 @@ def _linsvc(which="small"):
     return w
 
 
+def _linsvr(which="small"):
+    """LinearSVR on the SVR recipe: a C x epsilon x loss grid at 4000 x 32 (small: the dual CD for the default loss, TRON for
+    the squared loss, whose dual='auto' resolves to the primal with more rows than features), fewer training rows than
+    features (wide: 'auto' picks the dual CD for the squared loss too), and a 1000-fit search (c: 200 candidates x 5 folds
+    of the default loss at 5000 x 64, tools/bench_linsvr.py)."""
+    if which == "wide":
+        w = _svr(n=300, d=400, name="linsvr_wide",
+                 grid={"C": [0.1, 1.0], "epsilon": [0.0, 0.1], "loss": ["epsilon_insensitive", "squared_epsilon_insensitive"]})
+    elif which == "c":
+        w = _svr(n=5000, d=64, name="linsvr_c", grid={"C": np.logspace(-3, 2, 50), "epsilon": [0.0, 0.05, 0.1, 0.2]})
+    else:
+        w = _svr(n=4000, d=32, name="linsvr_small",
+                 grid={"C": [0.01, 0.1, 1.0, 10.0], "epsilon": [0.0, 0.1],
+                       "loss": ["epsilon_insensitive", "squared_epsilon_insensitive"]})
+    w.update(estimator="LinearSVR", est_params={"random_state": 0})
+    return w
+
+
 def _knn(which="small"):
     """k-nearest neighbours: config 3's recipe at 2000 x 32 (small, binary), a 4-class set (multi), the SVR recipe (reg_small),
     config 2's data with a 200-fit grid (c2) and config 3's 50000 x 256 data with a smaller grid (c3: the row-slab case)."""
@@ -192,6 +210,10 @@ WORKLOADS = {
     "linsvc_small": _linsvc,
     "linsvc_multi": lambda: _linsvc("multi"),
     "linsvc_c3": lambda: _linsvc("c3"),
+    # LinearSVR (csrc/linsvr.cu): the golden-sized grid, a dual-resolving wide set, and the 1000-fit search (tools/bench_linsvr.py)
+    "linsvr_small": _linsvr,
+    "linsvr_wide": lambda: _linsvr("wide"),
+    "linsvr_c": lambda: _linsvr("c"),
     # k-nearest neighbours (csrc/knn.cu): one neighbour selection per (split, metric) serves every candidate
     "knn_small": _knn,
     "knn_multi": lambda: _knn("multi"),
@@ -225,6 +247,9 @@ def make_estimator(w):
     if w["estimator"] == "LinearSVC":
         from sklearn.svm import LinearSVC
         return LinearSVC(**w["est_params"])
+    if w["estimator"] == "LinearSVR":
+        from sklearn.svm import LinearSVR
+        return LinearSVR(**w["est_params"])
     if w["estimator"] in ("KNeighborsClassifier", "KNeighborsRegressor"):
         import sklearn.neighbors as nb
         return getattr(nb, w["estimator"])(**w["est_params"])

@@ -1,0 +1,87 @@
+"""Measure the LinearSVR search on one GPU: fits/s from CUDA events with X resident, the solve / score split, the epoch range
+and the coordinate steps of the dual CD (ns per step over the whole solve, SM cycles per step inside one fit, the share of a
+fit's cycles spent in the per-epoch shuffles), and scikit-learn's GridSearchCV(n_jobs=cores) on a sample of the candidates
+(with a parity check on that sample).  The card's name and power limit are read in the same run.
+
+    python tools/bench_linsvr.py [--workload linsvr_c] [--steps 2] [--sk-cands 4]
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+import warnings
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+
+def card():
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()
+        return q[0] if q else None
+    except (OSError, subprocess.SubprocessError):
+        return None
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--workload", default="linsvr_c")
+    ap.add_argument("--steps", type=int, default=2)
+    ap.add_argument("--sk-cands", type=int, default=4, help="candidates scikit-learn fits for comparison (0: skip)")
+    a = ap.parse_args()
+
+    from sklearn.exceptions import ConvergenceWarning
+    from sklearn.model_selection import GridSearchCV as SkGridSearchCV, KFold
+    from sklearn.svm import LinearSVR
+    from spark_sklearn_b200.estimators import Folds, LinearSVRAdapter
+    from spark_sklearn_b200 import workloads as W
+
+    w = W.make_workload(a.workload)
+    X, y, cv = w["X"], w["y"], w["cv"]
+    cands = W.candidates(w)
+    splits = list(KFold(cv).split(X, y))
+    plan = LinearSVRAdapter.plan(LinearSVR(**w["est_params"]), cands, X, y, Folds(splits, len(X)), cv)   # X resident from here
+    plan.set_scoring(None)
+    n_fits = len(cands) * cv
+
+    plan.evaluate([0])                                            # warm-up: library load, buffers
+    runs = []
+    for _ in range(a.steps):
+        res = plan.evaluate(list(range(len(cands))))
+        runs.append((dict(plan.profile()), plan.cd_stats_.copy()))
+    prof, stats = min(runs, key=lambda r: r[0]["ms_total"])
+    ms = prof["ms_total"]
+    steps, shuf, cyc = stats[..., 0], stats[..., 1], stats[..., 2]
+    cd = steps > 0
+    out = dict(workload=a.workload, card=card(), n=int(X.shape[0]), d=int(X.shape[1]), candidates=len(cands), folds=cv,
+               fits=n_fits, gpu_ms=round(ms, 2), fits_per_s=round(n_fits / (ms * 1e-3), 2),
+               ms_solve=round(prof["ms_solve"], 2), ms_score=round(prof["ms_score"], 2),
+               n_iter_range=[int(plan.n_iter_.min()), int(plan.n_iter_.max())],
+               coordinate_steps=int(steps.sum()),
+               ns_per_coordinate_step_aggregate=round(prof["ms_solve"] * 1e6 / max(int(steps.sum()), 1), 4),
+               sm_cycles_per_step_in_fit_median=round(float(np.median(cyc[cd] / steps[cd])), 1) if cd.any() else None,
+               shuffle_share_of_fit_cycles=round(float(shuf[cd].sum() / cyc[cd].sum()), 4) if cd.any() else None,
+               launches=int(prof["launches"]), steps=a.steps, all_gpu_ms=[round(p["ms_total"], 2) for p, _ in runs])
+
+    if a.sk_cands > 0:
+        pick = list(np.linspace(0, len(cands) - 1, a.sk_cands).round().astype(int))
+        grid = [{k: [v] for k, v in cands[i].items()} for i in pick]
+        t0 = time.perf_counter()
+        with warnings.catch_warnings():
+            warnings.simplefilter("ignore", ConvergenceWarning)
+            sk = SkGridSearchCV(LinearSVR(**w["est_params"]), grid, cv=KFold(cv), n_jobs=os.cpu_count(), refit=False).fit(X, y)
+        sk_s = time.perf_counter() - t0
+        ref = np.stack([sk.cv_results_["split%d_test_score" % k] for k in range(cv)], 1)
+        got = res["test"][pick]
+        out.update(sklearn_fits=len(pick) * cv, sklearn_s=round(sk_s, 2), sklearn_fits_per_s=round(len(pick) * cv / sk_s, 3),
+                   sklearn_cores=os.cpu_count(), parity_max_abs_split_score_diff=float(np.abs(got - ref).max()))
+    print(json.dumps(out))
+
+
+if __name__ == "__main__":
+    main()
