@@ -376,6 +376,42 @@ int gs_set_train_order(gs_handle *h, const int32_t *rows, const int64_t *offsets
 /* Test hook: the first k outputs of the device std::mt19937(seed) that gs_linsvr's shuffles draw from. */
 int gs_debug_mt19937(gs_handle *h, uint32_t seed, int32_t k, uint32_t *out);
 
+/*
+ * SGDClassifier / SGDRegressor (csrc/sgd.cu).  Replaces: SGDClassifier.fit / SGDRegressor.fit and their score per
+ * (candidate, split) (reference base_search.py:83-87) with scikit-learn's _plain_sgd restated step for step, one warp per
+ * fit.  A classifier fits once per (candidate, split) with two classes (+1 = class 1, log_loss 1 / 0) and once per class
+ * with more (one-vs-rest: that class +1, negatives of class weight 1.0).  Per candidate: loss[c] (GS_SGD_HINGE ..
+ * GS_SGD_SQUARED_EPSILON_INSENSITIVE; a regression gs_set_data takes the last four), penalty[c] (GS_SGD_NONE / L1 / L2 /
+ * ELASTICNET), alpha[c] (> 0 with 'optimal'), l1_ratio[c] (elasticnet's mix), epsilon[c] (huber and the epsilon-insensitive
+ * losses), learning_rate[c] (1 constant, 2 optimal, 3 invscaling, 4 adaptive), eta0[c], power_t[c].  seed[t] with
+ * t = (c * n_splits + k) * KC + class, KC = n_classes for three or more classes and 1 otherwise: the fit's shuffle seed (the
+ * uint32 scikit-learn hands to _plain_sgd).  Scalars: tol (-inf for tol=None), max_iter, n_iter_no_change, fit_intercept,
+ * shuffle.  Rows: a split's training rows in gs_set_train_order's order (default ascending), none dropped; sample weights
+ * from gs_set_sample_weight, class weights from gs_set_class_weight (one set, or one per split).  X is float32 (the
+ * float32 path of _plain_sgd32) or float64; regression targets from gs_set_targets_f64 (rounded to float32 with float32
+ * X).  d <= GS_SGD_MAX_FEATURES.  Scores: every classification scorer (roc_auc binary) or r2 / neg MSE / neg RMSE, from the
+ * float64 decision values [X | 1] . [coef | intercept] of one FP64 tensor-core contraction.  Per (candidate, split):
+ * n_iter = the maximum over the classes (SGDClassifier.n_iter_), fit_status 0 stopped by the n_iter_no_change rule, 1 ran
+ * max_iter epochs, 2 a weight or the intercept became non-finite (scores NaN; n_iter is that epoch, of the first such
+ * class).  Test hooks: coef_out (may be NULL) [t][d + 1] every fit's coef then intercept; stats (may be NULL) [t][3] =
+ * samples processed, clock cycles drawing and applying the shuffles, clock cycles of the whole fit.
+ * gs_sgd_refit: one fit per class on every row in row order; seed [KC]; coef_out [KC][d + 1], n_iter [KC], fit_status [KC].
+ */
+#define GS_SGD_MAX_FEATURES 512
+enum { GS_SGD_HINGE = 0, GS_SGD_PERCEPTRON = 1, GS_SGD_SQUARED_HINGE = 2, GS_SGD_MODIFIED_HUBER = 3, GS_SGD_LOG_LOSS = 4,
+       GS_SGD_SQUARED_ERROR = 5, GS_SGD_HUBER = 6, GS_SGD_EPSILON_INSENSITIVE = 7, GS_SGD_SQUARED_EPSILON_INSENSITIVE = 8 };
+enum { GS_SGD_NONE = 0, GS_SGD_L1 = 1, GS_SGD_L2 = 2, GS_SGD_ELASTICNET = 3 };
+int gs_sgd(gs_handle *h, int32_t n_cand, const int32_t *loss, const int32_t *penalty, const double *alpha, const double *l1_ratio,
+           const double *epsilon, const int32_t *learning_rate, const double *eta0, const double *power_t, const uint32_t *seed,
+           double tol, int32_t max_iter, int32_t n_iter_no_change, int32_t fit_intercept, int32_t shuffle, uint32_t flags,
+           double *test_scores, double *train_scores, int32_t *n_iter, int32_t *fit_status, float *fit_ms, float *score_ms,
+           double *coef_out, int64_t *stats);
+int gs_sgd_refit(gs_handle *h, int32_t loss, int32_t penalty, double alpha, double l1_ratio, double epsilon, int32_t learning_rate,
+                 double eta0, double power_t, const uint32_t *seed, double tol, int32_t max_iter, int32_t n_iter_no_change,
+                 int32_t fit_intercept, int32_t shuffle, double *coef_out, int32_t *n_iter, int32_t *fit_status);
+/* Test hook: pi, the permutation of l positions the SGD shuffle with this seed applies every epoch. */
+int gs_debug_sgd_perm(gs_handle *h, uint32_t seed, int32_t l, int32_t *out);
+
 /* C[M][N] = sum_k A[M][k]*B[N][k] on the FP64 tensor-core path of gs_linsvc (K > 1024: split-K with the fixed-order sum of
  * the partials), host float64 row-major in/out. */
 int gs_debug_gemm_f64(gs_handle *h, const double *A, int32_t M, const double *B, int32_t N, int32_t K, double *C);

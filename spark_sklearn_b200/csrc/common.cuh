@@ -358,6 +358,11 @@ cudaError_t launch_tron_advance(TrState *St, double *Vec, double *V, const doubl
 // Xa = [X | bias | 0 ...] in float64 ([npad][nvp], rows >= n zero) and its transpose [nvp][npad]
 cudaError_t launch_build_xa64(const float *X32, const double *X64, int n, int d, double bias, int nvp, int64_t npad, double *Xa,
                               double *Xat, cudaStream_t st);
+// Per-class counts of the predictions of nfit fits from their KC decision rows Zt[(f KC + k) ldz + row] (KC == 1: z > 0 ->
+// class 1; else the first arg-max) on split fold_of_fit[f]: counts[f][split (0 test, 1 train)][class][3 = support, tp,
+// predicted], pre-zeroed
+cudaError_t launch_linsvc_count(const double *Zt, int64_t ldz, int n, int K, int KC, const int *y, SplitMasks sm,
+                                const int *fold_of_fit, int nfit, int *counts, cudaStream_t st);
 
 // ---- gemm_tc.cu: wgmma + TMA contraction  C[M][N] = sum_k A[M][k] B[N][k]  (3xTF32 split, fp32 accumulate) ----
 struct alignas(64) TcMap { unsigned char bytes[128]; };            // CUtensorMap

@@ -492,7 +492,7 @@ int linsvc_run(gs_handle *h, int n_cand, const double *Cv, double tol, int max_i
 
 }  // namespace
 
-// ---- the TRON pieces linsvr.cu shares (LinearSVR's primal solver, L2R_L2LOSS_SVR) ----
+// ---- the pieces linsvr.cu (LinearSVR's primal solver, L2R_L2LOSS_SVR) and sgd.cu (the classification scorers) share ----
 cudaError_t launch_tron_advance(TrState *St, double *Vec, double *V, const double *Gp, int nchunk, int64_t gp_stride,
                                 const double *fpart, int ncol, int nvp, int max_iter, int *n_open, cudaStream_t st)
 {
@@ -505,6 +505,13 @@ cudaError_t launch_build_xa64(const float *X32, const double *X64, int n, int d,
 {
     dim3 grid((unsigned)((npad + 31) / 32), (nvp + 31) / 32), block(32, 32);
     build_xa64_kernel<<<grid, block, 0, st>>>(X32, X64, n, d, bias, nvp, npad, Xa, Xat);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_linsvc_count(const double *Zt, int64_t ldz, int n, int K, int KC, const int *y, SplitMasks sm,
+                                const int *fold_of_fit, int nfit, int *counts, cudaStream_t st)
+{
+    linsvc_count_kernel<<<dim3(64, nfit), 256, (size_t)6 * K * 4, st>>>(Zt, ldz, n, K, KC, y, sm, fold_of_fit, counts);
     return cudaGetLastError();
 }
 

@@ -96,6 +96,9 @@ def load_library():
     L.gs_linsvr.argtypes = [vp, i32, vp, vp, vp, vp, dbl, i32, i32, dbl, u32, vp, vp, vp, vp, vp, vp, vp]
     L.gs_linsvr_refit.argtypes = [vp, dbl, dbl, i32, u32, dbl, i32, i32, dbl, vp, vp]
     L.gs_set_train_order.argtypes = [vp, vp, vp, i32]
+    L.gs_sgd.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, dbl, i32, i32, i32, i32, u32, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.gs_sgd_refit.argtypes = [vp, i32, i32, dbl, dbl, dbl, i32, dbl, dbl, vp, dbl, i32, i32, i32, i32, vp, vp, vp]
+    L.gs_debug_sgd_perm.argtypes = [vp, u32, i32, vp]
     L.gs_debug_mt19937.argtypes = [vp, u32, i32, vp]
     L.gs_knn.argtypes = [vp, i32, vp, vp, vp, u32, vp, vp, vp, vp]
     L.gs_debug_knn_neighbors.argtypes = [vp, i32, i32, i32, vp, vp]
@@ -116,7 +119,7 @@ def load_library():
               "gs_svr", "gs_svr_refit", "gs_nusvc", "gs_nusvc_refit", "gs_nusvr", "gs_nusvr_refit", "gs_logreg",
               "gs_logreg_refit", "gs_linsvc", "gs_linsvc_refit", "gs_get_profile", "gs_debug_gram", "gs_debug_kernel_matrix",
               "gs_debug_decision", "gs_debug_score", "gs_debug_linear", "gs_debug_gemm_nt", "gs_debug_gemm_f64", "gs_knn", "gs_debug_knn_neighbors",
-              "gs_linsvr", "gs_linsvr_refit", "gs_set_train_order", "gs_debug_mt19937"):
+              "gs_linsvr", "gs_linsvr_refit", "gs_set_train_order", "gs_debug_mt19937", "gs_sgd", "gs_sgd_refit", "gs_debug_sgd_perm"):
         getattr(L, f).restype = c.c_int
     _lib = L
     return L
@@ -418,6 +421,70 @@ class Engine:
         """the first k outputs of the device std::mt19937(seed) that the LinearSVR shuffles draw from"""
         out = np.zeros(int(k), np.uint32)
         self._check(self._L.gs_debug_mt19937(self._h, int(seed), int(k), _ptr(out)))
+        return out
+
+    SGD_LOSS = {"hinge": 0, "perceptron": 1, "squared_hinge": 2, "modified_huber": 3, "log_loss": 4, "squared_error": 5,
+                "huber": 6, "epsilon_insensitive": 7, "squared_epsilon_insensitive": 8}
+    SGD_PENALTY = {None: 0, "l1": 1, "l2": 2, "elasticnet": 3}
+    SGD_RATE = {"constant": 1, "optimal": 2, "invscaling": 3, "adaptive": 4}
+
+    def _sgd_cands(self, loss, penalty, alpha, l1_ratio, epsilon, learning_rate, eta0, power_t):
+        n = len(loss)
+        code = lambda table, v: [table[x] if isinstance(x, str) or x is None else int(x) for x in v]
+        i32 = lambda v: np.ascontiguousarray(v, np.int32)
+        f64 = lambda v: np.ascontiguousarray(np.broadcast_to(np.asarray(v, np.float64), (n,)))
+        return (i32(code(self.SGD_LOSS, loss)), i32(code(self.SGD_PENALTY, penalty)), f64(alpha), f64(l1_ratio), f64(epsilon),
+                i32(code(self.SGD_RATE, learning_rate)), f64(eta0), f64(power_t))
+
+    def sgd(self, loss, penalty, alpha, l1_ratio, epsilon, learning_rate, eta0, power_t, seed, tol=1e-3, max_iter=1000,
+            n_iter_no_change=5, fit_intercept=True, shuffle=True, return_train=True, return_coef=False, return_stats=False):
+        """SGDClassifier / SGDRegressor per (candidate, split) (include/b200gs.h gs_sgd): per-candidate loss / penalty /
+        learning_rate names or codes and numbers; seed [n_cand][n_splits][KC] shuffle seeds (KC = n_classes for three or
+        more classes, else 1); tol None = no stop rule.  -> test / train scores, n_iter, status (0 stopped, 1 max_iter,
+        2 non-finite), fit_ms, score_ms; return_coef: coef [n_cand][n_splits][KC][d + 1] (coef, then intercept);
+        return_stats: stats [n_cand][n_splits][KC][3] (samples, shuffle cycles, fit cycles)"""
+        cands = self._sgd_cands(loss, penalty, alpha, l1_ratio, epsilon, learning_rate, eta0, power_t)
+        n_cand = len(cands[0])
+        shape = (n_cand, self.n_splits)
+        kc = self.n_classes if self.n_classes > 2 else 1
+        seed = np.ascontiguousarray(np.broadcast_to(np.asarray(seed, np.int64).reshape(n_cand, self.n_splits, -1),
+                                                    shape + (kc,)), np.uint32)
+        out = dict(test=np.zeros(shape), train=np.zeros(shape), n_iter=np.zeros(shape, np.int32), status=np.zeros(shape, np.int32),
+                   fit_ms=np.zeros(shape, np.float32), score_ms=np.zeros(shape, np.float32))
+        coef = np.zeros(shape + (kc, self.d + 1)) if return_coef else None
+        stats = np.zeros(shape + (kc, 3), np.int64) if return_stats else None
+        self._check(self._L.gs_sgd(self._h, n_cand, *[_ptr(a) for a in cands], _ptr(seed), -np.inf if tol is None else float(tol),
+                                   int(max_iter), int(n_iter_no_change), int(bool(fit_intercept)), int(bool(shuffle)),
+                                   GS_RETURN_TRAIN if return_train else 0, _ptr(out["test"]), _ptr(out["train"]),
+                                   _ptr(out["n_iter"]), _ptr(out["status"]), _ptr(out["fit_ms"]), _ptr(out["score_ms"]),
+                                   _ptr(coef), _ptr(stats)))
+        if not return_train:
+            out["train"] = None
+        if return_coef:
+            out["coef"] = coef
+        if return_stats:
+            out["stats"] = stats
+        return out
+
+    def sgd_refit(self, loss, penalty, alpha, l1_ratio, epsilon, learning_rate, eta0, power_t, seed, tol=1e-3, max_iter=1000,
+                  n_iter_no_change=5, fit_intercept=True, shuffle=True):
+        """one fit per class (KC of them) on every row: seed [KC] -> (coef [KC][d + 1], n_iter [KC], status [KC])"""
+        c = self._sgd_cands([loss], [penalty], alpha, l1_ratio, epsilon, [learning_rate], eta0, power_t)
+        kc = self.n_classes if self.n_classes > 2 else 1
+        seed = np.ascontiguousarray(np.broadcast_to(np.asarray(seed, np.int64), (kc,)), np.uint32)
+        coef = np.zeros((kc, self.d + 1))
+        it = np.zeros(kc, np.int32)
+        st = np.zeros(kc, np.int32)
+        self._check(self._L.gs_sgd_refit(self._h, int(c[0][0]), int(c[1][0]), float(c[2][0]), float(c[3][0]), float(c[4][0]),
+                                         int(c[5][0]), float(c[6][0]), float(c[7][0]), _ptr(seed),
+                                         -np.inf if tol is None else float(tol), int(max_iter), int(n_iter_no_change),
+                                         int(bool(fit_intercept)), int(bool(shuffle)), _ptr(coef), _ptr(it), _ptr(st)))
+        return coef, it, st
+
+    def debug_sgd_perm(self, seed, l):
+        """pi: the permutation of l positions the device SGD shuffle with this seed applies every epoch"""
+        out = np.zeros(int(l), np.int32)
+        self._check(self._L.gs_debug_sgd_perm(self._h, int(seed), int(l), _ptr(out)))
         return out
 
     def knn(self, n_neighbors, weights, metric, return_train=True, y_f32=False):

@@ -4,7 +4,7 @@ and turn refit buffers back into genuine fitted scikit-learn estimators for ``be
 
 Only estimators with a CUDA path are accepted (SVC with the linear, rbf, poly and sigmoid kernels, SVR rbf/linear, Ridge,
 Lasso / ElasticNet, LogisticRegression, LinearSVC with the primal squared-hinge solver -- the families the reference ships
-examples for -- LinearSVR, and KNeighborsClassifier / KNeighborsRegressor); anything else raises: no CPU fallback.
+examples for -- LinearSVR, SGDClassifier / SGDRegressor, and KNeighborsClassifier / KNeighborsRegressor); anything else raises: no CPU fallback.
 """
 import copy
 import numbers
@@ -98,7 +98,7 @@ class Folds:
 
 
 def adapter_for(estimator):
-    from sklearn.linear_model import ElasticNet, Lasso, LogisticRegression, Ridge
+    from sklearn.linear_model import ElasticNet, Lasso, LogisticRegression, Ridge, SGDClassifier, SGDRegressor
     from sklearn.neighbors import KNeighborsClassifier, KNeighborsRegressor
     from sklearn.pipeline import Pipeline
     from sklearn.svm import SVC, SVR, LinearSVC, LinearSVR, NuSVC, NuSVR
@@ -121,6 +121,10 @@ def adapter_for(estimator):
         return LinearSVCAdapter
     if t is LinearSVR:
         return LinearSVRAdapter
+    if t is SGDClassifier:
+        return SGDClassifierAdapter
+    if t is SGDRegressor:
+        return SGDRegressorAdapter
     if t in (KNeighborsClassifier, KNeighborsRegressor):
         return KNeighborsAdapter if t is KNeighborsClassifier else KNeighborsRegressorAdapter
     if t is Pipeline and len(estimator.steps) == 1:
@@ -129,7 +133,7 @@ def adapter_for(estimator):
         return PipelineAdapter(estimator.steps[0][0], adapter_for(estimator.steps[0][1]))
     raise NotImplementedError(
         "spark_sklearn_b200 has CUDA paths for SVC, SVR, NuSVC, NuSVR, Ridge, Lasso, ElasticNet, LogisticRegression, LinearSVC, "
-        "LinearSVR, KNeighborsClassifier and KNeighborsRegressor (bare or as the only step of a Pipeline); got %s (no CPU fallback)"
+        "LinearSVR, SGDClassifier, SGDRegressor, KNeighborsClassifier and KNeighborsRegressor (bare or as the only step of a Pipeline); got %s (no CPU fallback)"
         % t.__name__)
 
 
@@ -1087,6 +1091,24 @@ def liblinear_seed(random_state):
     return int(check_random_state(rs).randint(_INT_MAX))
 
 
+def search_seed_table(plan, draw):
+    """The seeds of every fit of a search, drawn by draw(random_states) as scikit-learn's GridSearchCV draws them:
+    candidate-major, split-minor, random_state=None from numpy's global RandomState.  A search whose candidates draw from the
+    global RandomState computes the table once for all of its per-GPU plans (they share the Folds); the plan keeps it."""
+    if plan._seeds is not None:
+        return plan._seeds
+    states = [plan._base_params(c)["random_state"] for c in plan.cands]
+    if any(rs is None for rs in states) and plan.folds is not None:
+        with _SEED_LOCK:
+            table = getattr(plan.folds, "_search_seeds", None)
+            if table is None:
+                table = plan.folds._search_seeds = draw(states)
+    else:
+        table = draw(states)
+    plan._seeds = table
+    return table
+
+
 class LinearSVRPlan(_Plan):
     """sklearn.svm.LinearSVR with liblinear's solvers (csrc/linsvr.cu): the dual coordinate descent for
     loss='epsilon_insensitive' (13) and for the squared loss when dual resolves to True (12), TRON otherwise (11).  dual='auto'
@@ -1137,21 +1159,8 @@ class LinearSVRPlan(_Plan):
         return int(solver)
 
     def _seed_table(self):
-        """[n_cand][n_splits] liblinear seeds of every fit of the search, drawn as scikit-learn's GridSearchCV draws them:
-        candidate-major, split-minor, random_state=None from numpy's global RandomState.  A search whose candidates draw
-        from the global RandomState computes the table once for all of its per-GPU plans (they share the Folds)."""
-        if self._seeds is not None:
-            return self._seeds
-        states = [self._base_params(c)["random_state"] for c in self.cands]
-        if any(rs is None for rs in states) and self.folds is not None:
-            with _SEED_LOCK:
-                table = getattr(self.folds, "_liblinear_seeds", None)
-                if table is None:
-                    table = self.folds._liblinear_seeds = self._draw_seeds(states)
-        else:
-            table = self._draw_seeds(states)
-        self._seeds = table
-        return table
+        """[n_cand][n_splits] liblinear seeds of every fit of the search (search_seed_table)"""
+        return search_seed_table(self, self._draw_seeds)
 
     def _draw_seeds(self, states):
         table = np.zeros((len(states), self.n_splits), np.int64)
@@ -1217,6 +1226,225 @@ def materialize_linsvr(est, raw, n_iter, n_features):
     if est.n_iter_ >= est.max_iter:
         from sklearn.exceptions import ConvergenceWarning
         warnings.warn("Liblinear failed to converge, increase the number of iterations.", ConvergenceWarning)
+    return est
+
+
+# ------------------------------------------------------------------ SGDClassifier / SGDRegressor
+class SGDClassifierAdapter:
+    multi_device = True        # plan(..., device=d): one plan per GPU of the in-process scheduler
+    scorers = CLASSIFICATION_SCORERS
+
+    @staticmethod
+    def plan(estimator, cands, X, y, fold_id, n_splits, device=None):
+        return SGDPlan(estimator, cands, X, y, fold_id, n_splits, device)
+
+
+class SGDRegressorAdapter(SGDClassifierAdapter):
+    scorers = REGRESSION_SCORERS
+
+
+def sgd_seeds(random_state, n_classes):
+    """The shuffle seeds scikit-learn hands to _plain_sgd for one fit (n_classes 0: a regressor), drawing from
+    check_random_state(random_state) as fit does: binary fit_binary draws make_dataset's seed, then the shuffle seed;
+    one-vs-rest draws one seed per class and each class fit makes those two draws from RandomState(seed); _fit_regressor
+    draws the shuffle seed, then make_dataset's.  An int or a RandomState gives the same seeds to every fit (clone
+    deep-copies the parameter, so the caller's RandomState is not advanced); None draws from numpy's global RandomState."""
+    from sklearn.utils import check_random_state
+    if random_state is not None and not isinstance(random_state, (numbers.Integral, np.random.RandomState)):
+        raise ValueError("%r cannot be used to seed a numpy.random.RandomState instance" % (random_state,))
+    rs = check_random_state(copy.deepcopy(random_state) if isinstance(random_state, np.random.RandomState) else random_state)
+    if n_classes == 0:
+        seed = int(rs.randint(0, _INT_MAX))
+        rs.randint(1, _INT_MAX)
+        return [seed]
+    if n_classes == 2:
+        rs.randint(1, _INT_MAX)
+        return [int(rs.randint(_INT_MAX))]
+    out = []
+    for s in rs.randint(_INT_MAX, size=n_classes):
+        r = np.random.RandomState(s)
+        r.randint(1, _INT_MAX)
+        out.append(int(r.randint(_INT_MAX)))
+    return out
+
+
+class SGDPlan(_Plan):
+    """sklearn.linear_model.SGDClassifier / SGDRegressor (csrc/sgd.cu): _plain_sgd restated step for step, one warp per
+    (candidate, split, one-vs-rest class) fit.  X reaches the device in its own dtype (float32 runs _plain_sgd32, as
+    scikit-learn does), dense; the shuffle permutes the positions of X[train], so every split's training rows reach the
+    device in the splitter's order."""
+    supports_sample_weight = True
+    max_features = 512         # w and q live in registers (include/b200gs.h GS_SGD_MAX_FEATURES)
+
+    def __init__(self, estimator, cands, X, y, fold_id, n_splits, device=None):
+        import scipy.sparse as sp
+        from sklearn.linear_model import SGDClassifier
+        name = type(estimator).__name__
+        if sp.issparse(X):
+            raise NotImplementedError("%s on sparse X has no CUDA path (scikit-learn's sparse SGD decays the intercept and "
+                                      "touches only the stored entries): pass a dense X" % name)
+        super().__init__(estimator, cands, X, y, fold_id, n_splits, device)
+        if y is None:
+            raise ValueError("%s needs y" % name)
+        self.classifier = isinstance(estimator, SGDClassifier)
+        self.scorers = CLASSIFICATION_SCORERS if self.classifier else REGRESSION_SCORERS
+        if self.X.shape[1] > self.max_features:
+            raise NotImplementedError("%s on %d features: the CUDA path handles up to %d" % (name, self.X.shape[1], self.max_features))
+        y = np.asarray(y)
+        if self.classifier:
+            self.classes, self.y_class = np.unique(y, return_inverse=True)
+            if len(self.classes) < 2:
+                raise ValueError("The number of classes has to be greater than one; got %d class" % len(self.classes))
+            if len(self.classes) > 64:
+                raise NotImplementedError("%s CUDA path handles up to 64 classes (got %d)" % (name, len(self.classes)))
+            self._set_data(self.X, y_class=self.y_class.astype(np.int32))
+            self.kc = len(self.classes) if len(self.classes) > 2 else 1
+        else:
+            if y.ndim != 1:
+                raise NotImplementedError("multi-output %s is not supported by the CUDA path" % name)
+            self.y = y.astype(np.float64)
+            self._set_data(self.X, y_target=self.y.astype(np.float32))
+            self.engine.set_targets_f64(self.y)
+            self.kc = 1
+        if self.folds is not None:
+            self.engine.set_train_order(self.folds.train_order)
+        self._seeds = None
+
+    def _check(self, p):
+        """scikit-learn's own checks (ValueError), then the settings without a CUDA path"""
+        est = type(self.estimator)(**p)
+        est._validate_params()
+        est._more_validate_params()
+        name = type(self.estimator).__name__
+        if p["early_stopping"]:
+            raise NotImplementedError("%s early_stopping=True has no CUDA path" % name)
+        if p["average"] is not False and p["average"] != 0:
+            raise NotImplementedError("%s average=%r has no CUDA path" % (name, p["average"]))
+        if p["learning_rate"] in ("pa1", "pa2"):
+            raise NotImplementedError("%s learning_rate=%r has no CUDA path" % (name, p["learning_rate"]))
+        return est
+
+    def _class_weights(self, cw, k):
+        """SGD's class weights ignore sample weights: compute_class_weight(class_weight, classes, y_train)"""
+        from sklearn.utils.class_weight import compute_class_weight
+        return compute_class_weight(cw, classes=self.classes, y=np.asarray(self.y)[self._train_rows(k)])
+
+    def _draw_seeds(self, states):
+        nc = len(self.classes) if self.classifier else 0
+        table = np.zeros((len(states), self.n_splits, self.kc), np.int64)
+        for c, rs in enumerate(states):
+            if rs is None:
+                for k in range(self.n_splits):
+                    table[c, k] = sgd_seeds(None, nc)
+            else:
+                table[c, :] = sgd_seeds(rs, nc)
+        return table
+
+    @staticmethod
+    def _fit_args(p):
+        return dict(loss=p["loss"], penalty=p["penalty"], alpha=float(p["alpha"]),
+                    l1_ratio=float(0.0 if p["l1_ratio"] is None else p["l1_ratio"]), epsilon=float(p["epsilon"]),
+                    learning_rate=p["learning_rate"], eta0=float(p["eta0"]), power_t=float(p["power_t"]))
+
+    @staticmethod
+    def _overflow(epoch):
+        return ValueError("Floating-point under-/overflow occurred at epoch #%d. Scaling input data with StandardScaler or "
+                          "MinMaxScaler might help." % epoch)
+
+    def evaluate(self, my, return_train=True, error_score='raise'):
+        ns = self.n_splits
+        shape = (len(my), ns)
+        res = dict(test=np.zeros(shape), train=np.zeros(shape), fit_ms=np.zeros(shape), score_ms=np.zeros(shape),
+                   n_iter=np.zeros(shape, np.int64), status=np.zeros(shape, np.int64))
+        params = [self._base_params(self.cands[ci]) for ci in my]
+        for p in params:
+            self._check(p)
+        seeds = search_seed_table(self, self._draw_seeds)
+        groups = {}
+        for j, p in enumerate(params):
+            cw = p["class_weight"] if self.classifier else None
+            cwk = None if cw is None else (cw if isinstance(cw, str) else tuple(sorted(cw.items())))
+            key = (None if p["tol"] is None else float(p["tol"]), int(p["max_iter"]), int(p["n_iter_no_change"]),
+                   bool(p["fit_intercept"]), bool(p["shuffle"]), cwk)
+            groups.setdefault(key, []).append(j)
+        prof = {}
+        self.stats_ = np.zeros(shape + (self.kc, 3), np.int64)
+        for (tol, mi, nic, fi, sh, _cwk), idx in groups.items():
+            if self.classifier:
+                self._set_class_weight(params[idx[0]]["class_weight"])
+            self.engine.set_scoring(self.score_kind, self.score_pos)
+            args = [self._fit_args(params[j]) for j in idx]
+            r = self.engine.sgd(*[[a[k] for a in args] for k in ("loss", "penalty", "alpha", "l1_ratio", "epsilon", "learning_rate",
+                                                                 "eta0", "power_t")],
+                                seeds[[my[j] for j in idx]], tol=tol, max_iter=mi, n_iter_no_change=nic, fit_intercept=fi,
+                                shuffle=sh, return_train=return_train, return_stats=True)
+            for key in ("test", "fit_ms", "score_ms", "n_iter", "status"):
+                res[key][idx] = r[key]
+            if return_train:
+                res["train"][idx] = r["train"]
+            self.stats_[idx] = r["stats"]
+            for k, v in self.engine.profile().items():
+                prof[k] = prof.get(k, 0) + v
+        if self.classifier:
+            self.engine.set_class_weight(None)
+        self._prof = prof
+        self.n_iter_ = res["n_iter"]
+        bad = res["status"] == 2
+        if bad.any():
+            if error_score == 'raise':
+                j, k = map(int, np.argwhere(bad)[0])
+                raise self._overflow(int(res["n_iter"][j, k]))
+            warnings.warn("%d fits failed with a floating-point under-/overflow; their scores are error_score=%r"
+                          % (int(bad.sum()), error_score))
+            res["test"][bad] = error_score
+            if return_train:
+                res["train"][bad] = error_score
+        return self._finish(res, return_train, error_score, len(my))
+
+    def refit(self, best_params):
+        p = self._base_params(best_params)
+        self._check(p)
+        nc = len(self.classes) if self.classifier else 0
+        seeds = sgd_seeds(p["random_state"], nc)                # the refit's own draw, after every search fit's
+        cw_ = self._set_class_weight(p["class_weight"], refit=True) if self.classifier else None
+        try:
+            coef, n_iter, status = self.engine.sgd_refit(**self._fit_args(p), seed=seeds, tol=p["tol"], max_iter=p["max_iter"],
+                                                         n_iter_no_change=p["n_iter_no_change"], fit_intercept=p["fit_intercept"],
+                                                         shuffle=p["shuffle"])
+        finally:
+            if self.classifier:
+                self.engine.set_class_weight(None)
+        if (status == 2).any():
+            raise self._overflow(int(n_iter[int(np.argmax(status == 2))]))
+        est = clone(self.estimator).set_params(**best_params)
+        return materialize_sgd(est, self.X, coef, n_iter, self.classes if self.classifier else None, cw_)
+
+
+def materialize_sgd(est, X, coef, n_iter, classes, class_weight):
+    """Fill a (cloned, parametrised) SGDClassifier / SGDRegressor with the fitted state of its per-class fits coef
+    [KC][d + 1] (coef, then intercept) and n_iter [KC] (linear_model/_stochastic_gradient.py _fit_binary, _fit_multiclass,
+    _fit_regressor: coef_ in X's dtype; intercept_ float64 but for one-vs-rest; n_iter_ the maximum over the classes;
+    t_ = 1 + n_iter_ x n_samples; the classifier's _loss_function_), with scikit-learn's ConvergenceWarning."""
+    d = X.shape[1]
+    dt = np.float32 if X.dtype == np.float32 else np.float64
+    coef = np.asarray(coef, np.float64)
+    if classes is not None:
+        est.classes_ = np.asarray(classes)
+        est._expanded_class_weight = np.asarray(class_weight, np.float64)
+        est.coef_ = coef[:, :d].astype(dt)
+        est.intercept_ = coef[:, d].astype(dt if len(classes) > 2 else np.float64)
+    else:
+        est.coef_ = coef[0, :d].astype(dt)
+        est.intercept_ = coef[0, d:].astype(np.float64)
+    est.n_iter_ = int(np.max(n_iter))
+    est.t_ = 1.0 + est.n_iter_ * X.shape[0]
+    est.n_features_in_ = int(d)
+    if classes is not None:                                   # SGDClassifier.fit keeps its loss object; the regressor does not
+        est._loss_function_ = est._get_loss_function(est.loss)
+    if est.tol is not None and est.tol > -np.inf and est.n_iter_ == est.max_iter:
+        from sklearn.exceptions import ConvergenceWarning
+        warnings.warn("Maximum number of iteration reached before convergence. Consider increasing max_iter to improve the "
+                      "fit.", ConvergenceWarning)
     return est
 
 

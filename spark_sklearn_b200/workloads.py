@@ -142,6 +142,34 @@ def _linsvr(which="small"):
     return w
 
 
+def _sgd(which="small"):
+    """SGDClassifier / SGDRegressor (csrc/sgd.cu): config 3's recipe at 2000 x 32 (small, binary), a 4-class set (multi), the
+    SVR recipe (reg_small), and a 100-candidate x cv=5 search on 20000 x 128, 4 classes (c: 2000 one-vs-rest fits,
+    tools/bench_sgd.py)."""
+    from sklearn.datasets import make_classification
+    from sklearn.preprocessing import StandardScaler
+    if which == "reg_small":
+        w = _svr(n=2000, d=32, name="sgd_reg_small",
+                 grid={"alpha": [1e-4, 1e-2], "loss": ["squared_error", "huber", "epsilon_insensitive"],
+                       "penalty": ["l2", "elasticnet"]})
+        w.update(estimator="SGDRegressor", est_params={"random_state": 0})
+        return w
+    if which == "small":
+        w = _c3(n=2000, d=32, name="sgd_small")
+        w.update(estimator="SGDClassifier", est_params={"random_state": 0}, search="grid",
+                 param_grid={"alpha": [1e-5, 1e-4, 1e-3], "loss": ["hinge", "modified_huber", "log_loss"],
+                             "penalty": ["l2", "l1"]})
+        return w
+    n, d, grid = (3000, 32, {"alpha": [1e-4, 1e-3], "loss": ["hinge", "squared_hinge"], "learning_rate": ["optimal", "adaptive"],
+                             "eta0": [0.01]}) if which == "multi" else \
+        (20000, 128, {"alpha": np.logspace(-6, -1, 25), "loss": ["hinge", "log_loss"], "penalty": ["l2", "elasticnet"]})
+    X, y = make_classification(n_samples=n, n_features=d, n_informative=d // 4, n_redundant=0, n_classes=4, class_sep=1.0,
+                               flip_y=0.02, random_state=0)
+    X = np.ascontiguousarray(StandardScaler().fit_transform(X).astype(np.float32))
+    return dict(name="sgd_" + which, X=X, y=y.astype(np.int64), estimator="SGDClassifier", est_params={"random_state": 0},
+                param_grid=grid, cv=5, search="grid")
+
+
 def _knn(which="small"):
     """k-nearest neighbours: config 3's recipe at 2000 x 32 (small, binary), a 4-class set (multi), the SVR recipe (reg_small),
     config 2's data with a 200-fit grid (c2) and config 3's 50000 x 256 data with a smaller grid (c3: the row-slab case)."""
@@ -214,6 +242,12 @@ WORKLOADS = {
     "linsvr_small": _linsvr,
     "linsvr_wide": lambda: _linsvr("wide"),
     "linsvr_c": lambda: _linsvr("c"),
+    # SGDClassifier / SGDRegressor (csrc/sgd.cu): golden-sized binary, 4-class and regression grids, and the 2000-fit search
+    # (tools/bench_sgd.py)
+    "sgd_small": _sgd,
+    "sgd_multi": lambda: _sgd("multi"),
+    "sgd_reg_small": lambda: _sgd("reg_small"),
+    "sgd_c": lambda: _sgd("c"),
     # k-nearest neighbours (csrc/knn.cu): one neighbour selection per (split, metric) serves every candidate
     "knn_small": _knn,
     "knn_multi": lambda: _knn("multi"),
@@ -253,7 +287,7 @@ def make_estimator(w):
     if w["estimator"] in ("KNeighborsClassifier", "KNeighborsRegressor"):
         import sklearn.neighbors as nb
         return getattr(nb, w["estimator"])(**w["est_params"])
-    if w["estimator"] in ("Lasso", "ElasticNet"):
+    if w["estimator"] in ("Lasso", "ElasticNet", "SGDClassifier", "SGDRegressor"):
         import sklearn.linear_model as lm
         return getattr(lm, w["estimator"])(**w["est_params"])
     raise ValueError(w["estimator"])
