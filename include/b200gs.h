@@ -412,6 +412,38 @@ int gs_sgd_refit(gs_handle *h, int32_t loss, int32_t penalty, double alpha, doub
 /* Test hook: pi, the permutation of l positions the SGD shuffle with this seed applies every epoch. */
 int gs_debug_sgd_perm(gs_handle *h, uint32_t seed, int32_t l, int32_t *out);
 
+/*
+ * LogisticRegression(solver='sag' | 'saga') (csrc/sag.cu).  Replaces: LogisticRegression.fit / score per (candidate, split)
+ * (reference base_search.py:83-87) with scikit-learn's sag_solver (_sag_fast.pyx.tp sag64 / sag32) restated step for step,
+ * one warp per fit.  loss: GS_SAG_LOG (two classes, y = 1 for class 1, 0 otherwise), GS_SAG_MULTINOMIAL (three or more
+ * classes, y = the class index) or GS_SAG_SQUARED (a regression gs_set_data with gs_set_targets_f64: sag_solver's squared
+ * loss, which reports coef_out only).  Per fit t = c * n_splits + k, computed on the host as sag_solver computes them:
+ * solver[t] (GS_SAG_SOLVER_SAG / GS_SAG_SOLVER_SAGA), alpha_scaled[t] = alpha / n_train, beta_scaled[t] = beta / n_train
+ * (the L1 term, applied by SAGA only), step[t] (get_auto_step_size), seed[t] (make_dataset's draw).  Scalars: tol,
+ * max_iter (>= 0), fit_intercept.  Rows: a split's training rows in gs_set_train_order's order (default ascending), none
+ * dropped; sample weights (gs_set_sample_weight) times class weights (gs_set_class_weight: one set, or one per split),
+ * rounded to X's dtype as scikit-learn multiplies them.  X is float32 (sag32: every value scikit-learn keeps in float is
+ * rounded to float) or float64 (sag64).  d x K <= GS_SAG_MAX_COEF, K = n_classes with GS_SAG_MULTINOMIAL, else 1.
+ * Scores: every classification scorer (roc_auc binary), from the float64 decision values [X | 1] . [coef | intercept] of
+ * one FP64 tensor-core contraction.  Per fit: n_iter (sag's n_iter_), fit_status 0 stopped by the tol rule, 1 ran max_iter
+ * epochs, 2 a weight or the intercept became non-finite (scores NaN; n_iter is that epoch, as scikit-learn's ValueError
+ * reports it).  coef_out (may be NULL but for the squared loss) [t][K][d + 1] every fit's weights then intercept; stats
+ * (may be NULL) [t][2] = sample steps, clock cycles of the whole fit.
+ * gs_logreg_sag_refit: one fit on every row in row order; coef_out [K][d + 1], n_iter [1], fit_status [1].
+ */
+#define GS_SAG_MAX_COEF 512
+enum { GS_SAG_LOG = 0, GS_SAG_MULTINOMIAL = 1, GS_SAG_SQUARED = 2 };
+enum { GS_SAG_SOLVER_SAG = 0, GS_SAG_SOLVER_SAGA = 1 };
+int gs_logreg_sag(gs_handle *h, int32_t n_cand, const int32_t *solver, const double *alpha_scaled, const double *beta_scaled,
+                  const double *step, const uint32_t *seed, int32_t loss, double tol, int32_t max_iter, int32_t fit_intercept,
+                  uint32_t flags, double *test_scores, double *train_scores, int32_t *n_iter, int32_t *fit_status, float *fit_ms,
+                  float *score_ms, double *coef_out, int64_t *stats);
+int gs_logreg_sag_refit(gs_handle *h, int32_t solver, double alpha_scaled, double beta_scaled, double step, uint32_t seed,
+                        int32_t loss, double tol, int32_t max_iter, int32_t fit_intercept, double *coef_out, int32_t *n_iter,
+                        int32_t *fit_status);
+/* Test hook: the first count sample positions (of n) the device SAG draws from this seed. */
+int gs_debug_sag_draws(gs_handle *h, uint32_t seed, int32_t n, int32_t count, int32_t *out);
+
 /* C[M][N] = sum_k A[M][k]*B[N][k] on the FP64 tensor-core path of gs_linsvc (K > 1024: split-K with the fixed-order sum of
  * the partials), host float64 row-major in/out. */
 int gs_debug_gemm_f64(gs_handle *h, const double *A, int32_t M, const double *B, int32_t N, int32_t K, double *C);

@@ -77,7 +77,7 @@ __global__ void gather_rows_kernel(const T *__restrict__ src, const int *__restr
 
 extern "C" {
 
-int gs_version(void) { return 108; }
+int gs_version(void) { return 109; }
 
 int gs_set_class_weight(gs_handle *h, const double *w, int32_t n_sets)
 {

@@ -23,6 +23,7 @@
 // wscale, sq_norm and l1_norm stay double; every operation scikit-learn rounds to float is rounded to float (a float
 // operation made in double and rounded once gives the float result: 53 >= 2 x 24 + 2).
 #include "common.cuh"
+#include "sequential.cuh"
 #include <algorithm>
 #include <cmath>
 #include <cstring>
@@ -48,10 +49,6 @@ struct SgdFit {
     uint32_t seed;         // the shuffle seed
     double wpos, wneg;     // class weights of the +1 and the other rows
 };
-
-template <typename T> __host__ __device__ __forceinline__ double rnd(double v);
-template <> __host__ __device__ __forceinline__ double rnd<double>(double v) { return v; }
-template <> __host__ __device__ __forceinline__ double rnd<float>(double v) { return (double)(float)v; }
 
 // sklearn's log1pexp (_loss.pyx.tp)
 __host__ __device__ inline double log1pexp(double x)
@@ -124,9 +121,7 @@ __device__ __forceinline__ double sgd_dloss_rn(int loss, double th, double y, do
         if (z >= -1.0) return __dmul_rn(__dmul_rn(2.0, __dsub_rn(1.0, z)), -y);
         return __dmul_rn(-4.0, y);
     }
-    case GS_SGD_LOG_LOSS:
-        if (p > -37) { const double e = exp(-p); return __ddiv_rn(__dsub_rn(__dsub_rn(1.0, y), __dmul_rn(y, e)), __dadd_rn(1.0, e)); }
-        return __dsub_rn(exp(p), y);
+    case GS_SGD_LOG_LOSS: return grad_half_binomial(y, p);
     case GS_SGD_SQUARED_ERROR: return __dsub_rn(p, y);
     case GS_SGD_HUBER: { const double r = __dsub_rn(p, y); return fabs(r) <= th ? r : (r >= 0 ? th : -th); }
     case GS_SGD_EPSILON_INSENSITIVE: return __dsub_rn(y, p) > th ? -1.0 : (__dsub_rn(p, y) > th ? 1.0 : 0.0);
@@ -143,25 +138,13 @@ __device__ __forceinline__ double sgd_dloss_rn(int loss, double th, double y, do
 __device__ void sgd_draw_perm(uint32_t seed, int l, int *perm)
 {
     for (int i = 0; i < l; i++) perm[i] = i;
-    uint32_t s = seed ? seed : 1u;                                  // our_rand_r: a zero seed becomes DEFAULT_SEED
+    uint32_t s = seed;
     for (int i = 0; i < l - 1; i++) {
-        s ^= s << 13;
-        s ^= s >> 17;
-        s ^= s << 5;
-        const int j = i + (int)((s & 0x7fffffffu) % (uint32_t)(l - i));
+        const int j = i + (int)(our_rand_r(s) % (uint32_t)(l - i));
         const int a = perm[i];
         perm[i] = perm[j];
         perm[j] = a;
     }
-}
-
-// sum of v[0 .. d) in order, every lane (broadcast reads)
-__device__ __forceinline__ double seq_sum(const double *v, int d)
-{
-    double a = 0.0;
-#pragma unroll 8
-    for (int j = 0; j < d; j++) a = __dadd_rn(a, v[j]);
-    return a;
 }
 
 template <int NT, typename T, bool L1>
@@ -266,7 +249,7 @@ sgd_kernel(const SgdFit *__restrict__ fits, int nfits, const SgdCand *__restrict
                 l1_norm = __dmul_rn(a2, pend_ws);
                 pend = false;
             } else {
-                dot = seq_sum(sd, d);
+                dot = seq_sum<double>(sd, d, 1);
             }
             const double p = __dadd_rn(rnd<T>(__dmul_rn(dot, wscale)), intercept);
             if (P.lr == OPTIMAL) eta = __ddiv_rn(1.0, __dmul_rn(alpha, __dsub_rn(__dadd_rn(P.optimal_init, tt), 1.0)));

@@ -100,6 +100,9 @@ def load_library():
     L.gs_sgd_refit.argtypes = [vp, i32, i32, dbl, dbl, dbl, i32, dbl, dbl, vp, dbl, i32, i32, i32, i32, vp, vp, vp]
     L.gs_debug_sgd_perm.argtypes = [vp, u32, i32, vp]
     L.gs_debug_mt19937.argtypes = [vp, u32, i32, vp]
+    L.gs_logreg_sag.argtypes = [vp, i32, vp, vp, vp, vp, vp, i32, dbl, i32, i32, u32, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.gs_logreg_sag_refit.argtypes = [vp, i32, dbl, dbl, dbl, u32, i32, dbl, i32, i32, vp, vp, vp]
+    L.gs_debug_sag_draws.argtypes = [vp, u32, i32, i32, vp]
     L.gs_knn.argtypes = [vp, i32, vp, vp, vp, u32, vp, vp, vp, vp]
     L.gs_debug_knn_neighbors.argtypes = [vp, i32, i32, i32, vp, vp]
     L.gs_get_profile.argtypes = [vp, c.POINTER(GsProfile)]
@@ -119,7 +122,8 @@ def load_library():
               "gs_svr", "gs_svr_refit", "gs_nusvc", "gs_nusvc_refit", "gs_nusvr", "gs_nusvr_refit", "gs_logreg",
               "gs_logreg_refit", "gs_linsvc", "gs_linsvc_refit", "gs_get_profile", "gs_debug_gram", "gs_debug_kernel_matrix",
               "gs_debug_decision", "gs_debug_score", "gs_debug_linear", "gs_debug_gemm_nt", "gs_debug_gemm_f64", "gs_knn", "gs_debug_knn_neighbors",
-              "gs_linsvr", "gs_linsvr_refit", "gs_set_train_order", "gs_debug_mt19937", "gs_sgd", "gs_sgd_refit", "gs_debug_sgd_perm"):
+              "gs_linsvr", "gs_linsvr_refit", "gs_set_train_order", "gs_debug_mt19937", "gs_sgd", "gs_sgd_refit", "gs_debug_sgd_perm",
+              "gs_logreg_sag", "gs_logreg_sag_refit", "gs_debug_sag_draws"):
         getattr(L, f).restype = c.c_int
     _lib = L
     return L
@@ -485,6 +489,61 @@ class Engine:
         """pi: the permutation of l positions the device SGD shuffle with this seed applies every epoch"""
         out = np.zeros(int(l), np.int32)
         self._check(self._L.gs_debug_sgd_perm(self._h, int(seed), int(l), _ptr(out)))
+        return out
+
+    SAG_LOSS = {"log": 0, "multinomial": 1, "squared": 2}
+    SAG_SOLVER = {"sag": 0, "saga": 1}
+
+    def logreg_sag(self, solver, alpha_scaled, beta_scaled, step, seed, loss, tol=1e-4, max_iter=100, fit_intercept=True,
+                   return_train=True, return_coef=False, return_stats=False):
+        """LogisticRegression(solver='sag' | 'saga') per (candidate, split) (include/b200gs.h gs_logreg_sag): solver ('sag' /
+        'saga' or codes), alpha_scaled, beta_scaled, step and seed [n_cand][n_splits] as sag_solver computes them; loss 'log',
+        'multinomial' or 'squared' (a regression dataset: coef only).  -> test / train scores, n_iter, status (0 stopped,
+        1 max_iter, 2 non-finite), fit_ms, score_ms; return_coef: coef [n_cand][n_splits][K][d + 1] (weights, then
+        intercept); return_stats: stats [n_cand][n_splits][2] (sample steps, fit cycles)"""
+        solver = np.asarray([[self.SAG_SOLVER.get(v, v) if isinstance(v, str) else v for v in row]
+                             for row in np.atleast_2d(np.asarray(solver, object))], np.int64)
+        shape = solver.shape
+        assert shape[1] == self.n_splits
+        f64 = lambda v: np.ascontiguousarray(np.broadcast_to(np.asarray(v, np.float64), shape))
+        solver = np.ascontiguousarray(solver, np.int32)
+        seed = np.ascontiguousarray(np.broadcast_to(np.asarray(seed, np.int64), shape), np.uint32)
+        a, b, st = f64(alpha_scaled), f64(beta_scaled), f64(step)
+        lcode = self.SAG_LOSS[loss] if isinstance(loss, str) else int(loss)
+        k = self.n_classes if lcode == 1 else 1
+        out = dict(test=np.zeros(shape), train=np.zeros(shape), n_iter=np.zeros(shape, np.int32), status=np.zeros(shape, np.int32),
+                   fit_ms=np.zeros(shape, np.float32), score_ms=np.zeros(shape, np.float32))
+        coef = np.zeros(shape + (k, self.d + 1)) if return_coef or lcode == 2 else None
+        stats = np.zeros(shape + (2,), np.int64) if return_stats else None
+        self._check(self._L.gs_logreg_sag(self._h, shape[0], _ptr(solver), _ptr(a), _ptr(b), _ptr(st), _ptr(seed), lcode,
+                                          float(tol), int(max_iter), int(bool(fit_intercept)),
+                                          GS_RETURN_TRAIN if return_train else 0, _ptr(out["test"]), _ptr(out["train"]),
+                                          _ptr(out["n_iter"]), _ptr(out["status"]), _ptr(out["fit_ms"]), _ptr(out["score_ms"]),
+                                          _ptr(coef), _ptr(stats)))
+        if not return_train:
+            out["train"] = None
+        if coef is not None:
+            out["coef"] = coef
+        if return_stats:
+            out["stats"] = stats
+        return out
+
+    def logreg_sag_refit(self, solver, alpha_scaled, beta_scaled, step, seed, loss, tol=1e-4, max_iter=100, fit_intercept=True):
+        """one fit on every row -> (coef [K][d + 1]: weights then intercept, n_iter, status)"""
+        lcode = self.SAG_LOSS[loss] if isinstance(loss, str) else int(loss)
+        k = self.n_classes if lcode == 1 else 1
+        coef = np.zeros((k, self.d + 1))
+        it = np.zeros(1, np.int32)
+        st = np.zeros(1, np.int32)
+        self._check(self._L.gs_logreg_sag_refit(self._h, self.SAG_SOLVER.get(solver, solver), float(alpha_scaled),
+                                                float(beta_scaled), float(step), int(seed), lcode, float(tol), int(max_iter),
+                                                int(bool(fit_intercept)), _ptr(coef), _ptr(it), _ptr(st)))
+        return coef, int(it[0]), int(st[0])
+
+    def debug_sag_draws(self, seed, n, count):
+        """the first count sample positions (of n) the device SAG draws from this seed"""
+        out = np.zeros(int(count), np.int32)
+        self._check(self._L.gs_debug_sag_draws(self._h, int(seed), int(n), int(count), _ptr(out)))
         return out
 
     def knn(self, n_neighbors, weights, metric, return_train=True, y_f32=False):

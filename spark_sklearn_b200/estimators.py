@@ -3,7 +3,7 @@ and turn refit buffers back into genuine fitted scikit-learn estimators for ``be
 (reference base_search.py:165-174 delegates ``predict`` & co. to it).
 
 Only estimators with a CUDA path are accepted (SVC with the linear, rbf, poly and sigmoid kernels, SVR rbf/linear, Ridge,
-Lasso / ElasticNet, LogisticRegression, LinearSVC with the primal squared-hinge solver -- the families the reference ships
+Lasso / ElasticNet, LogisticRegression (lbfgs, sag, saga), LinearSVC with the primal squared-hinge solver -- the families the reference ships
 examples for -- LinearSVR, SGDClassifier / SGDRegressor, and KNeighborsClassifier / KNeighborsRegressor); anything else raises: no CPU fallback.
 """
 import copy
@@ -878,6 +878,14 @@ class LogRegAdapter:
 
     @staticmethod
     def plan(estimator, cands, X, y, fold_id, n_splits, device=None):
+        """lbfgs candidates run LogRegPlan, sag / saga candidates LogRegSAGPlan; one search runs one of the two"""
+        base = estimator.get_params(deep=False).get("solver", "lbfgs")
+        solvers = {c.get("solver", base) for c in cands} or {base}
+        if solvers & {"sag", "saga"}:
+            if not solvers <= {"sag", "saga"}:
+                raise NotImplementedError("LogisticRegression: a search that mixes solver='sag' / 'saga' with %s has no CUDA path "
+                                          "(search the two in separate searches)" % sorted(solvers - {"sag", "saga"}))
+            return LogRegSAGPlan(estimator, cands, X, y, fold_id, n_splits, device)
         return LogRegPlan(estimator, cands, X, y, fold_id, n_splits, device)
 
 
@@ -952,6 +960,221 @@ class LogRegPlan(_Plan):
         est.n_iter_ = np.array([it], np.int32)
         est.n_features_in_ = self.X.shape[1]
         return est
+
+
+def sag_seed(random_state):
+    """make_dataset's draw for one LogisticRegression(solver='sag' | 'saga') fit: check_random_state(random_state).randint(1,
+    np.iinfo(np.int32).max).  An int or a RandomState gives the same seed to every fit (clone deep-copies the parameter, so
+    the caller's RandomState is not advanced); None draws from numpy's global RandomState."""
+    from sklearn.utils import check_random_state
+    if random_state is not None and not isinstance(random_state, (numbers.Integral, np.random.RandomState)):
+        raise ValueError("%r cannot be used to seed a numpy.random.RandomState instance" % (random_state,))
+    rs = copy.deepcopy(random_state) if isinstance(random_state, np.random.RandomState) else random_state
+    return int(check_random_state(rs).randint(1, _INT_MAX))
+
+
+class LogRegSAGPlan(_Plan):
+    """sklearn.linear_model.LogisticRegression(solver='sag' | 'saga') (csrc/sag.cu): sag_solver restated step for step, one
+    warp per (candidate, split) fit.  X reaches the device dense in its own dtype (float32 runs sag32, float64 sag64, as
+    scikit-learn does).  The step size and the scaled penalties of every fit come from scikit-learn's own functions on that
+    fit's training rows, which reach the device in the splitter's order (the sample draws index them)."""
+    scorers = CLASSIFICATION_SCORERS
+    supports_sample_weight = True
+    max_coef = 512             # features x weight rows held in registers (include/b200gs.h GS_SAG_MAX_COEF)
+
+    def __init__(self, estimator, cands, X, y, fold_id, n_splits, device=None):
+        import scipy.sparse as sp
+        if sp.issparse(X):
+            raise NotImplementedError("LogisticRegression(solver='sag' | 'saga') on sparse X has no CUDA path (scikit-learn's "
+                                      "sparse SAG decays the intercept and lags its updates per stored entry): pass a dense X")
+        super().__init__(estimator, cands, X, y, fold_id, n_splits, device)
+        if y is None:
+            raise ValueError("LogisticRegression needs y")
+        self.classes, self.y_class = np.unique(np.asarray(y), return_inverse=True)
+        if len(self.classes) < 2:
+            raise ValueError("This solver needs samples of at least 2 classes in the data, but the data contains only one "
+                             "class: %r" % (self.classes[0],))
+        if len(self.classes) > 64:
+            raise NotImplementedError("LogisticRegression CUDA path handles up to 64 classes (got %d)" % len(self.classes))
+        self.kc = len(self.classes) if len(self.classes) > 2 else 1
+        self.loss = "multinomial" if self.kc > 1 else "log"
+        if self.X.shape[1] * self.kc > self.max_coef:
+            raise NotImplementedError("LogisticRegression(solver='sag' | 'saga') with %d features x %d weight rows: the CUDA "
+                                      "path handles up to %d" % (self.X.shape[1], self.kc, self.max_coef))
+        self._set_data(self.X, y_class=self.y_class.astype(np.int32))
+        if self.folds is not None:
+            self.engine.set_train_order(self.folds.train_order)
+        self._seeds = None
+        self._mss = {}
+
+    def _resolve(self, p):
+        """LogisticRegression.fit's checks and penalty resolution (scikit-learn 1.9): ValueError as scikit-learn raises it;
+        -> (solver, alpha, beta, C) with alpha / beta sag_solver's L2 and L1 terms before the 1 / n scaling"""
+        from sklearn.linear_model import LogisticRegression
+        from sklearn.linear_model._logistic import _check_solver
+        LogisticRegression(**p)._validate_params()
+        if p["penalty"] == "deprecated":
+            l1r = p["l1_ratio"]
+            if l1r == 0 or l1r is None:
+                penalty = "l2"
+                if l1r is None:
+                    warnings.warn("'l1_ratio=None' was deprecated in version 1.8 and will trigger an error in 1.10. Use "
+                                  "0<=l1_ratio<=1 instead.", FutureWarning)
+            elif l1r == 1:
+                penalty = "l1"
+            else:
+                penalty = "elasticnet"
+            if p["C"] == np.inf:
+                penalty = None
+        else:
+            penalty = p["penalty"]
+            warnings.warn("'penalty' was deprecated in version 1.8 and will be removed in 1.10. To avoid this warning, leave "
+                          "'penalty' set to its default value and use 'l1_ratio' or 'C' instead. Use l1_ratio=0 instead of "
+                          "penalty='l2', l1_ratio=1 instead of penalty='l1', l1_ratio set to a float between 0 and 1 instead "
+                          "of penalty='elasticnet', and C=np.inf instead of penalty=None.", FutureWarning)
+        solver = _check_solver(p["solver"], penalty, p["dual"])
+        if penalty == "elasticnet" and p["l1_ratio"] is None:
+            raise ValueError("l1_ratio must be specified when penalty is elasticnet.")
+        C = np.inf if p["penalty"] is None else p["C"]
+        if p["penalty"] is None:
+            penalty = "l2"
+        if penalty == "l1":
+            alpha, beta = 0.0, 1.0 / C
+        elif penalty == "l2":
+            alpha, beta = 1.0 / C, 0.0
+        else:
+            alpha, beta = (1.0 / C) * (1 - p["l1_ratio"]), (1.0 / C) * p["l1_ratio"]
+        return solver, alpha, beta
+
+    def _rows(self, k):
+        """the training rows of split k in the order the fit sees them (k < 0: every row)"""
+        if k < 0:
+            return np.arange(len(self.X))
+        if self.folds is not None:
+            return self.folds.train_order[k]
+        return np.flatnonzero(self.fold_id != k)
+
+    def _step(self, k, solver, alpha, beta, fit_intercept):
+        """sag_solver's (step, alpha_scaled, beta_scaled) on split k's training rows, computed by scikit-learn's functions in
+        X's dtype; ZeroDivisionError where sag_solver raises it"""
+        from sklearn.linear_model._sag import get_auto_step_size
+        from sklearn.utils.extmath import row_norms
+        rows = self._rows(k)
+        if k not in self._mss:
+            self._mss[k] = row_norms(self.X[rows], squared=True).max()
+        n = len(rows)
+        a, b = float(alpha) / n, float(beta) / n
+        step = get_auto_step_size(self._mss[k], a, self.loss, fit_intercept, n_samples=n, is_saga=solver == "saga")
+        if step * a == 1:
+            raise ZeroDivisionError("Current sag implementation does not handle the case step_size * alpha_scaled == 1")
+        return float(step), a, b
+
+    def _class_weights(self, cw, k):
+        """_logistic_regression_path: compute_class_weight on the training rows with their sample weights in X's dtype"""
+        from sklearn.utils.class_weight import compute_class_weight
+        rows = self._train_rows(k)
+        sw = getattr(self, "sample_weight", None)
+        sw = np.ones(int(rows.sum())) if sw is None else sw[rows]
+        return compute_class_weight(cw, classes=self.classes, y=np.asarray(self.y)[rows], sample_weight=sw.astype(self.X.dtype))
+
+    def _draw_seeds(self, states):
+        table = np.zeros((len(states), self.n_splits), np.int64)
+        for c, rs in enumerate(states):
+            if rs is None:
+                for k in range(self.n_splits):
+                    table[c, k] = sag_seed(None)
+            else:
+                table[c, :] = sag_seed(rs)
+        return table
+
+    def evaluate(self, my, return_train=True, error_score='raise'):
+        ns = self.n_splits
+        shape = (len(my), ns)
+        res = dict(test=np.zeros(shape), train=np.zeros(shape), fit_ms=np.zeros(shape), score_ms=np.zeros(shape),
+                   n_iter=np.zeros(shape, np.int64), status=np.zeros(shape, np.int64))
+        params = [self._base_params(self.cands[ci]) for ci in my]
+        resolved = [self._resolve(p) for p in params]
+        fits = np.zeros(shape + (4,))                       # solver, step, alpha_scaled, beta_scaled
+        zero_div = np.zeros(shape, bool)
+        for j, (p, (solver, alpha, beta)) in enumerate(zip(params, resolved)):
+            for k in range(ns):
+                try:
+                    fits[j, k] = (solver == "saga",) + self._step(k, solver, alpha, beta, bool(p["fit_intercept"]))
+                except ZeroDivisionError:
+                    if error_score == 'raise':
+                        raise
+                    zero_div[j, k] = True
+                    fits[j, k] = (solver == "saga", 1.0, 0.0, 0.0)
+        seeds = search_seed_table(self, self._draw_seeds)
+        groups = {}
+        for j, p in enumerate(params):
+            cw = p["class_weight"]
+            cwk = None if cw is None else (cw if isinstance(cw, str) else tuple(sorted(cw.items())))
+            groups.setdefault((float(p["tol"]), int(p["max_iter"]), bool(p["fit_intercept"]), cwk), []).append(j)
+        prof = {}
+        self.stats_ = np.zeros(shape + (2,), np.int64)
+        for (tol, mi, fi, _cwk), idx in groups.items():
+            self._set_class_weight(params[idx[0]]["class_weight"])
+            self.engine.set_scoring(self.score_kind, self.score_pos)
+            f = fits[idx]
+            r = self.engine.logreg_sag(f[..., 0].astype(np.int64), f[..., 2], f[..., 3], f[..., 1], seeds[[my[j] for j in idx]],
+                                       self.loss, tol=tol, max_iter=mi, fit_intercept=fi, return_train=return_train,
+                                       return_stats=True)
+            for key in ("test", "fit_ms", "score_ms", "n_iter", "status"):
+                res[key][idx] = r[key]
+            if return_train:
+                res["train"][idx] = r["train"]
+            self.stats_[idx] = r["stats"]
+            for k, v in self.engine.profile().items():
+                prof[k] = prof.get(k, 0) + v
+        self.engine.set_class_weight(None)
+        self._prof = prof
+        self.n_iter_ = res["n_iter"]
+        bad = (res["status"] == 2) | zero_div
+        if bad.any():
+            if error_score == 'raise':
+                j, k = map(int, np.argwhere(bad)[0])
+                raise SGDPlan._overflow(int(res["n_iter"][j, k]))
+            warnings.warn("%d fits failed (a floating-point under-/overflow, or step_size * alpha_scaled == 1); their scores "
+                          "are error_score=%r" % (int(bad.sum()), error_score))
+            res["test"][bad] = error_score
+            if return_train:
+                res["train"][bad] = error_score
+        return self._finish(res, return_train, error_score, len(my))
+
+    def refit(self, best_params):
+        p = self._base_params(best_params)
+        solver, alpha, beta = self._resolve(p)
+        step, a, b = self._step(-1, solver, alpha, beta, bool(p["fit_intercept"]))
+        seed = sag_seed(p["random_state"])                    # the refit's own draw, after every search fit's
+        self._set_class_weight(p["class_weight"], refit=True)
+        try:
+            coef, n_iter, status = self.engine.logreg_sag_refit(solver, a, b, step, seed, self.loss, tol=p["tol"],
+                                                                max_iter=p["max_iter"], fit_intercept=p["fit_intercept"])
+        finally:
+            self.engine.set_class_weight(None)
+        if status == 2:
+            raise SGDPlan._overflow(n_iter)
+        est = clone(self.estimator).set_params(**best_params)
+        return materialize_logreg_sag(est, self.X, coef, n_iter, self.classes)
+
+
+def materialize_logreg_sag(est, X, coef, n_iter, classes):
+    """Fill a (cloned, parametrised) LogisticRegression with the fitted state of one sag_solver fit coef [K][d + 1] (weights,
+    then intercept): coef_ [K][d] and intercept_ [K] in X's dtype (zeros without an intercept), n_iter_ = array([n_iter]),
+    classes_, n_features_in_ (linear_model/_logistic.py LogisticRegression.fit), with sag_solver's ConvergenceWarning."""
+    d = X.shape[1]
+    dt = np.float32 if X.dtype == np.float32 else np.float64
+    coef = np.asarray(coef, np.float64)
+    est.classes_ = np.asarray(classes)
+    est.coef_ = coef[:, :d].astype(dt)
+    est.intercept_ = coef[:, d].astype(dt) if est.fit_intercept else np.zeros(len(coef), dt)
+    est.n_iter_ = np.array([n_iter], np.int32)
+    est.n_features_in_ = int(d)
+    if n_iter == est.max_iter:
+        from sklearn.exceptions import ConvergenceWarning
+        warnings.warn("The max_iter was reached which means the coef_ did not converge", ConvergenceWarning)
+    return est
 
 
 # ------------------------------------------------------------------ LinearSVC -----------------

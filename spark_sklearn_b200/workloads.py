@@ -170,6 +170,27 @@ def _sgd(which="small"):
                 param_grid=grid, cv=5, search="grid")
 
 
+def _sag(which="small"):
+    """LogisticRegression(solver='sag' | 'saga') (csrc/sag.cu): a golden-sized binary grid over C and l1_ratio (small), a
+    3-class one (multi), and the usual saga grid of 10 C x 5 l1_ratio values x cv=5 on 20000 x 128 standardised rows, binary
+    and 4 classes (c2 / c4: 250 fits each, tools/bench_sag.py)."""
+    from sklearn.datasets import make_classification
+    from sklearn.preprocessing import StandardScaler
+    n, d, k, grid, est = {
+        "small": (600, 16, 2, {"C": [0.01, 1.0, 100.0], "l1_ratio": [0.0, 0.5, 1.0]}, {"solver": "saga", "random_state": 0}),
+        "multi": (600, 12, 3, {"C": [0.1, 10.0], "solver": ["sag", "saga"]}, {"random_state": 0}),
+        "c2": (20000, 128, 2, {"C": list(np.logspace(-3, 2, 10)), "l1_ratio": [0.0, 0.25, 0.5, 0.75, 1.0]},
+               {"solver": "saga", "random_state": 0}),
+        "c4": (20000, 128, 4, {"C": list(np.logspace(-3, 2, 10)), "l1_ratio": [0.0, 0.25, 0.5, 0.75, 1.0]},
+               {"solver": "saga", "random_state": 0}),
+    }[which]
+    X, y = make_classification(n_samples=n, n_features=d, n_informative=max(4, d // 4), n_redundant=2, n_classes=k,
+                               n_clusters_per_class=1, flip_y=0.05, random_state=11)
+    X = StandardScaler().fit_transform(X)
+    return dict(name="sag_" + which, X=X, y=y.astype(np.int64), estimator="LogisticRegression", est_params=est,
+                param_grid=grid, cv=5, search="grid")
+
+
 def _knn(which="small"):
     """k-nearest neighbours: config 3's recipe at 2000 x 32 (small, binary), a 4-class set (multi), the SVR recipe (reg_small),
     config 2's data with a 200-fit grid (c2) and config 3's 50000 x 256 data with a smaller grid (c3: the row-slab case)."""
@@ -248,6 +269,12 @@ WORKLOADS = {
     "sgd_multi": lambda: _sgd("multi"),
     "sgd_reg_small": lambda: _sgd("reg_small"),
     "sgd_c": lambda: _sgd("c"),
+    # LogisticRegression(solver='sag' | 'saga') (csrc/sag.cu): golden-sized binary and 3-class grids, and the 250-fit saga
+    # grids of tools/bench_sag.py (binary and 4 classes)
+    "sag_small": _sag,
+    "sag_multi": lambda: _sag("multi"),
+    "sag_c2": lambda: _sag("c2"),
+    "sag_c4": lambda: _sag("c4"),
     # k-nearest neighbours (csrc/knn.cu): one neighbour selection per (split, metric) serves every candidate
     "knn_small": _knn,
     "knn_multi": lambda: _knn("multi"),
