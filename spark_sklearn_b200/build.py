@@ -6,7 +6,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libb200gs.so")
-SOURCES = ["api.cu", "kernel_svm.cu", "gram.cu", "smo.cu", "smo_lean.cu", "smo_colown.cu", "score.cu", "svr.cu", "linear.cu", "logreg.cu", "gemm_tc.cu", "gemm_f64.cu", "linsvc.cu", "linsvr.cu", "sgd.cu", "sag.cu", "knn.cu"]
+SOURCES = ["api.cu", "kernel_svm.cu", "linear_search.cu", "gram.cu", "smo.cu", "smo_lean.cu", "smo_colown.cu", "score.cu", "svr.cu", "linear.cu", "logreg.cu", "gemm_tc.cu", "gemm_f64.cu", "linsvc.cu", "linsvr.cu", "sgd.cu", "sag.cu", "knn.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-cudart", "static"]
 

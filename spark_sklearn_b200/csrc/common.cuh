@@ -4,9 +4,12 @@
 #include <stdint.h>
 #include <cmath>
 #include <cstring>
+#include <functional>
 #include <string>
 #include <vector>
 #include "../../include/b200gs.h"
+
+inline int64_t round_up(int64_t x, int64_t m) { return (x + m - 1) / m * m; }
 
 #define GS_CUDA(call)                                                                         \
     do {                                                                                      \
@@ -363,6 +366,49 @@ cudaError_t launch_build_xa64(const float *X32, const double *X64, int n, int d,
 // predicted], pre-zeroed
 cudaError_t launch_linsvc_count(const double *Zt, int64_t ldz, int n, int K, int KC, const int *y, SplitMasks sm,
                                 const int *fold_of_fit, int nfit, int *counts, cudaStream_t st);
+
+// ---- linear_search.cu: the host steps the primal linear searches share (LinearSVC, LinearSVR, SGD, SAG; an int return is
+// a GS_* status).  The fits' weight rows are [mpad][nvp], nvp = round_up(d + 1, 64), mpad = round_up(rows, 64), row
+// f K + q for fit f = candidate x ns + split and decision row q; Xa = [X | bias] is [round_up(n, 64)][nvp] (launch_build_xa64). ----
+// Every split's training rows in fit order, as internal rows: gs_set_train_order's lists, else ascending original index; the
+// refit (ns = 1) trains on every row.  positive_only: only rows of positive sample weight (liblinear's remove_zero_weight).
+// Split k's rows are order[sp_off[k] .. sp_off[k + 1]).  Returns the longest split's row count, 0 when a split has none.
+int train_rows(const gs_handle *h, int ns, bool refit, bool positive_only, std::vector<int> &order, std::vector<int> &sp_off);
+// Rejects, with who in the message, a scorer the dataset cannot take: a classification scorer on a regressor, a regression
+// scorer on a classifier, or a binary-only scorer on K > 1 decision rows per fit
+int check_scorer(gs_handle *h, const char *who, int kind, int K);
+// Rejects class weights given per split for another number of splits than ns
+int check_class_weight_sets(gs_handle *h, const char *who, int ns);
+// liblinear's TRON (tron.cpp) on ncol columns, one round for all open columns at a time: Z = V Xa^T (every column's
+// submission), the caller's element-wise pass (Z, St -> R, F and the spare active set), Gp = R Xat^T split-K over rows, then
+// tron_advance_kernel.  reserve() takes h->dWork[2..6] and zeroes V, Vec, R and the masks; the caller uploads St.
+struct TronRounds {
+    static constexpr int KCH = 2048;           // split-K chunk of the gradient contraction
+    int ncol = 0, nvp = 0, mpad = 0, nchunk = 0;
+    int64_t npad = 0;
+    TrState *St = nullptr;                     // [ncol]
+    double *V = nullptr, *Vec = nullptr;       // submissions [mpad][nvp]; w, g, s, r, d of every column [ncol][NVEC][nvp]
+    double *R = nullptr, *F = nullptr;         // element-wise pass: [mpad][npad] and the loss partials [ncol][PW_BLOCKS]
+    double *Gp = nullptr;                      // gradient partials [nchunk][mpad][nvp]
+    unsigned char *mask = nullptr;             // active sets [2][ncol][npad], current one TrState::cur
+    int *open = nullptr;                       // columns still running after a round
+    int rounds = 0;
+    int reserve(gs_handle *h, int ncol);
+    // rounds until every column is done (GS_ERR_NUMERIC after 10^6, with who in the message); launches += 4 per round
+    int run(gs_handle *h, const char *who, const double *Xa, const double *Xat, double *Z, int max_iter,
+            const std::function<cudaError_t()> &pointwise, int64_t &launches);
+};
+// Scores nfit fits of K decision rows from their weight rows V: Z = V Xa^T in one FP64 contraction (timed by h->tt), then the
+// class counts (and ROC-AUC pair counts) or the residual sums of squares; records ev_end, synchronises and writes
+// test_scores / train_scores (train may be null) with kind's formula.  Z: [mpad][npad].  launches += its launches.
+int score_linear_fits(gs_handle *h, const double *V, const double *Xa, double *Z, int nfit, int K, int ns, int kind,
+                      double *test_scores, double *train_scores, cudaEvent_t ev_end, int64_t &launches);
+void gs_profile_reset(gs_profile &pf);   // clears pf but gs_set_data's ms_h2d / h2d_bytes
+// The profile of a call timed by ev[0] (start), ev[1] (fits done), ev[2] (scores done): reset, then the phase times (also
+// into *ms_solve / *ms_score), their total, the launches and the tensor-core time and flops
+void linear_profile(gs_handle *h, const cudaEvent_t ev[3], int64_t launches, float *ms_solve, float *ms_score);
+// fit_ms / score_ms (either may be null) of the nt tasks of a search call: its solve and score times spread evenly
+void spread_call_ms(int nt, float solve_ms, float score_ms, float *fit_ms, float *score_ms_out);
 
 // ---- gemm_tc.cu: wgmma + TMA contraction  C[M][N] = sum_k A[M][k] B[N][k]  (3xTF32 split, fp32 accumulate) ----
 struct alignas(64) TcMap { unsigned char bytes[128]; };            // CUtensorMap

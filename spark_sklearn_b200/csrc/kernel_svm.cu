@@ -45,10 +45,7 @@ int build_gram(gs_handle *h, uint32_t flags, cudaStream_t st)
 
 void SvmSearch::begin()
 {
-    gs_profile &pf = h->prof;
-    const float keep_h2d = pf.ms_h2d; const int64_t keep_h2d_bytes = pf.h2d_bytes;
-    memset(&pf, 0, sizeof pf);
-    pf.ms_h2d = keep_h2d; pf.h2d_bytes = keep_h2d_bytes;
+    gs_profile_reset(h->prof);
     h->evp.reset(); h->tt.reset();
     ev_begin = h->evp.get(); ev_end = h->evp.get();
     cudaEventRecord(ev_begin, st);

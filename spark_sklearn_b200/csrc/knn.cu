@@ -472,10 +472,7 @@ static int knn_run(gs_handle *h, int n_cand, const int32_t *nn, const int32_t *w
     }
 
     gs_profile &pf = h->prof;
-    const float keep_h2d = pf.ms_h2d;
-    const int64_t keep_h2d_bytes = pf.h2d_bytes;
-    memset(&pf, 0, sizeof pf);
-    pf.ms_h2d = keep_h2d; pf.h2d_bytes = keep_h2d_bytes;
+    gs_profile_reset(pf);
     h->evp.reset();
     EvTimer tm(st, h->evp);
     float acc[3] = {0, 0, 0};

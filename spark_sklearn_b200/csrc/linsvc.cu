@@ -22,6 +22,7 @@
 //   Hv mode:  R = C (X d) on the current active set.
 // liblinear's grad() reads the z of the latest fun() and Hv() the active set of the latest grad(): grad() only ever follows
 // an accepted fun(), so both are the trial point's, which is what the spare mask holds.
+// The host loop of the rounds and the scoring of the final weights are linear_search.cu's (TronRounds, score_linear_fits).
 #include "common.cuh"
 #include <algorithm>
 #include <cmath>
@@ -271,8 +272,6 @@ __global__ void linsvc_count_kernel(const double *__restrict__ Zt, int64_t ldz, 
         if (shc[e]) atomicAdd(&counts[(size_t)f * 6 * K + e], shc[e]);
 }
 
-int64_t round_up(int64_t x, int64_t m) { return (x + m - 1) / m * m; }
-
 int linsvc_run(gs_handle *h, int n_cand, const double *Cv, double tol, int max_iter, int fit_intercept, double intercept_scaling,
                bool refit, double *test_scores, double *train_scores, int32_t *n_iter, double *coef_out, float *ms_solve,
                float *ms_score)
@@ -288,18 +287,16 @@ int linsvc_run(gs_handle *h, int n_cand, const double *Cv, double tol, int max_i
     for (int c = 0; c < n_cand; c++)
         if (!(Cv[c] > 0) || !std::isfinite(Cv[c])) { gs_set_error(h, "gs_linsvc: C must be > 0 and finite"); return GS_ERR_ARG; }
     const int ns = refit ? 1 : h->n_splits, nc = h->n_classes;
+    const int KC = nc > 2 ? nc : 1;
+    if (int e = check_class_weight_sets(h, "gs_linsvc", ns)) return e;
+    if (int e = check_scorer(h, "gs_linsvc", refit ? GS_SCORE_DEFAULT : h->score_kind, KC)) return e;
     const bool weighted = h->class_w_sets > 0;
-    if (weighted && h->class_w_sets != 1 && h->class_w_sets != ns) {
-        gs_set_error(h, "gs_linsvc: gs_set_class_weight was given a weight set per split, but not for this number of splits"); return GS_ERR_ARG;
-    }
     GS_CUDA(cudaSetDevice(h->device));
     cudaStream_t st = h->stream;
     const int n = (int)h->n, d = (int)h->d;
     const int nvp = (int)round_up(d + 1, 64);
     const int64_t npad = round_up(n, 64);
-    const int nfit = n_cand * ns, KC = nc > 2 ? nc : 1, ncol = nfit * KC;
-    const int mpad = (int)round_up(ncol, 64);
-    const int KCH = 2048, nchunk = (int)((npad + KCH - 1) / KCH);              // split-K of the gradient contraction
+    const int nfit = n_cand * ns, ncol = nfit * KC;
 
     // training rows of positive weight per (split, class): liblinear's l, pos, neg after remove_zero_weight
     const bool has_sw = !h->sample_w.empty();
@@ -317,31 +314,18 @@ int linsvc_run(gs_handle *h, int n_cand, const double *Cv, double tol, int max_i
     for (auto &e : ev) e = h->evp.get();
     cudaEventRecord(ev[0], st);
 
-    DevBuf &bXa = h->dWork[0], &bZ = h->dWork[1], &bR = h->dWork[2], &bG = h->dWork[3], &bV = h->dWork[4], &bS = h->dWork[5],
-           &bM = h->dWork[6], &bMeta = h->dWork[7];
+    DevBuf &bXa = h->dWork[0], &bZ = h->dWork[1];
     const size_t xa_elems = (size_t)npad * nvp;
     GS_CUDA(bXa.reserve(xa_elems * 2 * 8 + (size_t)npad * 8));
-    GS_CUDA(bZ.reserve((size_t)mpad * npad * 8));
-    GS_CUDA(bR.reserve((size_t)mpad * npad * 8));
-    GS_CUDA(bG.reserve((size_t)nchunk * mpad * nvp * 8));
-    GS_CUDA(bV.reserve(((size_t)mpad * nvp + (size_t)ncol * NVEC * nvp) * 8));
-    GS_CUDA(bS.reserve((size_t)ncol * sizeof(TrState) + (size_t)ncol * PW_BLOCKS * 8));
-    GS_CUDA(bM.reserve((size_t)2 * ncol * npad));
-    GS_CUDA(bMeta.reserve((size_t)nfit * 4 * 2 + (size_t)nfit * 6 * nc * 4 + 64));
-    double *dXa = bXa.as<double>(), *dXat = dXa + xa_elems, *dW = dXat + xa_elems;
-    double *dZ = bZ.as<double>(), *dR = bR.as<double>(), *dGp = bG.as<double>();
-    double *dV = bV.as<double>(), *dVec = dV + (size_t)mpad * nvp;
-    TrState *dS = bS.as<TrState>();
-    double *dF = reinterpret_cast<double *>(dS + ncol);
-    unsigned char *dMask = bM.as<unsigned char>();
-    int *dFoldOf = bMeta.as<int>(), *dOpen = dFoldOf + nfit, *dCnt = dOpen + 16;
+    GS_CUDA(bZ.reserve((size_t)round_up(ncol, 64) * npad * 8));
+    double *dXa = bXa.as<double>(), *dXat = dXa + xa_elems, *dW = dXat + xa_elems, *dZ = bZ.as<double>();
+    TronRounds tr;
+    if (int e = tr.reserve(h, ncol)) return e;
 
     std::vector<TrState> hs(ncol);
-    std::vector<int> foldof(nfit);
     for (int c = 0; c < n_cand; c++)
         for (int k = 0; k < ns; k++) {
             const int fit = c * ns + k;
-            foldof[fit] = refit ? -100 : k;
             const double *cw = weighted ? &h->class_w[(size_t)(h->class_w_sets == 1 ? 0 : k) * nc] : nullptr;
             int64_t l = 0;
             for (int q = 0; q < nc; q++) l += cnt[(size_t)k * nc + q];
@@ -356,119 +340,36 @@ int linsvc_run(gs_handle *h, int n_cand, const double *Cv, double tol, int max_i
                 S.eps = tol * (double)std::max<int64_t>(std::min(pos, neg), 1) / (double)l;
             }
         }
-    GS_CUDA(cudaMemcpyAsync(dS, hs.data(), (size_t)ncol * sizeof(TrState), cudaMemcpyHostToDevice, st));
-    GS_CUDA(cudaMemcpyAsync(dFoldOf, foldof.data(), (size_t)nfit * 4, cudaMemcpyHostToDevice, st));
+    GS_CUDA(cudaMemcpyAsync(tr.St, hs.data(), (size_t)ncol * sizeof(TrState), cudaMemcpyHostToDevice, st));
     GS_CUDA(cudaMemcpyAsync(dW, W64.data(), (size_t)n * 8, cudaMemcpyHostToDevice, st));
-    GS_CUDA(cudaMemsetAsync(dV, 0, ((size_t)mpad * nvp + (size_t)ncol * NVEC * nvp) * 8, st));   // w0 = 0, the first trial point
-    GS_CUDA(cudaMemsetAsync(dMask, 0, (size_t)2 * ncol * npad, st));
-    GS_CUDA(cudaMemsetAsync(dR, 0, (size_t)mpad * npad * 8, st));                                // rows >= ncol stay zero
-    int64_t launches = 0;
-    {
-        dim3 grid((unsigned)((npad + 31) / 32), (nvp + 31) / 32), block(32, 32);
-        const bool f64 = h->x_dtype == GS_F64;
-        build_xa64_kernel<<<grid, block, 0, st>>>(f64 ? nullptr : h->dX.as<float>(), f64 ? h->dX64.as<double>() : nullptr, n, d,
-                                                  fit_intercept ? intercept_scaling : 0.0, nvp, npad, dXa, dXat);
-        GS_CUDA(cudaGetLastError());
-        launches++;
-    }
-    const double flops_fwd = 2.0 * mpad * (double)npad * nvp;
-    auto forward = [&]() -> int {
-        h->tt.begin(h->evp, st);
-        GS_CUDA(launch_gemm_nt_f64(dV, nvp, dXa, nvp, dZ, npad, mpad, (int)npad, nvp, nvp, 0, st));
-        h->tt.end(h->evp, st, flops_fwd);
-        return GS_OK;
+    GS_CUDA(launch_build_xa64(h->x_dtype == GS_F64 ? nullptr : h->dX.as<float>(), h->x_dtype == GS_F64 ? h->dX64.as<double>() : nullptr,
+                              n, d, fit_intercept ? intercept_scaling : 0.0, nvp, npad, dXa, dXat, st));
+    int64_t launches = 1;
+    const int *Y = h->dY.as<int>();
+    auto pointwise = [&]() {
+        linsvc_pointwise_kernel<<<dim3(PW_BLOCKS, ncol), 256, 0, st>>>(dZ, npad, n, Y, h->masks(), dW, tr.St, tr.mask,
+                                                                       (int64_t)ncol * npad, tr.R, tr.F);
+        return cudaGetLastError();
     };
-    const int pw_threads = 256;
-    int open = 1, rounds = 0;
-    const int max_rounds = 1000000;
-    while (open > 0) {
-        if (++rounds > max_rounds) { gs_set_error(h, "gs_linsvc: TRON did not terminate"); return GS_ERR_NUMERIC; }
-        if (int e = forward()) return e;
-        dim3 grid(PW_BLOCKS, ncol);
-        linsvc_pointwise_kernel<<<grid, pw_threads, 0, st>>>(dZ, npad, n, h->dY.as<int>(), h->masks(), dW, dS, dMask,
-                                                             (int64_t)ncol * npad, dR, dF);
-        GS_CUDA(cudaGetLastError());
-        h->tt.begin(h->evp, st);
-        GS_CUDA(launch_gemm_nt_f64(dR, npad, dXat, npad, dGp, nvp, mpad, nvp, (int)npad, KCH, (int64_t)mpad * nvp, st));
-        h->tt.end(h->evp, st, flops_fwd);
-        GS_CUDA(cudaMemsetAsync(dOpen, 0, 4, st));
-        tron_advance_kernel<<<(ncol + 3) / 4, 128, 0, st>>>(dS, dVec, dV, dGp, nchunk, (int64_t)mpad * nvp, dF, ncol, nvp, max_iter, dOpen);
-        GS_CUDA(cudaGetLastError());
-        GS_CUDA(cudaMemcpyAsync(&open, dOpen, 4, cudaMemcpyDeviceToHost, st));
-        GS_CUDA(cudaStreamSynchronize(st));
-        launches += 4;
-    }
+    if (int e = tr.run(h, "gs_linsvc", dXa, dXat, dZ, max_iter, pointwise, launches)) return e;
     cudaEventRecord(ev[1], st);
 
     std::vector<TrState> fin(ncol);
-    GS_CUDA(cudaMemcpyAsync(fin.data(), dS, (size_t)ncol * sizeof(TrState), cudaMemcpyDeviceToHost, st));
+    GS_CUDA(cudaMemcpyAsync(fin.data(), tr.St, (size_t)ncol * sizeof(TrState), cudaMemcpyDeviceToHost, st));
     if (!refit) {
         // ---- scoring: float64 decision values of the final weights for every row ----
-        export_w_kernel<<<ncol, 128, 0, st>>>(dVec, ncol, nvp, dV);
+        export_w_kernel<<<ncol, 128, 0, st>>>(tr.Vec, ncol, nvp, tr.V);
         GS_CUDA(cudaGetLastError());
-        if (int e = forward()) return e;
-        const int kind = h->score_kind;
-        if (kind == GS_SCORE_NEG_MSE || kind == GS_SCORE_NEG_RMSE) { gs_set_error(h, "gs_linsvc: regression scorer on a classifier"); return GS_ERR_ARG; }
-        if (KC > 1 && (kind == GS_SCORE_ROC_AUC || kind == GS_SCORE_F1 || kind == GS_SCORE_PRECISION || kind == GS_SCORE_RECALL)) {
-            gs_set_error(h, "gs_linsvc: this scorer is defined for binary problems only"); return GS_ERR_UNSUPPORTED;
-        }
-        const int per_fit = 6 * nc;
-        GS_CUDA(cudaMemsetAsync(dCnt, 0, (size_t)nfit * per_fit * 4, st));
-        linsvc_count_kernel<<<dim3(64, nfit), 256, (size_t)per_fit * 4, st>>>(dZ, npad, n, nc, KC, h->dY.as<int>(), h->masks(), dFoldOf, dCnt);
-        GS_CUDA(cudaGetLastError());
-        launches += 3;
-        std::vector<int> ccounts((size_t)nfit * per_fit);
-        GS_CUDA(cudaMemcpyAsync(ccounts.data(), dCnt, ccounts.size() * 4, cudaMemcpyDeviceToHost, st));
-        std::vector<unsigned long long> araw;
-        if (kind == GS_SCORE_ROC_AUC) {
-            std::vector<int> meta((size_t)nfit * 2);
-            for (int f = 0; f < nfit; f++) { meta[f] = f; meta[nfit + f] = f % ns; }
-            GS_CUDA(h->dScore.reserve((size_t)nfit * 40));
-            unsigned long long *d_auc = h->dScore.as<unsigned long long>();
-            int *d_meta = (int *)(d_auc + (size_t)nfit * 4);
-            GS_CUDA(cudaMemcpyAsync(d_meta, meta.data(), meta.size() * 4, cudaMemcpyHostToDevice, st));
-            GS_CUDA(cudaMemsetAsync(d_auc, 0, (size_t)nfit * 32, st));
-            GS_CUDA(launch_auc_pairs_f64(dZ, npad, n, h->class_start[1], h->masks(), d_meta, d_meta + nfit, nfit, +1, d_auc, st));
-            araw.resize((size_t)nfit * 4);
-            GS_CUDA(cudaMemcpyAsync(araw.data(), d_auc, (size_t)nfit * 32, cudaMemcpyDeviceToHost, st));
-            launches++;
-        }
-        cudaEventRecord(ev[2], st);
-        GS_CUDA(cudaStreamSynchronize(st));
-        for (int f = 0; f < nfit; f++) {
-            const int *cc = &ccounts[(size_t)f * per_fit];
-            const int k = f % ns;
-            for (int sp = 0; sp < 2; sp++) {
-                double *out = sp == 0 ? test_scores : train_scores;
-                if (!out) continue;
-                const int *cs = cc + sp * 3 * nc;
-                double val;
-                if (kind == GS_SCORE_DEFAULT) {
-                    int64_t ok = 0, tot = 0;
-                    for (int q = 0; q < nc; q++) { tot += cs[q * 3]; ok += cs[q * 3 + 1]; }
-                    val = tot > 0 ? (double)ok / (double)tot : NAN;
-                } else if (kind == GS_SCORE_ROC_AUC) {
-                    double na = 0, nb = 0;
-                    for (int r = 0; r < n; r++) {
-                        const bool in = sp == 0 ? h->is_test(r, k) : (!h->is_test(r, k) && h->is_train(r, k));
-                        if (in) (r >= h->class_start[1] ? nb : na) += 1;
-                    }
-                    const unsigned long long *a = &araw[(size_t)f * 4 + sp * 2];
-                    val = na * nb > 0 ? ((double)a[0] + 0.5 * (double)a[1]) / (na * nb) : NAN;
-                } else {
-                    val = gs_score_from_counts(kind, h->score_pos, nc, cs);
-                }
-                out[f] = val;
-            }
-            if (n_iter) {
-                int it = 0;
-                for (int q = 0; q < KC; q++) it = std::max(it, fin[(size_t)f * KC + q].n_iter);
-                n_iter[f] = it;
-            }
+        launches++;
+        if (int e = score_linear_fits(h, tr.V, dXa, dZ, nfit, KC, ns, h->score_kind, test_scores, train_scores, ev[2], launches)) return e;
+        for (int f = 0; f < nfit && n_iter; f++) {
+            int it = 0;
+            for (int q = 0; q < KC; q++) it = std::max(it, fin[(size_t)f * KC + q].n_iter);
+            n_iter[f] = it;
         }
     } else {
         std::vector<double> x((size_t)KC * NVEC * nvp);
-        GS_CUDA(cudaMemcpyAsync(x.data(), dVec, x.size() * 8, cudaMemcpyDeviceToHost, st));
+        GS_CUDA(cudaMemcpyAsync(x.data(), tr.Vec, x.size() * 8, cudaMemcpyDeviceToHost, st));
         cudaEventRecord(ev[2], st);
         GS_CUDA(cudaStreamSynchronize(st));
         for (int q = 0; q < KC; q++) {
@@ -476,23 +377,15 @@ int linsvc_run(gs_handle *h, int n_cand, const double *Cv, double tol, int max_i
             if (n_iter) n_iter[q] = fin[q].n_iter;
         }
     }
-    cudaEventElapsedTime(ms_solve, ev[0], ev[1]);
-    cudaEventElapsedTime(ms_score, ev[1], ev[2]);
-    gs_profile &pf = h->prof;
-    const float keep_h2d = pf.ms_h2d; const int64_t keep_b = pf.h2d_bytes;
-    memset(&pf, 0, sizeof pf);
-    pf.ms_h2d = keep_h2d; pf.h2d_bytes = keep_b;
-    pf.ms_total = *ms_solve + *ms_score; pf.ms_solve = *ms_solve; pf.ms_score = *ms_score;
-    pf.launches = launches;
-    pf.smo_iterations = rounds;                                 // TRON rounds: one fun() or Hv() per open column each
-    pf.d2h_bytes = (int64_t)ncol * sizeof(TrState);
-    pf.ms_tensor = h->tt.collect(); pf.tensor_flops = h->tt.flops;
+    linear_profile(h, ev, launches, ms_solve, ms_score);
+    h->prof.smo_iterations = tr.rounds;                         // TRON rounds: one fun() or Hv() per open column each
+    h->prof.d2h_bytes = (int64_t)ncol * sizeof(TrState);
     return GS_OK;
 }
 
 }  // namespace
 
-// ---- the pieces linsvr.cu (LinearSVR's primal solver, L2R_L2LOSS_SVR) and sgd.cu (the classification scorers) share ----
+// ---- the pieces linear_search.cu (TronRounds, the classification scorers), linsvr.cu, sgd.cu and sag.cu (Xa) share ----
 cudaError_t launch_tron_advance(TrState *St, double *Vec, double *V, const double *Gp, int nchunk, int64_t gp_stride,
                                 const double *fpart, int ncol, int nvp, int max_iter, int *n_open, cudaStream_t st)
 {
@@ -526,11 +419,7 @@ int gs_linsvc(gs_handle *h, int32_t n_cand, const double *C, double tol, int32_t
     const int st = linsvc_run(h, n_cand, C, tol, max_iter, fit_intercept, intercept_scaling, false, test_scores,
                               (flags & GS_RETURN_TRAIN) ? train_scores : nullptr, n_iter, nullptr, &a, &b);
     if (st) return st;
-    const int nt = n_cand * h->n_splits;
-    for (int i = 0; i < nt; i++) {
-        if (fit_ms) fit_ms[i] = a / (float)nt;
-        if (score_ms) score_ms[i] = b / (float)nt;
-    }
+    spread_call_ms(n_cand * h->n_splits, a, b, fit_ms, score_ms);
     return GS_OK;
 }
 

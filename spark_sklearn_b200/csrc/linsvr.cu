@@ -11,7 +11,7 @@
 //                                              std::mt19937), shrinking against Gmax_old, the |d| < 1e-12 skip, the clip,
 //                                              and the stop Gnorm1 <= eps Gnorm1_init that unshrinks while the set is not full
 //   linear.cpp l2r_l2_svr_fun + tron.cpp        solver 11: linsvr_pointwise_kernel between the two contractions, TRON itself
-//                                              is linsvc.cu's tron_advance_kernel
+//                                              is linsvc.cu's tron_advance_kernel, its rounds linear_search.cu's TronRounds
 //
 // A CD fit is one warp.  w lives in registers (lane L holds features L, L + 32, ...; the bias is feature d), beta and the
 // index permutation live in HBM (beta by internal row, the permutation as internal rows), the mt19937 state in shared memory.
@@ -19,6 +19,7 @@
 // the same on all lanes, so the update, the shrink decision and the stores need no broadcast.  Scalar arithmetic is rounded
 // operation by operation as liblinear's (no contraction); only the dot product's summation order differs from liblinear,
 // which accumulates the row into G in feature order (tests/linsvr_oracle.c restates both orders).
+// The training order and the scoring of the final weights are linear_search.cu's (train_rows, score_linear_fits).
 #include "common.cuh"
 #include <algorithm>
 #include <cmath>
@@ -371,8 +372,6 @@ __global__ void linsvr_scatter_w_kernel(const double *__restrict__ Vec, const in
     for (int j = threadIdx.x; j < nvp; j += blockDim.x) V[(size_t)out[c] * nvp + j] = Vec[(size_t)c * NVEC * nvp + j];
 }
 
-int64_t round_up(int64_t x, int64_t m) { return (x + m - 1) / m * m; }
-
 template <int NT, bool L1, typename TX>
 cudaError_t launch_cd_t(const CdFit *fits, int nfits, const TX *X, int d, double bias, const int *order, const double *QD,
                         const double *y, const double *W, double *beta, int *index, int64_t idx_stride, int n, double eps,
@@ -412,7 +411,7 @@ int linsvr_run(gs_handle *h, int n_cand, const double *Cv, const double *epsv, c
     if (h->d > GS_LINSVR_MAX_FEATURES)
         return fail(GS_ERR_UNSUPPORTED, "more than " + std::to_string(GS_LINSVR_MAX_FEATURES) + " features");
     const int kind = refit ? GS_SCORE_DEFAULT : h->score_kind;
-    if (kind != GS_SCORE_DEFAULT && kind != GS_SCORE_NEG_MSE && kind != GS_SCORE_NEG_RMSE) return fail(GS_ERR_ARG, "classification scorer on a regressor");
+    if (int e = check_scorer(h, who, kind, 1)) return e;
     const int ns = refit ? 1 : h->n_splits, nfit = n_cand * ns;
     for (int c = 0; c < n_cand; c++) {
         if (!(Cv[c] > 0) || !std::isfinite(Cv[c])) return fail(GS_ERR_ARG, "C must be > 0 and finite");
@@ -430,25 +429,9 @@ int linsvr_run(gs_handle *h, int n_cand, const double *Cv, const double *epsv, c
     const bool has_sw = !h->sample_w.empty();
 
     // ---- every split's training rows in fit order (internal rows), zero-weight rows dropped in order ----
-    std::vector<int> by_orig(n);
-    for (int r = 0; r < n; r++) by_orig[h->perm[r]] = r;
-    std::vector<int> order;
-    std::vector<int> sp_off(ns + 1, 0);
-    int lmax = 0;
-    for (int k = 0; k < ns; k++) {
-        sp_off[k] = (int)order.size();
-        auto take = [&](int o) {
-            const int r = by_orig[o];
-            if (!has_sw || h->sample_w64[r] > 0) order.push_back(r);
-        };
-        if (refit) for (int o = 0; o < n; o++) take(o);
-        else if (!h->train_off.empty()) for (int64_t e = h->train_off[k]; e < h->train_off[k + 1]; e++) take(h->train_order[e]);
-        else for (int o = 0; o < n; o++) if (h->is_train(by_orig[o], k)) take(o);
-        const int l = (int)order.size() - sp_off[k];
-        if (l == 0) return fail(GS_ERR_UNSUPPORTED, "a split has no training row of positive weight");
-        lmax = std::max(lmax, l);
-    }
-    sp_off[ns] = (int)order.size();
+    std::vector<int> order, sp_off;
+    const int lmax = train_rows(h, ns, refit, true, order, sp_off);
+    if (lmax == 0) return fail(GS_ERR_UNSUPPORTED, "a split has no training row of positive weight");
 
     std::vector<CdFit> cd[2];                                  // [0] solver 12, [1] solver 13
     std::vector<int> tron_fit;
@@ -459,8 +442,7 @@ int linsvr_run(gs_handle *h, int n_cand, const double *Cv, const double *epsv, c
             cd[solver[t] == 13].push_back(CdFit{sp_off[k], sp_off[k + 1] - sp_off[k], t, seed[t], Cv[c], epsv[c]});
         }
     const int ncd = (int)(cd[0].size() + cd[1].size()), ntr = (int)tron_fit.size();
-    const int mpad_all = (int)round_up(nfit, 64), mpad_t = (int)round_up(std::max(ntr, 1), 64);
-    const int KCH = 2048, nchunk = (int)((npad + KCH - 1) / KCH);
+    const int mpad_all = (int)round_up(nfit, 64), mpad_t = (int)round_up(ntr, 64);
 
     h->evp.reset(); h->tt.reset();
     cudaEvent_t ev[3];
@@ -468,22 +450,18 @@ int linsvr_run(gs_handle *h, int n_cand, const double *Cv, const double *epsv, c
     cudaEventRecord(ev[0], st);
 
     // ---- buffers ----
-    DevBuf &bXa = h->dWork[0], &bZ = h->dWork[1], &bR = h->dWork[2], &bG = h->dWork[3], &bVt = h->dWork[4], &bS = h->dWork[5],
-           &bM = h->dWork[6], &bCd = h->dWork[7], &bOut = h->dWork[8];
+    DevBuf &bXa = h->dWork[0], &bZ = h->dWork[1], &bCd = h->dWork[7], &bOut = h->dWork[8];
     const size_t xa_elems = (size_t)npad * nvp;
     GS_CUDA(bXa.reserve((xa_elems * 2 + (size_t)n * 2) * 8));
     double *dXa = bXa.as<double>(), *dXat = dXa + xa_elems, *dW = dXat + xa_elems, *dQD = dW + n;
-    GS_CUDA(bZ.reserve((size_t)std::max(mpad_all, ntr ? mpad_t : 0) * npad * 8));
+    GS_CUDA(bZ.reserve((size_t)std::max(mpad_all, mpad_t) * npad * 8));
     double *dZ = bZ.as<double>();
-    const size_t out_bytes = ((size_t)mpad_all * nvp + (size_t)nfit * n + (size_t)nfit * 3) * 8 + (size_t)nfit * (4 + sizeof(VoteTask)) +
-                             (size_t)nfit * 3 * 8 + 256;
-    GS_CUDA(bOut.reserve(out_bytes));
-    double *dV = bOut.as<double>(), *dZc = dV + (size_t)mpad_all * nvp, *dRho = dZc + (size_t)nfit * n, *dRss = dRho + nfit;
-    int *dIter = reinterpret_cast<int *>(dRss + (size_t)nfit * 2);
-    VoteTask *dVt = reinterpret_cast<VoteTask *>(dIter + round_up(nfit, 4));
-    long long *dStats = reinterpret_cast<long long *>(dVt + nfit);
+    GS_CUDA(bOut.reserve(((size_t)mpad_all * nvp + (size_t)nfit * 3) * 8 + (size_t)ntr * sizeof(SvrCol) + (size_t)(nfit + ntr) * 4));
+    double *dV = bOut.as<double>();
+    long long *dStats = reinterpret_cast<long long *>(dV + (size_t)mpad_all * nvp);
+    SvrCol *dCols = reinterpret_cast<SvrCol *>(dStats + (size_t)nfit * 3);
+    int *dIter = reinterpret_cast<int *>(dCols + ntr), *dOutRow = dIter + nfit;
     GS_CUDA(cudaMemsetAsync(dV, 0, (size_t)mpad_all * nvp * 8, st));
-    GS_CUDA(cudaMemsetAsync(dRho, 0, (size_t)nfit * 8, st));
     GS_CUDA(cudaMemsetAsync(dStats, 0, (size_t)nfit * 3 * 8, st));
     {
         std::vector<double> W64(n, 1.0);
@@ -531,19 +509,9 @@ int linsvr_run(gs_handle *h, int n_cand, const double *Cv, const double *epsv, c
     }
 
     // ---- the TRON fits (solver 11): linsvc.cu's rounds with the SVR element-wise pass ----
-    int rounds = 0;
+    TronRounds tr;
     if (ntr > 0) {
-        GS_CUDA(bR.reserve((size_t)mpad_t * npad * 8));
-        GS_CUDA(bG.reserve((size_t)nchunk * mpad_t * nvp * 8));
-        GS_CUDA(bVt.reserve(((size_t)mpad_t * nvp + (size_t)ntr * NVEC * nvp) * 8));
-        GS_CUDA(bS.reserve((size_t)ntr * (sizeof(TrState) + sizeof(SvrCol) + 4) + (size_t)ntr * PW_BLOCKS * 8 + 256));
-        GS_CUDA(bM.reserve((size_t)2 * ntr * npad));
-        double *dR = bR.as<double>(), *dGp = bG.as<double>(), *dVtr = bVt.as<double>(), *dVec = dVtr + (size_t)mpad_t * nvp;
-        TrState *dS = bS.as<TrState>();
-        double *dF = reinterpret_cast<double *>(dS + ntr);
-        SvrCol *dCols = reinterpret_cast<SvrCol *>(dF + (size_t)ntr * PW_BLOCKS);
-        int *dOutRow = reinterpret_cast<int *>(dCols + ntr);
-        unsigned char *dMask = bM.as<unsigned char>();
+        if (int e = tr.reserve(h, ntr)) return e;
         std::vector<TrState> hs(ntr);
         std::vector<SvrCol> hc(ntr);
         for (int q = 0; q < ntr; q++) {
@@ -554,37 +522,21 @@ int linsvr_run(gs_handle *h, int n_cand, const double *Cv, const double *epsv, c
             S.eps = tol;                                            // train_one, L2R_L2LOSS_SVR: TRON(eps) unscaled
             hc[q] = SvrCol{refit ? -100 : k, Cv[c], epsv[c]};
         }
-        GS_CUDA(cudaMemcpyAsync(dS, hs.data(), (size_t)ntr * sizeof(TrState), cudaMemcpyHostToDevice, st));
+        GS_CUDA(cudaMemcpyAsync(tr.St, hs.data(), (size_t)ntr * sizeof(TrState), cudaMemcpyHostToDevice, st));
         GS_CUDA(cudaMemcpyAsync(dCols, hc.data(), (size_t)ntr * sizeof(SvrCol), cudaMemcpyHostToDevice, st));
         GS_CUDA(cudaMemcpyAsync(dOutRow, tron_fit.data(), (size_t)ntr * 4, cudaMemcpyHostToDevice, st));
-        GS_CUDA(cudaMemsetAsync(dVtr, 0, ((size_t)mpad_t * nvp + (size_t)ntr * NVEC * nvp) * 8, st));
-        GS_CUDA(cudaMemsetAsync(dMask, 0, (size_t)2 * ntr * npad, st));
-        GS_CUDA(cudaMemsetAsync(dR, 0, (size_t)mpad_t * npad * 8, st));
-        int *dOpenCnt = reinterpret_cast<int *>(dStats + (size_t)nfit * 3);
-        const double flops = 2.0 * mpad_t * (double)npad * nvp;
-        int open = 1;
-        while (open > 0) {
-            if (++rounds > 1000000) return fail(GS_ERR_NUMERIC, "TRON did not terminate");
-            h->tt.begin(h->evp, st);
-            GS_CUDA(launch_gemm_nt_f64(dVtr, nvp, dXa, nvp, dZ, npad, mpad_t, (int)npad, nvp, nvp, 0, st));
-            h->tt.end(h->evp, st, flops);
-            linsvr_pointwise_kernel<<<dim3(PW_BLOCKS, ntr), 256, 0, st>>>(dZ, npad, n, h->dZ64.as<double>(), h->masks(), dW, dS, dCols,
-                                                                          dMask, (int64_t)ntr * npad, dR, dF);
-            GS_CUDA(cudaGetLastError());
-            h->tt.begin(h->evp, st);
-            GS_CUDA(launch_gemm_nt_f64(dR, npad, dXat, npad, dGp, nvp, mpad_t, nvp, (int)npad, KCH, (int64_t)mpad_t * nvp, st));
-            h->tt.end(h->evp, st, flops);
-            GS_CUDA(cudaMemsetAsync(dOpenCnt, 0, 4, st));
-            GS_CUDA(launch_tron_advance(dS, dVec, dVtr, dGp, nchunk, (int64_t)mpad_t * nvp, dF, ntr, nvp, max_iter, dOpenCnt, st));
-            GS_CUDA(cudaMemcpyAsync(&open, dOpenCnt, 4, cudaMemcpyDeviceToHost, st));
-            GS_CUDA(cudaStreamSynchronize(st));
-            launches += 4;
-        }
-        linsvr_scatter_w_kernel<<<ntr, 128, 0, st>>>(dVec, dOutRow, ntr, nvp, dV);
+        const double *Y = h->dZ64.as<double>();
+        auto pointwise = [&]() {
+            linsvr_pointwise_kernel<<<dim3(PW_BLOCKS, ntr), 256, 0, st>>>(dZ, npad, n, Y, h->masks(), dW, tr.St, dCols, tr.mask,
+                                                                          (int64_t)ntr * npad, tr.R, tr.F);
+            return cudaGetLastError();
+        };
+        if (int e = tr.run(h, who, dXa, dXat, dZ, max_iter, pointwise, launches)) return e;
+        linsvr_scatter_w_kernel<<<ntr, 128, 0, st>>>(tr.Vec, dOutRow, ntr, nvp, dV);
         GS_CUDA(cudaGetLastError());
         launches++;
         std::vector<TrState> fin(ntr);
-        GS_CUDA(cudaMemcpyAsync(fin.data(), dS, (size_t)ntr * sizeof(TrState), cudaMemcpyDeviceToHost, st));
+        GS_CUDA(cudaMemcpyAsync(fin.data(), tr.St, (size_t)ntr * sizeof(TrState), cudaMemcpyDeviceToHost, st));
         GS_CUDA(cudaStreamSynchronize(st));
         for (int q = 0; q < ntr; q++) iters[tron_fit[q]] = fin[q].n_iter;
     }
@@ -604,32 +556,13 @@ int linsvr_run(gs_handle *h, int n_cand, const double *Cv, const double *epsv, c
     }
 
     // ---- scoring: z = Xa w for every fit in one forward contraction, then the residual sums of squares ----
-    std::vector<double> rss((size_t)nfit * 2, 0.0);
     if (!refit) {
-        h->tt.begin(h->evp, st);
-        GS_CUDA(launch_gemm_nt_f64(dV, nvp, dXa, nvp, dZ, npad, mpad_all, (int)npad, nvp, nvp, 0, st));
-        h->tt.end(h->evp, st, 2.0 * mpad_all * (double)npad * nvp);
-        GS_CUDA(cudaMemcpy2DAsync(dZc, (size_t)n * 8, dZ, (size_t)npad * 8, (size_t)n * 8, nfit, cudaMemcpyDeviceToDevice, st));
-        std::vector<VoteTask> vt(nfit);
-        for (int t = 0; t < nfit; t++) vt[t] = VoteTask{t, t % ns};
-        GS_CUDA(cudaMemcpyAsync(dVt, vt.data(), (size_t)nfit * sizeof(VoteTask), cudaMemcpyHostToDevice, st));
-        GS_CUDA(launch_rss(dZc, dRho, n, h->dZ64.as<double>(), h->masks(), dVt, nfit, dRss, st));
-        GS_CUDA(cudaMemcpyAsync(rss.data(), dRss, rss.size() * 8, cudaMemcpyDeviceToHost, st));
-        launches += 3;
+        if (int e = score_linear_fits(h, dV, dXa, dZ, nfit, 1, ns, kind, test_scores, train_scores, ev[2], launches)) return e;
+    } else {
+        cudaEventRecord(ev[2], st);
+        GS_CUDA(cudaStreamSynchronize(st));
     }
-    cudaEventRecord(ev[2], st);
-    GS_CUDA(cudaStreamSynchronize(st));
     for (const auto &v : cd) for (const CdFit &F : v) iters[F.out] = cd_iter[F.out];
-
-    if (!refit) {
-        std::vector<double> tss, cnt;
-        regression_split_stats(h, ns, tss, cnt);
-        for (int t = 0; t < nfit; t++) {
-            const int k = t % ns;
-            test_scores[t] = regression_score(kind, rss[(size_t)t * 2], tss[(size_t)k * 2], cnt[(size_t)k * 2]);
-            if (train_scores) train_scores[t] = regression_score(kind, rss[(size_t)t * 2 + 1], tss[(size_t)k * 2 + 1], cnt[(size_t)k * 2 + 1]);
-        }
-    }
     for (int t = 0; t < nfit; t++) {
         if (n_iter) n_iter[t] = iters[t];
         if (coef_out) {
@@ -637,58 +570,16 @@ int linsvr_run(gs_handle *h, int n_cand, const double *Cv, const double *epsv, c
         }
         if (cd_stats) for (int e = 0; e < 3; e++) cd_stats[(size_t)t * 3 + e] = stats[(size_t)t * 3 + e];
     }
-    cudaEventElapsedTime(ms_solve, ev[0], ev[1]);
-    cudaEventElapsedTime(ms_score, ev[1], ev[2]);
-    gs_profile &pf = h->prof;
-    const float keep_h2d = pf.ms_h2d; const int64_t keep_b = pf.h2d_bytes;
-    memset(&pf, 0, sizeof pf);
-    pf.ms_h2d = keep_h2d; pf.h2d_bytes = keep_b;
-    pf.ms_total = *ms_solve + *ms_score; pf.ms_solve = *ms_solve; pf.ms_score = *ms_score;
-    pf.launches = launches;
+    linear_profile(h, ev, launches, ms_solve, ms_score);
     int64_t total_steps = 0;
     for (int t = 0; t < nfit; t++) total_steps += stats[(size_t)t * 3];
-    pf.smo_iterations = total_steps + rounds;                   // CD coordinate steps plus TRON rounds
-    pf.ms_tensor = h->tt.collect(); pf.tensor_flops = h->tt.flops;
+    h->prof.smo_iterations = total_steps + tr.rounds;          // CD coordinate steps plus TRON rounds
     return GS_OK;
 }
 
 }  // namespace
 
 extern "C" {
-
-int gs_set_train_order(gs_handle *h, const int32_t *rows, const int64_t *offsets, int32_t n_splits)
-{
-    if (!h) return GS_ERR_ARG;
-    if (h->n == 0) { gs_set_error(h, "gs_set_train_order: no dataset (call gs_set_data first)"); return GS_ERR_NO_DATA; }
-    if (!rows || !offsets) { h->train_order.clear(); h->train_off.clear(); return GS_OK; }
-    if (n_splits != h->n_splits) { gs_set_error(h, "gs_set_train_order: n_splits differs from the dataset's splits"); return GS_ERR_ARG; }
-    const int n = (int)h->n;
-    std::vector<int> by_orig(n);
-    for (int r = 0; r < n; r++) by_orig[h->perm[r]] = r;
-    if (offsets[0] != 0) { gs_set_error(h, "gs_set_train_order: offsets[0] must be 0"); return GS_ERR_ARG; }
-    std::vector<char> seen(n);
-    for (int k = 0; k < n_splits; k++) {
-        if (offsets[k + 1] < offsets[k]) { gs_set_error(h, "gs_set_train_order: offsets must not decrease"); return GS_ERR_ARG; }
-        std::fill(seen.begin(), seen.end(), 0);
-        int64_t want = 0;
-        for (int r = 0; r < n; r++) want += h->is_train(r, k);
-        if (offsets[k + 1] - offsets[k] != want) {
-            gs_set_error(h, "gs_set_train_order: split " + std::to_string(k) + " lists a different number of rows than its training set");
-            return GS_ERR_ARG;
-        }
-        for (int64_t e = offsets[k]; e < offsets[k + 1]; e++) {
-            const int o = rows[e];
-            if (o < 0 || o >= n || seen[o] || !h->is_train(by_orig[o], k)) {
-                gs_set_error(h, "gs_set_train_order: split " + std::to_string(k) + " lists a row twice or a row outside its training set");
-                return GS_ERR_ARG;
-            }
-            seen[o] = 1;
-        }
-    }
-    h->train_order.assign(rows, rows + offsets[n_splits]);
-    h->train_off.assign(offsets, offsets + n_splits + 1);
-    return GS_OK;
-}
 
 int gs_linsvr(gs_handle *h, int32_t n_cand, const double *C, const double *epsilon, const int32_t *solver, const uint32_t *seed,
               double tol, int32_t max_iter, int32_t fit_intercept, double intercept_scaling, uint32_t flags, double *test_scores,
@@ -699,11 +590,7 @@ int gs_linsvr(gs_handle *h, int32_t n_cand, const double *C, const double *epsil
     const int st = linsvr_run(h, n_cand, C, epsilon, solver, seed, tol, max_iter, fit_intercept, intercept_scaling, false, test_scores,
                               (flags & GS_RETURN_TRAIN) ? train_scores : nullptr, n_iter, coef_out, cd_stats, &a, &b);
     if (st) return st;
-    const int nt = n_cand * h->n_splits;
-    for (int i = 0; i < nt; i++) {
-        if (fit_ms) fit_ms[i] = a / (float)nt;
-        if (score_ms) score_ms[i] = b / (float)nt;
-    }
+    spread_call_ms(n_cand * h->n_splits, a, b, fit_ms, score_ms);
     return GS_OK;
 }
 

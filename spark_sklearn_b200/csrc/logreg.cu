@@ -602,10 +602,8 @@ int logreg_run(gs_handle *h, int n_cand, const double *Cv, double tol, int max_i
                 ntrain[k] += wi; ntrain_c[(size_t)k * nc + h->yc[i]] += wi;
             }
     const float *dSw = has_sw ? h->dSw.as<float>() : nullptr;
+    if (int e = check_class_weight_sets(h, "gs_logreg", ns)) return e;
     const bool weighted = h->class_w_sets > 0;
-    if (weighted && h->class_w_sets != 1 && h->class_w_sets != ns) {
-        gs_set_error(h, "gs_logreg: gs_set_class_weight was given a weight set per split, but not for this number of splits"); return GS_ERR_ARG;
-    }
     std::vector<float> cwcol((size_t)nfit * CWS, 1.f);
     std::vector<LbScalars> hs(nfit);
     std::vector<double> inv(nfit);
@@ -700,10 +698,7 @@ int logreg_run(gs_handle *h, int n_cand, const double *Cv, double tol, int max_i
         GS_CUDA(cudaMemsetAsync(dCounts, 0, (size_t)nfit * 16, st));
         dim3 grid(64, nfit);
         const int kind = h->score_kind;
-        if (kind == GS_SCORE_NEG_MSE || kind == GS_SCORE_NEG_RMSE) { gs_set_error(h, "gs_logreg: regression scorer on a classifier"); return GS_ERR_ARG; }
-        if (multi && (kind == GS_SCORE_ROC_AUC || kind == GS_SCORE_F1 || kind == GS_SCORE_PRECISION || kind == GS_SCORE_RECALL)) {
-            gs_set_error(h, "gs_logreg: this scorer is defined for binary problems only"); return GS_ERR_UNSUPPORTED;
-        }
+        if (int e = check_scorer(h, "gs_logreg", kind, KC)) return e;
         // non-default scorers (gs_set_scoring): class counts or ROC-AUC pair counts from the z values already in HBM
         std::vector<int> ccounts;
         std::vector<unsigned long long> araw;
@@ -786,18 +781,11 @@ int logreg_run(gs_handle *h, int n_cand, const double *Cv, double tol, int max_i
     }
     for (int col = 0; col < nfit; col++)
         if (fin[col].task != T_DONE) { gs_set_error(h, "gs_logreg: optimiser did not terminate"); return GS_ERR_NUMERIC; }
-    cudaEventElapsedTime(ms_solve, ev[0], ev[1]);
-    cudaEventElapsedTime(ms_score, ev[1], ev[2]);
+    linear_profile(h, ev, launches, ms_solve, ms_score);
     gs_profile &pf = h->prof;
-    const float keep_h2d = pf.ms_h2d; const int64_t keep_b = pf.h2d_bytes;
-    memset(&pf, 0, sizeof pf);
-    pf.ms_h2d = keep_h2d; pf.h2d_bytes = keep_b;
-    pf.ms_total = *ms_solve + *ms_score; pf.ms_solve = *ms_solve; pf.ms_score = *ms_score;
-    pf.launches = launches;
     pf.smo_iterations = rounds;                                 // function-evaluation rounds
     pf.gram_flops = (double)rounds * 2.0 * 2.0 * (double)n * nv * ncol;
     pf.d2h_bytes = (int64_t)nfit * (16 + sizeof(LbScalars));
-    pf.ms_tensor = h->tt.collect(); pf.tensor_flops = h->tt.flops;
     return GS_OK;
 }
 
@@ -813,11 +801,7 @@ int gs_logreg(gs_handle *h, int32_t n_cand, const double *C, double tol, int32_t
     const int st = logreg_run(h, n_cand, C, tol, max_iter, fit_intercept, false, test_scores,
                               (flags & GS_RETURN_TRAIN) ? train_scores : nullptr, n_iter, nullptr, &a, &b);
     if (st) return st;
-    const int nt = n_cand * h->n_splits;
-    for (int i = 0; i < nt; i++) {
-        if (fit_ms) fit_ms[i] = a / (float)nt;
-        if (score_ms) score_ms[i] = b / (float)nt;
-    }
+    spread_call_ms(n_cand * h->n_splits, a, b, fit_ms, score_ms);
     return GS_OK;
 }
 

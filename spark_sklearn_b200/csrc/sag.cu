@@ -22,6 +22,7 @@
 // sequence), every operation is rounded on its own (no contraction), and float32 X runs sag32: every value scikit-learn
 // keeps in float -- the weights, wscale, the cumulative sums, the gradients -- is rounded to float where its C expression
 // is, while the step size and the penalties stay double.  Only exp (the logistic gradients) comes from CUDA's math library.
+// The training order and the scoring of the final weights are linear_search.cu's (train_rows, score_linear_fits).
 #include "common.cuh"
 #include "sequential.cuh"
 #include <algorithm>
@@ -311,8 +312,6 @@ __global__ void sag_draws_kernel(uint32_t seed, int n, int count, int *out)
     for (int i = 0; i < count; i++) out[i] = (int)(our_rand_r(seed) % (uint32_t)n);
 }
 
-int64_t round_up(int64_t x, int64_t m) { return (x + m - 1) / m * m; }
-
 size_t sag_smem(int dk, int K) { return (size_t)SAG_WARPS * (((dk + 1) & ~1) + 3 * ((K + 1) & ~1)) * sizeof(double); }
 
 template <int S, typename T>
@@ -377,12 +376,9 @@ int sag_run(gs_handle *h, int n_cand, const int32_t *solver, const double *alpha
     const int n = (int)h->n, d = (int)h->d, dk = d * K;
     if (dk > GS_SAG_MAX_COEF) return fail(GS_ERR_UNSUPPORTED, "features x weight rows above GS_SAG_MAX_COEF (" + std::to_string(GS_SAG_MAX_COEF) + ")");
     const int kind = refit || !cls ? GS_SCORE_DEFAULT : h->score_kind;
-    if (cls && (kind == GS_SCORE_NEG_MSE || kind == GS_SCORE_NEG_RMSE)) return fail(GS_ERR_ARG, "regression scorer on a classifier");
-    if (cls && K > 1 && (kind == GS_SCORE_ROC_AUC || kind == GS_SCORE_F1 || kind == GS_SCORE_PRECISION || kind == GS_SCORE_RECALL))
-        return fail(GS_ERR_UNSUPPORTED, "this scorer is defined for binary problems only");
+    if (int e = check_scorer(h, who, kind, K)) return e;
+    if (int e = check_class_weight_sets(h, who, ns)) return e;
     const bool weighted = cls && h->class_w_sets > 0;
-    if (weighted && h->class_w_sets != 1 && h->class_w_sets != ns)
-        return fail(GS_ERR_ARG, "gs_set_class_weight was given a weight set per split, but not for this number of splits");
     GS_CUDA(cudaSetDevice(h->device));
     cudaStream_t st = h->stream;
     const int S = std::max(1, (dk + 31) / 32);
@@ -393,20 +389,9 @@ int sag_run(gs_handle *h, int n_cand, const int32_t *solver, const double *alpha
     const int tsize = f64 ? 8 : 4;
 
     // ---- every split's training rows in the splitter's order (internal rows); zero-weight rows stay (they count in n) ----
-    std::vector<int> by_orig(n);
-    for (int r = 0; r < n; r++) by_orig[h->perm[r]] = r;
-    std::vector<int> order, sp_off(ns + 1, 0);
-    int lmax = 0;
-    for (int k = 0; k < ns; k++) {
-        sp_off[k] = (int)order.size();
-        if (refit) for (int o = 0; o < n; o++) order.push_back(by_orig[o]);
-        else if (!h->train_off.empty()) for (int64_t e = h->train_off[k]; e < h->train_off[k + 1]; e++) order.push_back(by_orig[h->train_order[e]]);
-        else for (int o = 0; o < n; o++) if (h->is_train(by_orig[o], k)) order.push_back(by_orig[o]);
-        const int l = (int)order.size() - sp_off[k];
-        if (l == 0) return fail(GS_ERR_UNSUPPORTED, "a split has no training row");
-        lmax = std::max(lmax, l);
-    }
-    sp_off[ns] = (int)order.size();
+    std::vector<int> order, sp_off;
+    const int lmax = train_rows(h, ns, refit, false, order, sp_off);
+    if (lmax == 0) return fail(GS_ERR_UNSUPPORTED, "a split has no training row");
 
     const int nfit = n_cand * ns;
     std::vector<SagFit> hf(nfit);
@@ -426,7 +411,7 @@ int sag_run(gs_handle *h, int n_cand, const int32_t *solver, const double *alpha
     for (auto &e : ev) e = h->evp.get();
     cudaEventRecord(ev[0], st);
 
-    DevBuf &bXa = h->dWork[0], &bZ = h->dWork[1], &bFit = h->dWork[2], &bScr = h->dWork[3], &bOut = h->dWork[4], &bMeta = h->dWork[5];
+    DevBuf &bXa = h->dWork[0], &bZ = h->dWork[1], &bFit = h->dWork[2], &bScr = h->dWork[3], &bOut = h->dWork[4];
     const size_t xa_elems = (size_t)npad * nvp;
     GS_CUDA(bXa.reserve((xa_elems * 2 + (size_t)n + (size_t)std::max(1, h->class_w_sets) * nc) * 8));
     double *dXa = bXa.as<double>(), *dXat = dXa + xa_elems, *dSw = dXat + xa_elems, *dCw = dSw + n;
@@ -478,74 +463,19 @@ int sag_run(gs_handle *h, int n_cand, const int32_t *solver, const double *alpha
     }
 
     // ---- scoring: decision values [X | 1] . [coef | intercept] of every fit in one FP64 contraction ----
-    std::vector<int> ccounts;
-    std::vector<unsigned long long> araw;
-    const int per_fit = 6 * nc;
     const bool score = !refit && cls;
     if (score) {
         GS_CUDA(launch_build_xa64(f64 ? nullptr : X32, X64, n, d, 1.0, nvp, npad, dXa, dXat, st));
-        GS_CUDA(bZ.reserve((size_t)mpad * npad * 8));
-        double *dZ = bZ.as<double>();
-        h->tt.begin(h->evp, st);
-        GS_CUDA(launch_gemm_nt_f64(dV, nvp, dXa, nvp, dZ, npad, mpad, (int)npad, nvp, nvp, 0, st));
-        h->tt.end(h->evp, st, 2.0 * mpad * (double)npad * nvp);
-        launches += 2;
-        GS_CUDA(bMeta.reserve((size_t)nfit * 4 * 2 + (size_t)nfit * per_fit * 4 + 256));
-        int *dFoldOf = bMeta.as<int>(), *dCnt = dFoldOf + round_up(nfit, 4);
-        std::vector<int> foldof(nfit);
-        for (int f = 0; f < nfit; f++) foldof[f] = f % ns;
-        GS_CUDA(cudaMemcpyAsync(dFoldOf, foldof.data(), (size_t)nfit * 4, cudaMemcpyHostToDevice, st));
-        GS_CUDA(cudaMemsetAsync(dCnt, 0, (size_t)nfit * per_fit * 4, st));
-        GS_CUDA(launch_linsvc_count(dZ, npad, n, nc, K, Yc, h->masks(), dFoldOf, nfit, dCnt, st));
-        ccounts.resize((size_t)nfit * per_fit);
-        GS_CUDA(cudaMemcpyAsync(ccounts.data(), dCnt, ccounts.size() * 4, cudaMemcpyDeviceToHost, st));
         launches++;
-        if (kind == GS_SCORE_ROC_AUC) {
-            std::vector<int> meta((size_t)nfit * 2);
-            for (int f = 0; f < nfit; f++) { meta[f] = f; meta[nfit + f] = f % ns; }
-            GS_CUDA(h->dScore.reserve((size_t)nfit * 40));
-            unsigned long long *d_auc = h->dScore.as<unsigned long long>();
-            int *d_meta = (int *)(d_auc + (size_t)nfit * 4);
-            GS_CUDA(cudaMemcpyAsync(d_meta, meta.data(), meta.size() * 4, cudaMemcpyHostToDevice, st));
-            GS_CUDA(cudaMemsetAsync(d_auc, 0, (size_t)nfit * 32, st));
-            GS_CUDA(launch_auc_pairs_f64(dZ, npad, n, h->class_start[1], h->masks(), d_meta, d_meta + nfit, nfit, +1, d_auc, st));
-            araw.resize((size_t)nfit * 4);
-            GS_CUDA(cudaMemcpyAsync(araw.data(), d_auc, (size_t)nfit * 32, cudaMemcpyDeviceToHost, st));
-            launches++;
-        }
+        GS_CUDA(bZ.reserve((size_t)mpad * npad * 8));
+        if (int e = score_linear_fits(h, dV, dXa, bZ.as<double>(), nfit, K, ns, kind, test_scores, train_scores, ev[2], launches)) return e;
+    } else {
+        cudaEventRecord(ev[2], st);
+        GS_CUDA(cudaStreamSynchronize(st));
     }
-    cudaEventRecord(ev[2], st);
-    GS_CUDA(cudaStreamSynchronize(st));
 
-    if (score) {
-        for (int f = 0; f < nfit; f++) {
-            const int k = f % ns;
-            for (int sp = 0; sp < 2; sp++) {
-                double *out = sp == 0 ? test_scores : train_scores;
-                if (!out) continue;
-                double val;
-                const int *cs = &ccounts[(size_t)f * per_fit + sp * 3 * nc];
-                if (status[f] == 2) val = NAN;
-                else if (kind == GS_SCORE_DEFAULT) {
-                    int64_t ok = 0, tot = 0;
-                    for (int q = 0; q < nc; q++) { tot += cs[q * 3]; ok += cs[q * 3 + 1]; }
-                    val = tot > 0 ? (double)ok / (double)tot : NAN;
-                } else if (kind == GS_SCORE_ROC_AUC) {
-                    double na = 0, nb = 0;
-                    for (int r = 0; r < n; r++) {
-                        const bool in = sp == 0 ? h->is_test(r, k) : (!h->is_test(r, k) && h->is_train(r, k));
-                        if (in) (r >= h->class_start[1] ? nb : na) += 1;
-                    }
-                    const unsigned long long *a = &araw[(size_t)f * 4 + sp * 2];
-                    val = na * nb > 0 ? ((double)a[0] + 0.5 * (double)a[1]) / (na * nb) : NAN;
-                } else {
-                    val = gs_score_from_counts(kind, h->score_pos, nc, cs);
-                }
-                out[f] = val;
-            }
-        }
-    }
     for (int f = 0; f < nfit; f++) {
+        if (score && status[f] == 2) { test_scores[f] = NAN; if (train_scores) train_scores[f] = NAN; }   // a non-finite fit
         if (n_iter) n_iter[f] = iters[f];
         if (fit_status) fit_status[f] = status[f];
         if (coef_out)
@@ -553,18 +483,10 @@ int sag_run(gs_handle *h, int n_cand, const int32_t *solver, const double *alpha
                 for (int j = 0; j <= d; j++) coef_out[((size_t)f * K + q) * (d + 1) + j] = wraw[((size_t)f * K + q) * nvp + j];
         if (stats_out) for (int e = 0; e < 2; e++) stats_out[(size_t)f * 2 + e] = stats[(size_t)f * 2 + e];
     }
-    cudaEventElapsedTime(ms_solve, ev[0], ev[1]);
-    cudaEventElapsedTime(ms_score, ev[1], ev[2]);
-    gs_profile &pf = h->prof;
-    const float keep_h2d = pf.ms_h2d; const int64_t keep_b = pf.h2d_bytes;
-    memset(&pf, 0, sizeof pf);
-    pf.ms_h2d = keep_h2d; pf.h2d_bytes = keep_b;
-    pf.ms_total = *ms_solve + *ms_score; pf.ms_solve = *ms_solve; pf.ms_score = *ms_score;
-    pf.launches = launches;
+    linear_profile(h, ev, launches, ms_solve, ms_score);
     int64_t total = 0;
     for (int t = 0; t < nfit; t++) total += stats[(size_t)t * 2];
-    pf.smo_iterations = total;                                       // SAG sample steps
-    pf.ms_tensor = h->tt.collect(); pf.tensor_flops = h->tt.flops;
+    h->prof.smo_iterations = total;                                  // SAG sample steps
     return GS_OK;
 }
 
@@ -583,11 +505,7 @@ int gs_logreg_sag(gs_handle *h, int32_t n_cand, const int32_t *solver, const dou
                            test_scores, (flags & GS_RETURN_TRAIN) ? train_scores : nullptr, n_iter, fit_status, coef_out, stats,
                            &a, &b);
     if (st) return st;
-    const int nt = n_cand * h->n_splits;
-    for (int i = 0; i < nt; i++) {
-        if (fit_ms) fit_ms[i] = a / (float)nt;
-        if (score_ms) score_ms[i] = b / (float)nt;
-    }
+    spread_call_ms(n_cand * h->n_splits, a, b, fit_ms, score_ms);
     return GS_OK;
 }
 

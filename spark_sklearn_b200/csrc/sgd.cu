@@ -22,6 +22,7 @@
 // float copies WeightVector32 makes (wscale in add() and reset_wscale(), norm(), l1norm()) are float32 values, while its
 // wscale, sq_norm and l1_norm stay double; every operation scikit-learn rounds to float is rounded to float (a float
 // operation made in double and rounded once gives the float result: 53 >= 2 x 24 + 2).
+// The training order and the scoring of the final weights are linear_search.cu's (train_rows, score_linear_fits).
 #include "common.cuh"
 #include "sequential.cuh"
 #include <algorithm>
@@ -351,8 +352,6 @@ sgd_kernel(const SgdFit *__restrict__ fits, int nfits, const SgdCand *__restrict
 
 __global__ void sgd_perm_kernel(uint32_t seed, int l, int *out) { sgd_draw_perm(seed, l, out); }
 
-int64_t round_up(int64_t x, int64_t m) { return (x + m - 1) / m * m; }
-
 template <int NT, typename T>
 cudaError_t launch_sgd_t(bool l1, const SgdFit *fits, int nfits, const SgdCand *cands, const T *X, int d, const int *yc,
                          const double *z, const double *sw, const int *order, int *idx, int64_t lstride, double tol, int max_iter,
@@ -414,15 +413,11 @@ int sgd_run(gs_handle *h, int n_cand, const int32_t *loss, const int32_t *penalt
         if (!(eta0[c] >= 0) || !std::isfinite(eta0[c]) || !std::isfinite(power_t[c])) return fail(GS_ERR_ARG, "eta0 must be >= 0, eta0 and power_t finite");
     }
     const int kind = refit ? GS_SCORE_DEFAULT : h->score_kind;
-    if (!cls && kind != GS_SCORE_DEFAULT && kind != GS_SCORE_NEG_MSE && kind != GS_SCORE_NEG_RMSE) return fail(GS_ERR_ARG, "classification scorer on a regressor");
-    if (cls && (kind == GS_SCORE_NEG_MSE || kind == GS_SCORE_NEG_RMSE)) return fail(GS_ERR_ARG, "regression scorer on a classifier");
     const int ns = refit ? 1 : h->n_splits, nc = cls ? h->n_classes : 1;
     const int KC = cls && nc > 2 ? nc : 1;
-    if (cls && KC > 1 && (kind == GS_SCORE_ROC_AUC || kind == GS_SCORE_F1 || kind == GS_SCORE_PRECISION || kind == GS_SCORE_RECALL))
-        return fail(GS_ERR_UNSUPPORTED, "this scorer is defined for binary problems only");
+    if (int e = check_scorer(h, who, kind, KC)) return e;
+    if (int e = check_class_weight_sets(h, who, ns)) return e;
     const bool weighted = cls && h->class_w_sets > 0;
-    if (weighted && h->class_w_sets != 1 && h->class_w_sets != ns)
-        return fail(GS_ERR_ARG, "gs_set_class_weight was given a weight set per split, but not for this number of splits");
     GS_CUDA(cudaSetDevice(h->device));
     cudaStream_t st = h->stream;
     const int n = (int)h->n, d = (int)h->d;
@@ -432,20 +427,9 @@ int sgd_run(gs_handle *h, int n_cand, const int32_t *loss, const int32_t *penalt
     const bool has_sw = !h->sample_w.empty();
 
     // ---- every split's training rows in the splitter's order (internal rows); zero-weight rows stay (they scale w) ----
-    std::vector<int> by_orig(n);
-    for (int r = 0; r < n; r++) by_orig[h->perm[r]] = r;
-    std::vector<int> order, sp_off(ns + 1, 0);
-    int lmax = 0;
-    for (int k = 0; k < ns; k++) {
-        sp_off[k] = (int)order.size();
-        if (refit) for (int o = 0; o < n; o++) order.push_back(by_orig[o]);
-        else if (!h->train_off.empty()) for (int64_t e = h->train_off[k]; e < h->train_off[k + 1]; e++) order.push_back(by_orig[h->train_order[e]]);
-        else for (int o = 0; o < n; o++) if (h->is_train(by_orig[o], k)) order.push_back(by_orig[o]);
-        const int l = (int)order.size() - sp_off[k];
-        if (l == 0) return fail(GS_ERR_UNSUPPORTED, "a split has no training row");
-        lmax = std::max(lmax, l);
-    }
-    sp_off[ns] = (int)order.size();
+    std::vector<int> order, sp_off;
+    const int lmax = train_rows(h, ns, refit, false, order, sp_off);
+    if (lmax == 0) return fail(GS_ERR_UNSUPPORTED, "a split has no training row");
 
     std::vector<SgdCand> hc(n_cand);
     for (int c = 0; c < n_cand; c++) {
@@ -488,7 +472,7 @@ int sgd_run(gs_handle *h, int n_cand, const int32_t *loss, const int32_t *penalt
     for (auto &e : ev) e = h->evp.get();
     cudaEventRecord(ev[0], st);
 
-    DevBuf &bXa = h->dWork[0], &bZ = h->dWork[1], &bFit = h->dWork[2], &bIdx = h->dWork[3], &bOut = h->dWork[4], &bMeta = h->dWork[5];
+    DevBuf &bXa = h->dWork[0], &bZ = h->dWork[1], &bFit = h->dWork[2], &bIdx = h->dWork[3], &bOut = h->dWork[4];
     const size_t xa_elems = (size_t)npad * nvp;
     GS_CUDA(bXa.reserve((xa_elems * 2 + (size_t)n) * 8));
     double *dXa = bXa.as<double>(), *dXat = dXa + xa_elems, *dSw = dXat + xa_elems;
@@ -538,98 +522,18 @@ int sgd_run(gs_handle *h, int n_cand, const int32_t *loss, const int32_t *penalt
     }
 
     // ---- scoring: decision values [X | 1] . [coef | intercept] of every fit in one FP64 contraction ----
-    std::vector<int> ccounts;
-    std::vector<unsigned long long> araw;
-    std::vector<double> rss;
-    const int per_fit = 6 * nc;
     if (!refit) {
         GS_CUDA(launch_build_xa64(f64 ? nullptr : X32, X64, n, d, 1.0, nvp, npad, dXa, dXat, st));
-        GS_CUDA(bZ.reserve(((size_t)mpad * npad + (cls ? 0 : (size_t)nfit * n)) * 8));
-        double *dZ = bZ.as<double>();
-        h->tt.begin(h->evp, st);
-        GS_CUDA(launch_gemm_nt_f64(dV, nvp, dXa, nvp, dZ, npad, mpad, (int)npad, nvp, nvp, 0, st));
-        h->tt.end(h->evp, st, 2.0 * mpad * (double)npad * nvp);
-        launches += 2;
-        GS_CUDA(bMeta.reserve((size_t)nfit * 4 * 2 + (size_t)nfit * per_fit * 4 + (size_t)nfit * (sizeof(VoteTask) + 16) + (size_t)nfit * 8 + 256));
-        int *dFoldOf = bMeta.as<int>(), *dCnt = dFoldOf + round_up(nfit, 4);
-        if (cls) {
-            std::vector<int> foldof(nfit);
-            for (int f = 0; f < nfit; f++) foldof[f] = f % ns;
-            GS_CUDA(cudaMemcpyAsync(dFoldOf, foldof.data(), (size_t)nfit * 4, cudaMemcpyHostToDevice, st));
-            GS_CUDA(cudaMemsetAsync(dCnt, 0, (size_t)nfit * per_fit * 4, st));
-            GS_CUDA(launch_linsvc_count(dZ, npad, n, nc, KC, Yc, h->masks(), dFoldOf, nfit, dCnt, st));
-            ccounts.resize((size_t)nfit * per_fit);
-            GS_CUDA(cudaMemcpyAsync(ccounts.data(), dCnt, ccounts.size() * 4, cudaMemcpyDeviceToHost, st));
-            launches++;
-            if (kind == GS_SCORE_ROC_AUC) {
-                std::vector<int> meta((size_t)nfit * 2);
-                for (int f = 0; f < nfit; f++) { meta[f] = f; meta[nfit + f] = f % ns; }
-                GS_CUDA(h->dScore.reserve((size_t)nfit * 40));
-                unsigned long long *d_auc = h->dScore.as<unsigned long long>();
-                int *d_meta = (int *)(d_auc + (size_t)nfit * 4);
-                GS_CUDA(cudaMemcpyAsync(d_meta, meta.data(), meta.size() * 4, cudaMemcpyHostToDevice, st));
-                GS_CUDA(cudaMemsetAsync(d_auc, 0, (size_t)nfit * 32, st));
-                GS_CUDA(launch_auc_pairs_f64(dZ, npad, n, h->class_start[1], h->masks(), d_meta, d_meta + nfit, nfit, +1, d_auc, st));
-                araw.resize((size_t)nfit * 4);
-                GS_CUDA(cudaMemcpyAsync(araw.data(), d_auc, (size_t)nfit * 32, cudaMemcpyDeviceToHost, st));
-                launches++;
-            }
-        } else {
-            double *dZc = dZ + (size_t)mpad * npad;                // launch_rss reads rows of n
-            GS_CUDA(cudaMemcpy2DAsync(dZc, (size_t)n * 8, dZ, (size_t)npad * 8, (size_t)n * 8, nfit, cudaMemcpyDeviceToDevice, st));
-            VoteTask *dVt = reinterpret_cast<VoteTask *>(dCnt);
-            double *dRho = reinterpret_cast<double *>(dVt + nfit), *dRss = dRho + nfit;
-            std::vector<VoteTask> vt(nfit);
-            for (int t = 0; t < nfit; t++) vt[t] = VoteTask{t, t % ns};
-            GS_CUDA(cudaMemcpyAsync(dVt, vt.data(), (size_t)nfit * sizeof(VoteTask), cudaMemcpyHostToDevice, st));
-            GS_CUDA(cudaMemsetAsync(dRho, 0, (size_t)nfit * 8, st));
-            GS_CUDA(launch_rss(dZc, dRho, n, Z, h->masks(), dVt, nfit, dRss, st));
-            rss.resize((size_t)nfit * 2);
-            GS_CUDA(cudaMemcpyAsync(rss.data(), dRss, rss.size() * 8, cudaMemcpyDeviceToHost, st));
-            launches += 2;
-        }
+        launches++;
+        GS_CUDA(bZ.reserve((size_t)mpad * npad * 8));
+        if (int e = score_linear_fits(h, dV, dXa, bZ.as<double>(), nfit, KC, ns, kind, test_scores, train_scores, ev[2], launches)) return e;
+    } else {
+        cudaEventRecord(ev[2], st);
+        GS_CUDA(cudaStreamSynchronize(st));
     }
-    cudaEventRecord(ev[2], st);
-    GS_CUDA(cudaStreamSynchronize(st));
 
-    // results by (candidate, split) x class: the fits were launched penalty-grouped, F.out keeps their place
-    if (!refit) {
-        std::vector<double> tss, cntv;
-        if (!cls) regression_split_stats(h, ns, tss, cntv);
-        for (int f = 0; f < nfit; f++) {
-            const int k = f % ns;
-            bool bad = false;
-            for (int q = 0; q < KC; q++) bad |= status[(size_t)f * KC + q] == 2;
-            for (int sp = 0; sp < 2; sp++) {
-                double *out = sp == 0 ? test_scores : train_scores;
-                if (!out) continue;
-                double val;
-                if (bad) val = NAN;
-                else if (!cls) val = regression_score(kind, rss[(size_t)f * 2 + sp], tss[(size_t)k * 2 + sp], cntv[(size_t)k * 2 + sp]);
-                else {
-                    const int *cs = &ccounts[(size_t)f * per_fit + sp * 3 * nc];
-                    if (kind == GS_SCORE_DEFAULT) {
-                        int64_t ok = 0, tot = 0;
-                        for (int q = 0; q < nc; q++) { tot += cs[q * 3]; ok += cs[q * 3 + 1]; }
-                        val = tot > 0 ? (double)ok / (double)tot : NAN;
-                    } else if (kind == GS_SCORE_ROC_AUC) {
-                        double na = 0, nb = 0;
-                        for (int r = 0; r < n; r++) {
-                            const bool in = sp == 0 ? h->is_test(r, k) : (!h->is_test(r, k) && h->is_train(r, k));
-                            if (in) (r >= h->class_start[1] ? nb : na) += 1;
-                        }
-                        const unsigned long long *a = &araw[(size_t)f * 4 + sp * 2];
-                        val = na * nb > 0 ? ((double)a[0] + 0.5 * (double)a[1]) / (na * nb) : NAN;
-                    } else {
-                        val = gs_score_from_counts(kind, h->score_pos, nc, cs);
-                    }
-                }
-                out[f] = val;
-            }
-        }
-    }
     // n_iter / status per (candidate, split): the maximum over the classes; a non-finite class fit (the first in class
-    // order, as one-vs-rest raises it) gives status 2 and its epoch.  The refit reports each class.
+    // order, as one-vs-rest raises it) gives status 2, its epoch and NaN scores.  The refit reports each class.
     for (int f = 0; f < nfit; f++)
         for (int q = 0; q < KC; q++) {
             const int t = f * KC + q;
@@ -653,19 +557,12 @@ int sgd_run(gs_handle *h, int n_cand, const int32_t *loss, const int32_t *penalt
             s = bad ? 2 : (stopped_all ? 0 : 1);
             if (n_iter) n_iter[f] = bad ? bad_it : it;
             if (fit_status) fit_status[f] = s;
+            if (bad) { test_scores[f] = NAN; if (train_scores) train_scores[f] = NAN; }
         }
-    cudaEventElapsedTime(ms_solve, ev[0], ev[1]);
-    cudaEventElapsedTime(ms_score, ev[1], ev[2]);
-    gs_profile &pf = h->prof;
-    const float keep_h2d = pf.ms_h2d; const int64_t keep_b = pf.h2d_bytes;
-    memset(&pf, 0, sizeof pf);
-    pf.ms_h2d = keep_h2d; pf.h2d_bytes = keep_b;
-    pf.ms_total = *ms_solve + *ms_score; pf.ms_solve = *ms_solve; pf.ms_score = *ms_score;
-    pf.launches = launches;
+    linear_profile(h, ev, launches, ms_solve, ms_score);
     int64_t total = 0;
     for (int t = 0; t < nfit_all; t++) total += stats[(size_t)t * 3];
-    pf.smo_iterations = total;                                       // SGD samples processed
-    pf.ms_tensor = h->tt.collect(); pf.tensor_flops = h->tt.flops;
+    h->prof.smo_iterations = total;                                  // SGD samples processed
     return GS_OK;
 }
 
@@ -685,11 +582,7 @@ int gs_sgd(gs_handle *h, int32_t n_cand, const int32_t *loss, const int32_t *pen
                            n_iter_no_change, fit_intercept, shuffle, false, test_scores, (flags & GS_RETURN_TRAIN) ? train_scores : nullptr,
                            n_iter, fit_status, coef_out, stats, &a, &b);
     if (st) return st;
-    const int nt = n_cand * h->n_splits;
-    for (int i = 0; i < nt; i++) {
-        if (fit_ms) fit_ms[i] = a / (float)nt;
-        if (score_ms) score_ms[i] = b / (float)nt;
-    }
+    spread_call_ms(n_cand * h->n_splits, a, b, fit_ms, score_ms);
     return GS_OK;
 }
 
