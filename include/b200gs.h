@@ -88,10 +88,14 @@ int gs_set_kernel_params(gs_handle *h, const int32_t *degree, const double *coef
  * gs_set_data resets the weights. */
 int gs_set_sample_weight(gs_handle *h, const double *w);
 
-/* Scorer of the following gs_svc / gs_logreg / gs_ridge calls.  Replaces: check_scoring(estimator, scoring) and the scorer
- * call inside _fit_and_score (reference base_search.py:43,83-87; grid_search.py:212-214 `scoring=`).  The score is
- * computed on the device from the decision values / Gram statistics already in HBM.  pos_class: class id (index into the
- * sorted labels) that precision / recall / f1 treat as positive (scikit-learn's pos_label=1). */
+/* Scorer of the following search calls (every search; refits do not score).  Replaces: check_scoring(estimator, scoring)
+ * and the scorer call inside _fit_and_score (reference base_search.py:43,83-87; grid_search.py:212-214 `scoring=`).  The
+ * score is computed on the device from the decision values / Gram statistics already in HBM.  pos_class: class id (index
+ * into the sorted labels) that precision / recall / f1 treat as positive (scikit-learn's pos_label=1).  gs_set_scoring
+ * checks only that kind is known and pos_class is in 0..31; every search rejects, before any device work, a scorer its
+ * dataset cannot take: a classification scorer on a regression dataset or a regression scorer on a classification
+ * dataset (GS_ERR_ARG); f1, precision, recall or roc_auc on a dataset without exactly two classes (GS_ERR_UNSUPPORTED);
+ * on a classification dataset, a kind other than GS_SCORE_DEFAULT with pos_class >= n_classes (GS_ERR_ARG). */
 enum {
     GS_SCORE_DEFAULT = 0,            /* accuracy (classifiers) / r2 (Ridge): estimator.score                */
     GS_SCORE_BALANCED_ACCURACY = 1,

@@ -13,43 +13,6 @@
 
 static std::string g_create_error;
 
-// scikit-learn's count-based scores (metrics/_classification.py) from cnt[class][3] = {support, tp, predicted}, float64.
-// Undefined ratios follow zero_division="warn": 0.0.  accuracy_score :187; balanced_accuracy_score :2362 (mean recall over
-// the classes present in y_true); precision_recall_fscore_support :1573 with beta = 1: f = 2 tp / (2 tp + fp + fn).
-double gs_score_from_counts(int kind, int pos_class, int n_classes, const int *cnt)
-{
-    auto sup = [&](int c) { return (double)cnt[c * 3 + 0]; };
-    auto tp = [&](int c) { return (double)cnt[c * 3 + 1]; };
-    auto prd = [&](int c) { return (double)cnt[c * 3 + 2]; };
-    auto f1c = [&](int c) { const double den = sup(c) + prd(c); return den > 0 ? 2.0 * tp(c) / den : 0.0; };   // 2tp + fp + fn = support + predicted
-    double n = 0, correct = 0;
-    for (int c = 0; c < n_classes; c++) { n += sup(c); correct += tp(c); }
-    if (!(n > 0)) return NAN;
-    switch (kind) {
-    case GS_SCORE_DEFAULT: return correct / n;
-    case GS_SCORE_BALANCED_ACCURACY: {
-        double s = 0; int k = 0;
-        for (int c = 0; c < n_classes; c++) if (sup(c) > 0) { s += tp(c) / sup(c); k++; }
-        return k ? s / k : NAN;
-    }
-    case GS_SCORE_F1: return f1c(pos_class);
-    case GS_SCORE_PRECISION: return prd(pos_class) > 0 ? tp(pos_class) / prd(pos_class) : 0.0;
-    case GS_SCORE_RECALL: return sup(pos_class) > 0 ? tp(pos_class) / sup(pos_class) : 0.0;
-    case GS_SCORE_F1_MACRO: {
-        double s = 0;
-        for (int c = 0; c < n_classes; c++) s += f1c(c);
-        return s / n_classes;
-    }
-    case GS_SCORE_F1_MICRO: return correct / n;                         // single-label: micro f1 == accuracy
-    case GS_SCORE_F1_WEIGHTED: {
-        double s = 0;
-        for (int c = 0; c < n_classes; c++) s += f1c(c) * sup(c);
-        return s / n;
-    }
-    default: return NAN;
-    }
-}
-
 void gs_set_error(gs_handle *h, const std::string &msg)
 {
     if (h) h->err = msg; else g_create_error = msg;
@@ -430,6 +393,8 @@ static int svc_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
     }
     const int32_t *degree = h->kp_degree.empty() ? nullptr : h->kp_degree.data();
     const double *coef0 = h->kp_coef0.empty() ? nullptr : h->kp_coef0.data();
+    const int kind = refit ? GS_SCORE_DEFAULT : h->score_kind;
+    if (int e = check_scorer(h, who, kind)) return e;
 
     gs_profile &pf = h->prof;
     SvmSearch search(h, st);
@@ -438,6 +403,7 @@ static int svc_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
     // ---- 1. Gram X X^T, enqueued first: the host prepares the sub-problems below while it runs ----
     if (const int rc = build_gram(h, flags, st)) return rc;
     search.tm.mark(0);
+    const SplitScoreStats ss(h, n_splits, kind);
 
     // ---- 2. sub-problem row lists per (fold, pair): class a rows then class b rows, train rows only ----
     std::vector<int> rows_all;
@@ -518,19 +484,10 @@ static int svc_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
 
     std::vector<int> task_iter(n_tasks, 0), task_sv(n_tasks, 0);
     std::vector<double> task_fit_ms(n_tasks, 0.0);
-    std::vector<int> all_counts((size_t)n_tasks * 4, 0);
-    std::vector<double> task_score((size_t)n_tasks * 2, 0.0);         // non-default scorers: test, train
+    std::vector<double> task_score((size_t)n_tasks * 2, 0.0);         // test, train
     std::vector<char> task_bad(n_tasks, 0);
     std::vector<int> class_counts;
     std::vector<unsigned long long> score_raw;
-    if (!refit && h->score_kind != GS_SCORE_DEFAULT) {
-        const int kd = h->score_kind;
-        if (kd == GS_SCORE_NEG_MSE || kd == GS_SCORE_NEG_RMSE) { gs_set_error(h, std::string(who) + ": regression scorer on a classifier"); return GS_ERR_ARG; }
-        if ((kd == GS_SCORE_ROC_AUC || kd == GS_SCORE_F1 || kd == GS_SCORE_PRECISION || kd == GS_SCORE_RECALL) && nc != 2) {
-            gs_set_error(h, std::string(who) + ": this scorer is defined for binary problems only"); return GS_ERR_UNSUPPORTED;
-        }
-        if (h->score_pos >= nc) { gs_set_error(h, std::string(who) + ": positive class out of range"); return GS_ERR_ARG; }
-    }
     int64_t total_iter = 0;
     double solve_bytes = 0;
 
@@ -721,7 +678,7 @@ static int svc_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
         // -- score (skipped for refit) --
         if (!refit) {
             if (const int rc = search.decisions(g0, g1, group_first)) return rc;
-            const int kind = h->score_kind, nvt = (int)vtasks.size();
+            const int nvt = (int)vtasks.size();
             if (kind == GS_SCORE_DEFAULT) {
                 GS_CUDA(launch_vote(h->dWork[4].as<double>(), search.d_rho, n, nc, h->dY.as<int>(), h->masks(),
                                     d_vt, nvt, d_counts, st));
@@ -802,27 +759,14 @@ static int svc_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
             for (int e = 0; e < 10; e++) fprintf(stderr, " %.0f", pn[2 + e] / it);
             fprintf(stderr, "\n");
         }
-        for (size_t v = 0; v < vtasks.size(); v++)
-            for (int e = 0; e < 4; e++) all_counts[(size_t)vtask_id[v] * 4 + e] = counts[v * 4 + e];
-        if (!refit && h->score_kind == GS_SCORE_ROC_AUC) {
-            for (size_t v = 0; v < vtasks.size(); v++) {
-                const int k = vtasks[v].fold;
-                double na_te = 0, nb_te = 0, na_tr = 0, nb_tr = 0;            // rows of the first / second class inside / outside fold k
-                for (int r = 0; r < n; r++) {
-                    const bool b = r >= h->class_start[1];
-                    if (h->is_test(r, k)) (b ? nb_te : na_te) += 1;
-                    else if (h->is_train(r, k)) (b ? nb_tr : na_tr) += 1;
-                }
-                const unsigned long long *a = &score_raw[v * 4];
-                task_score[(size_t)vtask_id[v] * 2 + 0] = na_te * nb_te > 0 ? ((double)a[0] + 0.5 * (double)a[1]) / (na_te * nb_te) : NAN;
-                task_score[(size_t)vtask_id[v] * 2 + 1] = na_tr * nb_tr > 0 ? ((double)a[2] + 0.5 * (double)a[3]) / (na_tr * nb_tr) : NAN;
-            }
-        } else if (!refit && h->score_kind != GS_SCORE_DEFAULT) {
+        if (!refit)
             for (size_t v = 0; v < vtasks.size(); v++)
-                for (int sp = 0; sp < 2; sp++)
-                    task_score[(size_t)vtask_id[v] * 2 + sp] =
-                        gs_score_from_counts(h->score_kind, h->score_pos, nc, &class_counts[(v * 2 + sp) * nc * 3]);
-        }
+                for (int sp = 0; sp < 2; sp++) {
+                    double &sc = task_score[(size_t)vtask_id[v] * 2 + sp];
+                    if (kind == GS_SCORE_DEFAULT) sc = SplitScoreStats::accuracy(&counts[v * 4 + sp * 2]);
+                    else if (kind == GS_SCORE_ROC_AUC) sc = ss.auc(vtasks[v].fold, sp, &score_raw[v * 4 + sp * 2]);
+                    else sc = ss.counts(&class_counts[(v * 2 + sp) * nc * 3]);
+                }
         if (refit) {
             for (int q = 0; q < np; q++) {
                 if (rho_out) rho_out[q] = rho[q];
@@ -836,15 +780,9 @@ static int svc_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
 
     if (!refit) {
         for (int t = 0; t < n_tasks; t++) {
-            const int *cn = &all_counts[(size_t)t * 4];
-            if (h->score_kind == GS_SCORE_DEFAULT) {
-                test_scores[t] = cn[1] > 0 ? (double)cn[0] / (double)cn[1] : NAN;
-                if (train_scores) train_scores[t] = cn[3] > 0 ? (double)cn[2] / (double)cn[3] : NAN;
-            } else {
-                test_scores[t] = task_score[(size_t)t * 2];
-                if (train_scores) train_scores[t] = task_score[(size_t)t * 2 + 1];
-            }
-            if (task_bad[t] || infeasible[t]) { test_scores[t] = NAN; if (train_scores) train_scores[t] = NAN; }
+            const bool nan = task_bad[t] || infeasible[t];
+            test_scores[t] = nan ? NAN : task_score[(size_t)t * 2];
+            if (train_scores) train_scores[t] = nan ? NAN : task_score[(size_t)t * 2 + 1];
             if (n_iter) n_iter[t] = infeasible[t] ? -1 : task_iter[t];
             if (n_sv) n_sv[t] = task_sv[t];
             if (fit_ms) fit_ms[t] = (float)task_fit_ms[t];

@@ -162,7 +162,7 @@ struct gs_handle {
     DevBuf dS, dXsq;                  // float64 Gram [n][n], squared norms [n]
     DevBuf dK;                        // float32 kernel matrices (batch)
     DevBuf dWork[9];                  // per-search scratch
-    DevBuf dScore;                    // class counts / AUC pair counts of the SVC scorers, SVR's residual sums of squares
+    DevBuf dScore;                    // every search's scoring scratch: class counts, AUC pair counts, residual sums of squares
     int score_kind = 0, score_pos = 1;   // gs_set_scoring
     std::vector<double> class_w;         // gs_set_class_weight: [sets][n_classes]; empty = all ones
     int class_w_sets = 0;
@@ -275,19 +275,31 @@ cudaError_t launch_auc_pairs_f64(const double *score, int64_t ld, int n, int n_a
                                  const int *fold_of_task, int n_tasks, int sign, unsigned long long *out, cudaStream_t st);
 cudaError_t launch_auc_pairs_f32(const float *score, int64_t ld, int n, int n_a, SplitMasks sm, const int *col_of_task,
                                  const int *fold_of_task, int n_tasks, int sign, unsigned long long *out, cudaStream_t st);
-// score of one (task, split) from the class counts cnt[class][3] (float64, scikit-learn's formulas); NaN when undefined
-double gs_score_from_counts(int kind, int pos_class, int n_classes, const int *cnt);
-
-// ---- svr.cu ----
 // Residual sums of squares of regression tasks: rss[task][0 test, 1 train] = sum over the split's rows of
 // (z_r - (dec[first_col][r] - rho[first_col]))^2, float64, fixed-order block reduction (deterministic, no atomics).
 cudaError_t launch_rss(const double *dec, const double *rho, int n, const double *z, SplitMasks sm, const VoteTask *tasks,
                        int n_tasks, double *rss, cudaStream_t st);
-// Per split (0 test, 1 train): row count and total sum of squares of the float64 targets about their mean, in ascending
-// original row order as scikit-learn's y[test] / y[train]
-void regression_split_stats(const gs_handle *h, int n_splits, std::vector<double> &tss, std::vector<double> &cnt);
-// The regression score (r2 / neg MSE / neg RMSE) of one split from its residual sum of squares; NaN for an empty split
-double regression_score(int kind, double rss, double tss, double m);
+// score of one (task, split) from the class counts cnt[class][3] (float64, scikit-learn's formulas); NaN when undefined
+double gs_score_from_counts(int kind, int pos_class, int n_classes, const int *cnt);
+// Rejects, with who in the message, a scorer the dataset cannot take: a classification scorer on a regressor or a
+// regression scorer on a classifier (GS_ERR_ARG), f1 / precision / recall / roc_auc without exactly two classes
+// (GS_ERR_UNSUPPORTED), a scorer other than the default whose positive class is not a class of the dataset (GS_ERR_ARG).
+// Every search calls it before its device work; a refit does not score.
+int check_scorer(gs_handle *h, const char *who, int kind);
+// The score denominators of every split k and part sp (0 test, 1 train: its training rows that are not test rows), and the
+// formulas that turn a search's device outputs into kind's score (float64, scikit-learn's; NaN when undefined).  One host
+// pass over the rows, none for the count-based scorers, which carry their own totals.
+struct SplitScoreStats {
+    int kind, pos_class, n_classes;
+    std::vector<double> rows, n_a, n_b;   // [ns][2]: rows; of those, rows of the first / second class (classifier)
+    std::vector<double> tss;              // [ns][2], regressor: total sum of squares of the float64 targets about their mean,
+                                          // in ascending original row order as scikit-learn's y[test] / y[train]
+    SplitScoreStats(const gs_handle *h, int ns, int kind);
+    static double accuracy(const int *vote);                         // {correct, total} of launch_vote
+    double auc(int k, int sp, const unsigned long long *pairs) const;   // {wins, ties} of launch_auc_pairs_*
+    double counts(const int *cnt) const;                               // cnt[class][3]: gs_score_from_counts
+    double regression(int k, int sp, double rss) const;                // r2 / neg MSE / neg RMSE from a residual sum of squares
+};
 
 // ---- kernel_svm.cu: the host steps the SVC and SVR searches share (an int return is a GS_* status) ----
 int build_gram(gs_handle *h, uint32_t flags, cudaStream_t st);   // S = X X^T -> h->dS, diag(S) -> h->dXsq
@@ -374,9 +386,6 @@ cudaError_t launch_linsvc_count(const double *Zt, int64_t ldz, int n, int K, int
 // refit (ns = 1) trains on every row.  positive_only: only rows of positive sample weight (liblinear's remove_zero_weight).
 // Split k's rows are order[sp_off[k] .. sp_off[k + 1]).  Returns the longest split's row count, 0 when a split has none.
 int train_rows(const gs_handle *h, int ns, bool refit, bool positive_only, std::vector<int> &order, std::vector<int> &sp_off);
-// Rejects, with who in the message, a scorer the dataset cannot take: a classification scorer on a regressor, a regression
-// scorer on a classifier, or a binary-only scorer on K > 1 decision rows per fit
-int check_scorer(gs_handle *h, const char *who, int kind, int K);
 // Rejects class weights given per split for another number of splits than ns
 int check_class_weight_sets(gs_handle *h, const char *who, int ns);
 // liblinear's TRON (tron.cpp) on ncol columns, one round for all open columns at a time: Z = V Xa^T (every column's

@@ -426,10 +426,7 @@ static int knn_run(gs_handle *h, int n_cand, const int32_t *nn, const int32_t *w
     if (classif && nc > 64) { gs_set_error(h, "gs_knn: more than 64 classes"); return GS_ERR_UNSUPPORTED; }
     if (!classif && h->z64.empty()) { gs_set_error(h, "gs_knn: no float64 targets (call gs_set_targets_f64 after gs_set_data)"); return GS_ERR_NO_DATA; }
     const int kind = h->score_kind;
-    const bool reg_kind = kind == GS_SCORE_DEFAULT || kind == GS_SCORE_NEG_MSE || kind == GS_SCORE_NEG_RMSE;
-    if (!classif && !reg_kind) { gs_set_error(h, "gs_knn: classification scorer on a regressor"); return GS_ERR_ARG; }
-    if (classif && (kind == GS_SCORE_NEG_MSE || kind == GS_SCORE_NEG_RMSE)) { gs_set_error(h, "gs_knn: regression scorer on a classifier"); return GS_ERR_ARG; }
-    if (classif && kind == GS_SCORE_ROC_AUC && nc != 2) { gs_set_error(h, "gs_knn: roc_auc needs two classes"); return GS_ERR_UNSUPPORTED; }
+    if (int e = check_scorer(h, "gs_knn", kind)) return e;
     for (int c = 0; c < n_cand; c++) {
         if (nn[c] < 1 || nn[c] > GS_KNN_MAX_NEIGHBORS) { gs_set_error(h, "gs_knn: n_neighbors must be in 1.." + std::to_string(GS_KNN_MAX_NEIGHBORS)); return GS_ERR_UNSUPPORTED; }
         if (weights[c] != GS_KNN_UNIFORM && weights[c] != GS_KNN_DISTANCE) { gs_set_error(h, "gs_knn: unknown weights code"); return GS_ERR_ARG; }
@@ -441,35 +438,11 @@ static int knn_run(gs_handle *h, int n_cand, const int32_t *nn, const int32_t *w
     const bool with_train = (flags & GS_RETURN_TRAIN) && train_scores;
     const int n_tasks = n_cand * ns;
 
-    // training rows of every split, and the sizes / r2 denominators of its test and training sets (original row order)
-    std::vector<int> by_orig(n);
-    for (int r = 0; r < n; r++) by_orig[h->perm[r]] = r;
-    std::vector<double> m_train(ns, 0.0), cnt((size_t)ns * 2, 0.0), tss((size_t)ns * 2, 0.0);
-    std::vector<double> na((size_t)ns * 2, 0.0), nb((size_t)ns * 2, 0.0);        // roc_auc: class-0 / class-1 rows per set
-    for (int k = 0; k < ns; k++) {
-        double sum[2] = {0, 0};
-        for (int o = 0; o < n; o++) {
-            const int r = by_orig[o];
-            const bool te = h->is_test(r, k), tr = h->is_train(r, k);
-            if (tr) m_train[k] += 1;
-            const int sp = te ? 0 : (tr ? 1 : -1);
-            if (sp < 0) continue;
-            cnt[(size_t)k * 2 + sp] += 1;
-            if (classif) ((h->yc[r] == 0 ? na : nb)[(size_t)k * 2 + sp]) += 1;
-            else sum[sp] += h->z64[r];
-        }
-        if (!classif)
-            for (int sp = 0; sp < 2; sp++) {
-                const double m = cnt[(size_t)k * 2 + sp], mean = m > 0 ? sum[sp] / m : 0.0;
-                double s = 0;
-                for (int o = 0; o < n; o++) {
-                    const int r = by_orig[o];
-                    const bool te = h->is_test(r, k), tr = !te && h->is_train(r, k);
-                    if (sp == 0 ? te : tr) { const double e = h->z64[r] - mean; s += e * e; }
-                }
-                tss[(size_t)k * 2 + sp] = s;
-            }
-    }
+    // training rows of every split (a task whose n_neighbors exceeds them scores NaN)
+    std::vector<double> m_train(ns, 0.0);
+    for (int k = 0; k < ns; k++)
+        for (int r = 0; r < n; r++) m_train[k] += h->is_train(r, k);
+    const SplitScoreStats ss(h, ns, kind);
 
     gs_profile &pf = h->prof;
     gs_profile_reset(pf);
@@ -592,19 +565,9 @@ static int knn_run(gs_handle *h, int n_cand, const int32_t *nn, const int32_t *w
                 if (!tasks[q].valid) continue;
                 for (int sp = 0; sp < 2; sp++) {
                     double s;
-                    if (classif && kind == GS_SCORE_ROC_AUC) {
-                        const unsigned long long *a = (const unsigned long long *)host.data() + (size_t)q * 4 + sp * 2;
-                        const double pairs = na[(size_t)k * 2 + sp] * nb[(size_t)k * 2 + sp];
-                        s = pairs > 0 ? ((double)a[0] + 0.5 * (double)a[1]) / pairs : NAN;
-                    } else if (classif) {
-                        s = gs_score_from_counts(kind, h->score_pos, nc, (const int *)host.data() + ((size_t)q * 2 + sp) * nc * 3);
-                    } else {
-                        const double rss = ((const double *)host.data())[(size_t)q * 2 + sp], m = cnt[(size_t)k * 2 + sp];
-                        if (!(m > 0)) s = NAN;
-                        else if (kind == GS_SCORE_NEG_MSE) s = -(rss / m);
-                        else if (kind == GS_SCORE_NEG_RMSE) s = -std::sqrt(rss / m);
-                        else s = gs_r2_score(rss, tss[(size_t)k * 2 + sp], m);
-                    }
+                    if (classif && kind == GS_SCORE_ROC_AUC) s = ss.auc(k, sp, (const unsigned long long *)host.data() + (size_t)q * 4 + sp * 2);
+                    else if (classif) s = ss.counts((const int *)host.data() + ((size_t)q * 2 + sp) * nc * 3);
+                    else s = ss.regression(k, sp, ((const double *)host.data())[(size_t)q * 2 + sp]);
                     (sp == 0 ? sc_test : sc_train)[t] = s;
                 }
             }

@@ -602,9 +602,8 @@ int ridge_run(gs_handle *h, int n_cand, const double *alpha, int fit_intercept, 
     if (n_cand <= 0 || !alpha) { gs_set_error(h, "gs_ridge: bad arguments"); return GS_ERR_ARG; }
     for (int c = 0; c < n_cand; c++)
         if (!(alpha[c] >= 0)) { gs_set_error(h, "gs_ridge: alpha must be >= 0"); return GS_ERR_ARG; }
-    if (h->score_kind != GS_SCORE_DEFAULT && h->score_kind != GS_SCORE_NEG_MSE && h->score_kind != GS_SCORE_NEG_RMSE) {
-        gs_set_error(h, "gs_ridge: classification scorer on a regressor"); return GS_ERR_ARG;
-    }
+    if (!refit)
+        if (int e = check_scorer(h, "gs_ridge", h->score_kind)) return e;
     GS_CUDA(cudaSetDevice(h->device));
     cudaStream_t st = h->stream;
     const int n = (int)h->n, d = (int)h->d, ns = h->n_splits;

@@ -1,6 +1,6 @@
 // linear_search.cu -- the host steps of a primal linear-model search that do not depend on the model (linsvc_run in
-// linsvc.cu, linsvr_run in linsvr.cu, sgd_run in sgd.cu, sag_run in sag.cu): the training rows in fit order, the scorer
-// checks, TRON's round loop, the scoring of the final weights and the call's profile.  Host code only.
+// linsvc.cu, linsvr_run in linsvr.cu, sgd_run in sgd.cu, sag_run in sag.cu): the training rows in fit order, the class
+// weight check, TRON's round loop, the scoring of the final weights and the call's profile.  Host code only.
 #include "common.cuh"
 #include <algorithm>
 #include <cstring>
@@ -29,24 +29,6 @@ int train_rows(const gs_handle *h, int ns, bool refit, bool positive_only, std::
     }
     sp_off[ns] = (int)order.size();
     return lmax;
-}
-
-int check_scorer(gs_handle *h, const char *who, int kind, int K)
-{
-    const bool regression_kind = kind == GS_SCORE_NEG_MSE || kind == GS_SCORE_NEG_RMSE;
-    const char *msg = nullptr;
-    int code = GS_ERR_ARG;
-    if (!h->classification) {
-        if (kind != GS_SCORE_DEFAULT && !regression_kind) msg = "classification scorer on a regressor";
-    } else if (regression_kind) {
-        msg = "regression scorer on a classifier";
-    } else if (K > 1 && (kind == GS_SCORE_ROC_AUC || kind == GS_SCORE_F1 || kind == GS_SCORE_PRECISION || kind == GS_SCORE_RECALL)) {
-        msg = "this scorer is defined for binary problems only";
-        code = GS_ERR_UNSUPPORTED;
-    }
-    if (!msg) return GS_OK;
-    gs_set_error(h, std::string(who) + ": " + msg);
-    return code;
 }
 
 int check_class_weight_sets(gs_handle *h, const char *who, int ns)
@@ -162,37 +144,15 @@ int score_linear_fits(gs_handle *h, const double *V, const double *Xa, double *Z
     cudaEventRecord(ev_end, st);
     GS_CUDA(cudaStreamSynchronize(st));
 
-    // per split k and part sp (0 test, 1 train): row count and total sum of squares (regression), or the class sizes of the
-    // binary problem (ROC-AUC: rows are class-sorted, class 1 from class_start[1])
-    std::vector<double> tss, cnt, na((size_t)ns * 2, 0.0), nb((size_t)ns * 2, 0.0);
-    if (!cls) regression_split_stats(h, ns, tss, cnt);
-    else if (kind == GS_SCORE_ROC_AUC)
-        for (int k = 0; k < ns; k++)
-            for (int r = 0; r < n; r++) {
-                const int sp = h->is_test(r, k) ? 0 : (h->is_train(r, k) ? 1 : -1);
-                if (sp >= 0) (r >= h->class_start[1] ? nb : na)[(size_t)k * 2 + sp] += 1;
-            }
+    const SplitScoreStats ss(h, ns, kind);
     for (int f = 0; f < nfit; f++) {
         const int k = f % ns;
         for (int sp = 0; sp < 2; sp++) {
             double *out = sp == 0 ? test_scores : train_scores;
             if (!out) continue;
-            const size_t ks = (size_t)k * 2 + sp;
-            const int *cs = cls ? &ccounts[(size_t)f * per_fit + sp * 3 * nc] : nullptr;
-            double val;
-            if (!cls) {
-                val = regression_score(kind, rss[(size_t)f * 2 + sp], tss[ks], cnt[ks]);
-            } else if (kind == GS_SCORE_DEFAULT) {
-                int64_t ok = 0, tot = 0;
-                for (int q = 0; q < nc; q++) { tot += cs[q * 3]; ok += cs[q * 3 + 1]; }
-                val = tot > 0 ? (double)ok / (double)tot : NAN;
-            } else if (kind == GS_SCORE_ROC_AUC) {
-                const unsigned long long *a = &araw[(size_t)f * 4 + sp * 2];
-                val = na[ks] * nb[ks] > 0 ? ((double)a[0] + 0.5 * (double)a[1]) / (na[ks] * nb[ks]) : NAN;
-            } else {
-                val = gs_score_from_counts(kind, h->score_pos, nc, cs);
-            }
-            out[f] = val;
+            if (!cls) out[f] = ss.regression(k, sp, rss[(size_t)f * 2 + sp]);
+            else if (kind == GS_SCORE_ROC_AUC) out[f] = ss.auc(k, sp, &araw[(size_t)f * 4 + sp * 2]);
+            else out[f] = ss.counts(&ccounts[(size_t)f * per_fit + sp * 3 * nc]);
         }
     }
     return GS_OK;

@@ -289,7 +289,7 @@ int linsvc_run(gs_handle *h, int n_cand, const double *Cv, double tol, int max_i
     const int ns = refit ? 1 : h->n_splits, nc = h->n_classes;
     const int KC = nc > 2 ? nc : 1;
     if (int e = check_class_weight_sets(h, "gs_linsvc", ns)) return e;
-    if (int e = check_scorer(h, "gs_linsvc", refit ? GS_SCORE_DEFAULT : h->score_kind, KC)) return e;
+    if (int e = check_scorer(h, "gs_linsvc", refit ? GS_SCORE_DEFAULT : h->score_kind)) return e;
     const bool weighted = h->class_w_sets > 0;
     GS_CUDA(cudaSetDevice(h->device));
     cudaStream_t st = h->stream;

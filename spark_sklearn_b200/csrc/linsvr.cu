@@ -411,7 +411,7 @@ int linsvr_run(gs_handle *h, int n_cand, const double *Cv, const double *epsv, c
     if (h->d > GS_LINSVR_MAX_FEATURES)
         return fail(GS_ERR_UNSUPPORTED, "more than " + std::to_string(GS_LINSVR_MAX_FEATURES) + " features");
     const int kind = refit ? GS_SCORE_DEFAULT : h->score_kind;
-    if (int e = check_scorer(h, who, kind, 1)) return e;
+    if (int e = check_scorer(h, who, kind)) return e;
     const int ns = refit ? 1 : h->n_splits, nfit = n_cand * ns;
     for (int c = 0; c < n_cand; c++) {
         if (!(Cv[c] > 0) || !std::isfinite(Cv[c])) return fail(GS_ERR_ARG, "C must be > 0 and finite");

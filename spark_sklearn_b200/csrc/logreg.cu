@@ -547,6 +547,8 @@ int logreg_run(gs_handle *h, int n_cand, const double *Cv, double tol, int max_i
     if (n_cand <= 0 || !Cv) { gs_set_error(h, "gs_logreg: bad arguments"); return GS_ERR_ARG; }
     for (int c = 0; c < n_cand; c++)
         if (!(Cv[c] > 0)) { gs_set_error(h, "gs_logreg: C must be > 0"); return GS_ERR_ARG; }
+    const int kind = refit ? GS_SCORE_DEFAULT : h->score_kind;
+    if (int e = check_scorer(h, "gs_logreg", kind)) return e;
     GS_CUDA(cudaSetDevice(h->device));
     cudaStream_t st = h->stream;
     const int n = (int)h->n, d = (int)h->d, ns = refit ? 1 : h->n_splits;
@@ -697,8 +699,6 @@ int logreg_run(gs_handle *h, int n_cand, const double *Cv, double tol, int max_i
         h->tt.end(h->evp, st, 3.0 * 2.0 * (double)ncol * n * nvp);
         GS_CUDA(cudaMemsetAsync(dCounts, 0, (size_t)nfit * 16, st));
         dim3 grid(64, nfit);
-        const int kind = h->score_kind;
-        if (int e = check_scorer(h, "gs_logreg", kind, KC)) return e;
         // non-default scorers (gs_set_scoring): class counts or ROC-AUC pair counts from the z values already in HBM
         std::vector<int> ccounts;
         std::vector<unsigned long long> araw;
@@ -746,25 +746,14 @@ int logreg_run(gs_handle *h, int n_cand, const double *Cv, double tol, int max_i
         }
         cudaEventRecord(ev[2], st);
         GS_CUDA(cudaStreamSynchronize(st));
+        const SplitScoreStats ss(h, ns, kind);
         for (int col = 0; col < nfit; col++) {
-            const int *cn = &counts[(size_t)col * 4];
-            if (kind == GS_SCORE_DEFAULT) {
-                test_scores[col] = cn[1] > 0 ? (double)cn[0] / cn[1] : NAN;
-                if (train_scores) train_scores[col] = cn[3] > 0 ? (double)cn[2] / cn[3] : NAN;
-            } else if (kind == GS_SCORE_ROC_AUC) {
-                const int k = col % ns;
-                double na_te = 0, nb_te = 0, na_tr = 0, nb_tr = 0;
-                for (int r = 0; r < n; r++) {
-                    const bool b = r >= h->class_start[1];
-                    if (h->is_test(r, k)) (b ? nb_te : na_te) += 1;
-                    else if (h->is_train(r, k)) (b ? nb_tr : na_tr) += 1;
-                }
-                const unsigned long long *a = &araw[(size_t)col * 4];
-                test_scores[col] = na_te * nb_te > 0 ? ((double)a[0] + 0.5 * (double)a[1]) / (na_te * nb_te) : NAN;
-                if (train_scores) train_scores[col] = na_tr * nb_tr > 0 ? ((double)a[2] + 0.5 * (double)a[3]) / (na_tr * nb_tr) : NAN;
-            } else {
-                test_scores[col] = gs_score_from_counts(kind, h->score_pos, nc, &ccounts[(size_t)col * per_fit]);
-                if (train_scores) train_scores[col] = gs_score_from_counts(kind, h->score_pos, nc, &ccounts[(size_t)col * per_fit + 3 * nc]);
+            for (int sp = 0; sp < 2; sp++) {
+                double *out = sp == 0 ? test_scores : train_scores;
+                if (!out) continue;
+                if (kind == GS_SCORE_DEFAULT) out[col] = SplitScoreStats::accuracy(&counts[(size_t)col * 4 + sp * 2]);
+                else if (kind == GS_SCORE_ROC_AUC) out[col] = ss.auc(col % ns, sp, &araw[(size_t)col * 4 + sp * 2]);
+                else out[col] = ss.counts(&ccounts[(size_t)col * per_fit + sp * 3 * nc]);
             }
             if (n_iter) n_iter[col] = fin[col].iter;
         }

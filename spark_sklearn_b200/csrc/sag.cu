@@ -376,7 +376,7 @@ int sag_run(gs_handle *h, int n_cand, const int32_t *solver, const double *alpha
     const int n = (int)h->n, d = (int)h->d, dk = d * K;
     if (dk > GS_SAG_MAX_COEF) return fail(GS_ERR_UNSUPPORTED, "features x weight rows above GS_SAG_MAX_COEF (" + std::to_string(GS_SAG_MAX_COEF) + ")");
     const int kind = refit || !cls ? GS_SCORE_DEFAULT : h->score_kind;
-    if (int e = check_scorer(h, who, kind, K)) return e;
+    if (int e = check_scorer(h, who, kind)) return e;
     if (int e = check_class_weight_sets(h, who, ns)) return e;
     const bool weighted = cls && h->class_w_sets > 0;
     GS_CUDA(cudaSetDevice(h->device));

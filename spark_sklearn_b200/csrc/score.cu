@@ -1,4 +1,5 @@
-// score.cu -- SVC decision values for every (row, sub-model) and one-vs-one voting / accuracy.
+// score.cu -- SVC decision values for every (row, sub-model), one-vs-one voting / accuracy, the scorers' device counts, and
+// the host side of scoring every search shares: the scorer check, the per-split score denominators and the score formulas.
 //
 // libsvm predicts with float64 kernel values (svm.cpp:2821-2904 svm_predict_values calls
 // Kernel::k_function in double; the float32 rounding applies only to the training Q matrix), so the
@@ -9,6 +10,7 @@
 // with the exp (or powi / tanh) fused into the operand load.  coef is zero outside a sub-model's training rows.
 #include "common.cuh"
 #include <algorithm>
+#include <cmath>
 
 namespace {
 
@@ -247,6 +249,40 @@ auc_pairs_kernel(const T *__restrict__ score, int64_t ld, int n, int n_a, SplitM
     if (threadIdx.x < 4 && red[threadIdx.x]) atomicAdd(&out[(size_t)task * 4 + threadIdx.x], red[threadIdx.x]);
 }
 
+
+// rss[task][0 / 1] = sum over test / training rows of the split of (z - (dec - rho))^2.  One block per task; every thread
+// sums a fixed row stride, then a fixed shared-memory tree: the same bits every run.
+constexpr int RSS_NT = 256;
+
+__global__ void __launch_bounds__(RSS_NT)
+rss_kernel(const double *__restrict__ dec, const double *__restrict__ rho, int n, const double *__restrict__ z, SplitMasks sm,
+           const VoteTask *__restrict__ tasks, double *__restrict__ rss)
+{
+    __shared__ double red[2][RSS_NT];
+    const VoteTask T = tasks[blockIdx.x];
+    const double *__restrict__ dv = dec + (size_t)T.first_col * n;
+    const double b = rho[T.first_col];
+    double s_te = 0.0, s_tr = 0.0;
+    for (int r = threadIdx.x; r < n; r += RSS_NT) {
+        const bool te = split_test(sm, r, T.fold), tr = !te && split_train(sm, r, T.fold);
+        if (te || tr) {
+            const double e = __dsub_rn(z[r], __dsub_rn(dv[r], b));
+            const double e2 = __dmul_rn(e, e);
+            if (te) s_te = __dadd_rn(s_te, e2); else s_tr = __dadd_rn(s_tr, e2);
+        }
+    }
+    red[0][threadIdx.x] = s_te; red[1][threadIdx.x] = s_tr;
+    __syncthreads();
+    for (int w = RSS_NT / 2; w > 0; w >>= 1) {
+        if ((int)threadIdx.x < w) {
+            red[0][threadIdx.x] = __dadd_rn(red[0][threadIdx.x], red[0][threadIdx.x + w]);
+            red[1][threadIdx.x] = __dadd_rn(red[1][threadIdx.x], red[1][threadIdx.x + w]);
+        }
+        __syncthreads();
+    }
+    if (threadIdx.x < 2) rss[(size_t)blockIdx.x * 2 + threadIdx.x] = red[threadIdx.x][0];
+}
+
 }  // namespace
 
 cudaError_t launch_vote_classes(const double *dec, const double *rho, int n, int n_classes, const int *y,
@@ -357,4 +393,128 @@ cudaError_t launch_vote(const double *dec, const double *rho, int n, int n_class
         vote_kernel<<<grid, 256, 0, st>>>(dec, rho, n, n_classes, y, sm, tasks + t0, counts + (size_t)t0 * 4);
     }
     return cudaGetLastError();
+}
+
+cudaError_t launch_rss(const double *dec, const double *rho, int n, const double *z, SplitMasks sm, const VoteTask *tasks,
+                       int n_tasks, double *rss, cudaStream_t st)
+{
+    if (n_tasks <= 0) return cudaSuccess;
+    rss_kernel<<<n_tasks, RSS_NT, 0, st>>>(dec, rho, n, z, sm, tasks, rss);
+    return cudaGetLastError();
+}
+
+// scikit-learn's count-based scores (metrics/_classification.py) from cnt[class][3] = {support, tp, predicted}, float64.
+// Undefined ratios follow zero_division="warn": 0.0.  accuracy_score :187; balanced_accuracy_score :2362 (mean recall over
+// the classes present in y_true); precision_recall_fscore_support :1573 with beta = 1: f = 2 tp / (2 tp + fp + fn).
+double gs_score_from_counts(int kind, int pos_class, int n_classes, const int *cnt)
+{
+    auto sup = [&](int c) { return (double)cnt[c * 3 + 0]; };
+    auto tp = [&](int c) { return (double)cnt[c * 3 + 1]; };
+    auto prd = [&](int c) { return (double)cnt[c * 3 + 2]; };
+    auto f1c = [&](int c) { const double den = sup(c) + prd(c); return den > 0 ? 2.0 * tp(c) / den : 0.0; };   // 2tp + fp + fn = support + predicted
+    double n = 0, correct = 0;
+    for (int c = 0; c < n_classes; c++) { n += sup(c); correct += tp(c); }
+    if (!(n > 0)) return NAN;
+    switch (kind) {
+    case GS_SCORE_DEFAULT: return correct / n;
+    case GS_SCORE_BALANCED_ACCURACY: {
+        double s = 0; int k = 0;
+        for (int c = 0; c < n_classes; c++) if (sup(c) > 0) { s += tp(c) / sup(c); k++; }
+        return k ? s / k : NAN;
+    }
+    case GS_SCORE_F1: return f1c(pos_class);
+    case GS_SCORE_PRECISION: return prd(pos_class) > 0 ? tp(pos_class) / prd(pos_class) : 0.0;
+    case GS_SCORE_RECALL: return sup(pos_class) > 0 ? tp(pos_class) / sup(pos_class) : 0.0;
+    case GS_SCORE_F1_MACRO: {
+        double s = 0;
+        for (int c = 0; c < n_classes; c++) s += f1c(c);
+        return s / n_classes;
+    }
+    case GS_SCORE_F1_MICRO: return correct / n;                         // single-label: micro f1 == accuracy
+    case GS_SCORE_F1_WEIGHTED: {
+        double s = 0;
+        for (int c = 0; c < n_classes; c++) s += f1c(c) * sup(c);
+        return s / n;
+    }
+    default: return NAN;
+    }
+}
+
+int check_scorer(gs_handle *h, const char *who, int kind)
+{
+    const bool regression_kind = kind == GS_SCORE_NEG_MSE || kind == GS_SCORE_NEG_RMSE;
+    const bool binary_kind = kind == GS_SCORE_ROC_AUC || kind == GS_SCORE_F1 || kind == GS_SCORE_PRECISION || kind == GS_SCORE_RECALL;
+    const char *msg = nullptr;
+    int code = GS_ERR_ARG;
+    if (!h->classification) {
+        if (kind != GS_SCORE_DEFAULT && !regression_kind) msg = "classification scorer on a regressor";
+    } else if (regression_kind) {
+        msg = "regression scorer on a classifier";
+    } else if (binary_kind && h->n_classes != 2) {
+        msg = "this scorer is defined for binary problems only";
+        code = GS_ERR_UNSUPPORTED;
+    } else if (kind != GS_SCORE_DEFAULT && h->score_pos >= h->n_classes) {
+        msg = "positive class out of range";
+    }
+    if (!msg) return GS_OK;
+    gs_set_error(h, std::string(who) + ": " + msg);
+    return code;
+}
+
+SplitScoreStats::SplitScoreStats(const gs_handle *h, int ns, int kind_)
+    : kind(kind_), pos_class(h->score_pos), n_classes(h->n_classes)
+{
+    const bool cls = h->classification;
+    if (cls && kind != GS_SCORE_ROC_AUC) return;                         // the count-based scores carry their own totals
+    const int n = (int)h->n;
+    std::vector<int> by_orig(n);
+    for (int r = 0; r < n; r++) by_orig[h->perm[r]] = r;
+    rows.assign((size_t)ns * 2, 0.0); n_a.assign((size_t)ns * 2, 0.0); n_b.assign((size_t)ns * 2, 0.0); tss.assign((size_t)ns * 2, 0.0);
+    for (int k = 0; k < ns; k++) {
+        double sum[2] = {0, 0};
+        for (int o = 0; o < n; o++) {
+            const int r = by_orig[o];
+            const int sp = h->is_test(r, k) ? 0 : (h->is_train(r, k) ? 1 : -1);
+            if (sp < 0) continue;
+            rows[(size_t)k * 2 + sp] += 1;
+            if (cls) (r >= h->class_start[1] ? n_b : n_a)[(size_t)k * 2 + sp] += 1;    // rows are class-sorted
+            else sum[sp] += h->z64[r];
+        }
+        if (cls) continue;
+        for (int sp = 0; sp < 2; sp++) {
+            // np.average then sum of squared deviations, ascending original row order as scikit-learn's y[test] / y[train]
+            const double m = rows[(size_t)k * 2 + sp], mean = m > 0 ? sum[sp] / m : 0.0;
+            double s = 0;
+            for (int o = 0; o < n; o++) {
+                const int r = by_orig[o];
+                if (sp == 0 ? h->is_test(r, k) : (!h->is_test(r, k) && h->is_train(r, k))) { const double e = h->z64[r] - mean; s += e * e; }
+            }
+            tss[(size_t)k * 2 + sp] = s;
+        }
+    }
+}
+
+double SplitScoreStats::accuracy(const int *vote)
+{
+    return vote[1] > 0 ? (double)vote[0] / (double)vote[1] : NAN;
+}
+
+double SplitScoreStats::auc(int k, int sp, const unsigned long long *pairs) const
+{
+    const double np_ = n_a[(size_t)k * 2 + sp] * n_b[(size_t)k * 2 + sp];
+    return np_ > 0 ? ((double)pairs[0] + 0.5 * (double)pairs[1]) / np_ : NAN;
+}
+
+double SplitScoreStats::counts(const int *cnt) const
+{
+    return gs_score_from_counts(kind, pos_class, n_classes, cnt);
+}
+
+double SplitScoreStats::regression(int k, int sp, double rss) const
+{
+    const double m = rows[(size_t)k * 2 + sp];
+    if (!(m > 0)) return NAN;
+    if (kind == GS_SCORE_NEG_MSE) return -(rss / m);                       // mean_squared_error
+    if (kind == GS_SCORE_NEG_RMSE) return -std::sqrt(rss / m);             // root_mean_squared_error
+    return gs_r2_score(rss, tss[(size_t)k * 2 + sp], m);
 }

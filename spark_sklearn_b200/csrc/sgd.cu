@@ -415,7 +415,7 @@ int sgd_run(gs_handle *h, int n_cand, const int32_t *loss, const int32_t *penalt
     const int kind = refit ? GS_SCORE_DEFAULT : h->score_kind;
     const int ns = refit ? 1 : h->n_splits, nc = cls ? h->n_classes : 1;
     const int KC = cls && nc > 2 ? nc : 1;
-    if (int e = check_scorer(h, who, kind, KC)) return e;
+    if (int e = check_scorer(h, who, kind)) return e;
     if (int e = check_class_weight_sets(h, who, ns)) return e;
     const bool weighted = cls && h->class_w_sets > 0;
     GS_CUDA(cudaSetDevice(h->device));

@@ -1,5 +1,4 @@
-// svr.cu -- epsilon-SVR and nu-SVR searches and refits (gs_svr / gs_svr_refit, gs_nusvr / gs_nusvr_refit) and the regression
-// scorer over SVR decision values.
+// svr.cu -- epsilon-SVR and nu-SVR searches and refits (gs_svr / gs_svr_refit, gs_nusvr / gs_nusvr_refit).
 //
 // An SVR fit on l training rows is libsvm's C-SVC Solver on 2l variables (svm.cpp solve_epsilon_svr): positions 0..l-1 are
 // the rows with y = +1 and linear term eps - z, positions l..2l-1 the same rows with y = -1 and linear term eps + z.  The
@@ -11,83 +10,6 @@
 #include <cmath>
 #include <cstring>
 #include <numeric>
-
-namespace {
-
-// rss[task][0 / 1] = sum over test / training rows of the split of (z - (dec - rho))^2.  One block per task; every thread
-// sums a fixed row stride, then a fixed shared-memory tree: the same bits every run.
-constexpr int RSS_NT = 256;
-
-__global__ void __launch_bounds__(RSS_NT)
-rss_kernel(const double *__restrict__ dec, const double *__restrict__ rho, int n, const double *__restrict__ z, SplitMasks sm,
-           const VoteTask *__restrict__ tasks, double *__restrict__ rss)
-{
-    __shared__ double red[2][RSS_NT];
-    const VoteTask T = tasks[blockIdx.x];
-    const double *__restrict__ dv = dec + (size_t)T.first_col * n;
-    const double b = rho[T.first_col];
-    double s_te = 0.0, s_tr = 0.0;
-    for (int r = threadIdx.x; r < n; r += RSS_NT) {
-        const bool te = split_test(sm, r, T.fold), tr = !te && split_train(sm, r, T.fold);
-        if (te || tr) {
-            const double e = __dsub_rn(z[r], __dsub_rn(dv[r], b));
-            const double e2 = __dmul_rn(e, e);
-            if (te) s_te = __dadd_rn(s_te, e2); else s_tr = __dadd_rn(s_tr, e2);
-        }
-    }
-    red[0][threadIdx.x] = s_te; red[1][threadIdx.x] = s_tr;
-    __syncthreads();
-    for (int w = RSS_NT / 2; w > 0; w >>= 1) {
-        if ((int)threadIdx.x < w) {
-            red[0][threadIdx.x] = __dadd_rn(red[0][threadIdx.x], red[0][threadIdx.x + w]);
-            red[1][threadIdx.x] = __dadd_rn(red[1][threadIdx.x], red[1][threadIdx.x + w]);
-        }
-        __syncthreads();
-    }
-    if (threadIdx.x < 2) rss[(size_t)blockIdx.x * 2 + threadIdx.x] = red[threadIdx.x][0];
-}
-
-}  // namespace
-
-cudaError_t launch_rss(const double *dec, const double *rho, int n, const double *z, SplitMasks sm, const VoteTask *tasks,
-                       int n_tasks, double *rss, cudaStream_t st)
-{
-    if (n_tasks <= 0) return cudaSuccess;
-    rss_kernel<<<n_tasks, RSS_NT, 0, st>>>(dec, rho, n, z, sm, tasks, rss);
-    return cudaGetLastError();
-}
-
-void regression_split_stats(const gs_handle *h, int n_splits, std::vector<double> &tss, std::vector<double> &cnt)
-{
-    const int n = (int)h->n;
-    std::vector<int> by_orig(n);
-    for (int r = 0; r < n; r++) by_orig[h->perm[r]] = r;
-    tss.assign((size_t)n_splits * 2, 0.0); cnt.assign((size_t)n_splits * 2, 0.0);
-    for (int k = 0; k < n_splits; k++)
-        for (int sp = 0; sp < 2; sp++) {
-            // np.average then sum of squared deviations, ascending original row order as scikit-learn's y[test] / y[train]
-            double sum = 0, m = 0;
-            for (int o = 0; o < n; o++) {
-                const int r = by_orig[o];
-                if (sp == 0 ? h->is_test(r, k) : (!h->is_test(r, k) && h->is_train(r, k))) { sum += h->z64[r]; m += 1; }
-            }
-            const double mean = m > 0 ? sum / m : 0.0;
-            double s = 0;
-            for (int o = 0; o < n; o++) {
-                const int r = by_orig[o];
-                if (sp == 0 ? h->is_test(r, k) : (!h->is_test(r, k) && h->is_train(r, k))) { const double e = h->z64[r] - mean; s += e * e; }
-            }
-            tss[(size_t)k * 2 + sp] = s; cnt[(size_t)k * 2 + sp] = m;
-        }
-}
-
-double regression_score(int kind, double rss, double tss, double m)
-{
-    if (!(m > 0)) return NAN;
-    if (kind == GS_SCORE_NEG_MSE) return -(rss / m);                       // mean_squared_error
-    if (kind == GS_SCORE_NEG_RMSE) return -std::sqrt(rss / m);             // root_mean_squared_error
-    return gs_r2_score(rss, tss, m);
-}
 
 // nu == false: epsilon-SVR, epsv[c] is epsilon.  nu == true: nu-SVR (svm.cpp solve_nu_svr on Solver_NU), epsv[c] is nu.
 static int svr_run(gs_handle *h, int n_cand, const int32_t *kernel, const double *Cv, const double *epsv, const double *gamma,
@@ -104,9 +26,7 @@ static int svr_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
     if (!h->sample_w.empty()) { gs_set_error(h, std::string(who) + ": sample weights are not supported by the SVR kernels"); return GS_ERR_UNSUPPORTED; }
     if (h->class_w_sets > 0) { gs_set_error(h, std::string(who) + ": class weights do not apply to a regressor"); return GS_ERR_ARG; }
     const int kind = refit ? GS_SCORE_DEFAULT : h->score_kind;
-    if (kind != GS_SCORE_DEFAULT && kind != GS_SCORE_NEG_MSE && kind != GS_SCORE_NEG_RMSE) {
-        gs_set_error(h, std::string(who) + ": classification scorer on a regressor"); return GS_ERR_ARG;
-    }
+    if (int e = check_scorer(h, who, kind)) return e;
     for (int c = 0; c < n_cand; c++) {
         if (kernel[c] != GS_KERNEL_LINEAR && kernel[c] != GS_KERNEL_RBF) { gs_set_error(h, std::string(who) + ": unsupported kernel id"); return GS_ERR_UNSUPPORTED; }
         if (!(Cv[c] > 0) || !std::isfinite(Cv[c])) { gs_set_error(h, std::string(who) + ": C must be > 0"); return GS_ERR_ARG; }
@@ -147,10 +67,6 @@ static int svr_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
     }
     sp_off[n_splits] = (int)rows_all.size();
     if (const int rc = search.group(who, n_cand, n_splits, kernel, gamma, nullptr, nullptr)) return rc;   // groups by kernel matrix (kernel, gamma)
-
-    // ---- per-split sizes and r2 denominators (they depend on the split only) ----
-    std::vector<double> tss((size_t)n_splits * 2, 0.0), cnt((size_t)n_splits * 2, 0.0);
-    if (!refit) regression_split_stats(h, n_splits, tss, cnt);
 
     gs_profile &pf = h->prof;
     search.begin();
@@ -292,13 +208,11 @@ static int svr_run(gs_handle *h, int n_cand, const int32_t *kernel, const double
     if (const int rc = search.finish(total_iter, solve_bytes)) return rc;
 
     if (!refit) {
+        const SplitScoreStats ss(h, n_splits, kind);
         for (int t = 0; t < n_tasks; t++) {
             const int k = t % n_splits;
-            double sc[2];
-            for (int sp = 0; sp < 2; sp++)
-                sc[sp] = regression_score(kind, task_rss[(size_t)t * 2 + sp], tss[(size_t)k * 2 + sp], cnt[(size_t)k * 2 + sp]);
-            test_scores[t] = task_bad[t] ? NAN : sc[0];
-            if (train_scores) train_scores[t] = task_bad[t] ? NAN : sc[1];
+            test_scores[t] = task_bad[t] ? NAN : ss.regression(k, 0, task_rss[(size_t)t * 2]);
+            if (train_scores) train_scores[t] = task_bad[t] ? NAN : ss.regression(k, 1, task_rss[(size_t)t * 2 + 1]);
             if (n_iter) n_iter[t] = task_iter[t];
             if (n_sv) n_sv[t] = task_sv[t];
             if (fit_ms) fit_ms[t] = (float)task_fit_ms[t];

@@ -80,3 +80,34 @@ def test_ridge_scorers(engine, scoring):
         rel = np.abs(a["mean_train_score"] - b["mean_train_score"]) / np.abs(b["mean_train_score"])
         assert rel.max() <= 3e-3, rel
     assert a["rank_test_score"][np.argmin(b["rank_test_score"])] == 1 or np.ptp(b["mean_test_score"][a["rank_test_score"] <= 2]) < 1e-2 * np.abs(b["mean_test_score"]).min()
+
+
+_SEARCHES = {
+    "svc": lambda e: e.svc(["rbf"], [1.0], [0.1]),
+    "nusvc": lambda e: e.svc(["rbf"], [0.5], [0.1], nu=True),
+    "logreg": lambda e: e.logreg([1.0]),
+    "linsvc": lambda e: e.linsvc([1.0]),
+    "sgd": lambda e: e.sgd(["hinge"], ["l2"], 1e-4, 0.15, 0.1, ["optimal"], 0.0, 0.5, np.ones((1, 3))),
+    "logreg_sag": lambda e: e.logreg_sag([["sag"] * 3], 1e-3, 0.0, 0.1, [[1, 2, 3]], "log"),
+    "knn": lambda e: e.knn([3], ["uniform"], ["euclidean"]),
+}
+
+
+@pytest.mark.parametrize("search", sorted(_SEARCHES))
+def test_positive_class_out_of_range_is_rejected(engine, search):
+    """A positive class the dataset does not have (f1 with class 5 of two) is rejected before any device work"""
+    from spark_sklearn_b200.engine import EngineError
+    rng = np.random.RandomState(0)
+    X = rng.standard_normal((60, 4))
+    y = (X[:, 0] > 0).astype(np.int32)
+    engine.set_data(X, (np.arange(60) % 3).astype(np.int8), 3, y_class=y)
+    try:
+        engine.set_scoring(2, 5)
+        before = engine.profile()
+        with pytest.raises(EngineError) as e:
+            _SEARCHES[search](engine)
+        assert e.value.status == -2, str(e.value)
+        assert "positive class out of range" in str(e.value)
+        assert engine.profile() == before                  # the search returned before it reset its profile
+    finally:
+        engine.set_scoring(0, 1)

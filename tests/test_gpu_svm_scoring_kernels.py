@@ -1,5 +1,5 @@
-"""The kernel-SVM scoring kernels (csrc/score.cu, csrc/svr.cu) and the kernel-matrix guard (csrc/gram.cu), one kernel at a
-time, against float64 / integer references in numpy.
+"""The kernel-SVM scoring kernels (csrc/score.cu) and the kernel-matrix guard (csrc/gram.cu), one kernel at a time, against
+float64 / integer references in numpy.
 
 The GPU tests feed each kernel through its test hook (gs_debug_decision, gs_debug_score, gs_debug_kernel_matrix) and compare
 number for number: decision values within a rounding-error bound of a long-double sum over the GPU's own float64 Gram,
