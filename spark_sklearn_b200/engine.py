@@ -133,6 +133,11 @@ def _ptr(a):
     return None if a is None else a.ctypes.data_as(ctypes.c_void_p)
 
 
+def _kernel_id(kernel):
+    """a kernel name (KERNEL_ID) or id -> the id"""
+    return KERNEL_ID[kernel] if isinstance(kernel, str) else int(kernel)
+
+
 _device_count = None
 
 
@@ -169,6 +174,19 @@ class Engine:
     def _check(self, st):
         if st != 0:
             raise EngineError(st, (self._L.gs_last_error(self._h) or b"").decode())
+
+    def _search(self, n_cand, return_train, call, counts=()):
+        """One search call: out = the per-(candidate, split) outputs (float64 test / train scores, float32 fit_ms / score_ms,
+        int32 counts such as n_iter); call(out) runs the gs_* function, which always gets a train buffer.  -> out, train None
+        unless return_train."""
+        shape = (n_cand, self.n_splits)
+        out = dict(test=np.zeros(shape), train=np.zeros(shape), fit_ms=np.zeros(shape, np.float32),
+                   score_ms=np.zeros(shape, np.float32))
+        out.update((k, np.zeros(shape, np.int32)) for k in counts)
+        self._check(call(out))
+        if not return_train:
+            out["train"] = None
+        return out
 
     def set_splits(self, test_mask, train_mask, n_splits):
         """General CV splits (include/b200gs.h gs_set_splits): uint64 [n][2] membership masks, after set_data."""
@@ -216,22 +234,16 @@ class Engine:
     def _kernel_svm(self, fn, kernel, C, per_cand, gamma, tol, max_iter, shrinking, return_train, flags):
         """gs_svc / gs_svr: kernel names or ids, C and the estimator's other per-candidate arrays (per_cand), gamma per
         candidate or per (candidate, split) -> the per-(candidate, split) outputs"""
-        kernel = np.ascontiguousarray([KERNEL_ID[k] if isinstance(k, str) else int(k) for k in kernel], np.int32)
+        kernel = np.ascontiguousarray([_kernel_id(k) for k in kernel], np.int32)
         C = np.ascontiguousarray(C, np.float64)
         n_cand = len(C)
         gamma = np.ascontiguousarray(np.broadcast_to(np.asarray(gamma, np.float64).reshape(n_cand, -1),
                                                      (n_cand, self.n_splits)))
-        shape = (n_cand, self.n_splits)
-        out = dict(test=np.zeros(shape), train=np.zeros(shape), n_iter=np.zeros(shape, np.int32),
-                   n_sv=np.zeros(shape, np.int32), fit_ms=np.zeros(shape, np.float32),
-                   score_ms=np.zeros(shape, np.float32))
         fl = int(flags) | (GS_RETURN_TRAIN if return_train else 0) | (0 if shrinking else GS_NO_SHRINKING)
-        self._check(fn(self._h, n_cand, _ptr(kernel), _ptr(C), *[_ptr(a) for a in per_cand], _ptr(gamma), float(tol),
-                       int(max_iter), fl, _ptr(out["test"]), _ptr(out["train"]), _ptr(out["n_iter"]), _ptr(out["n_sv"]),
-                       _ptr(out["fit_ms"]), _ptr(out["score_ms"])))
-        if not return_train:
-            out["train"] = None
-        return out
+        return self._search(n_cand, return_train, lambda out: fn(
+            self._h, n_cand, _ptr(kernel), _ptr(C), *[_ptr(a) for a in per_cand], _ptr(gamma), float(tol), int(max_iter), fl,
+            _ptr(out["test"]), _ptr(out["train"]), _ptr(out["n_iter"]), _ptr(out["n_sv"]), _ptr(out["fit_ms"]),
+            _ptr(out["score_ms"])), ("n_iter", "n_sv"))
 
     def _with_kernel_params(self, kernel_ids, degree, coef0, call):
         """call() with gs_set_kernel_params set to degree / coef0 (scalars or one per candidate) when a poly or sigmoid
@@ -251,7 +263,7 @@ class Engine:
             nu=False):
         """degree / coef0: scalars or one per candidate, read by the poly and sigmoid candidates (defaults 3 / 0.0).
         nu=True: NuSVC (gs_nusvc), C holds nu; a fit that is infeasible for its nu scores NaN with n_iter -1."""
-        ids = [KERNEL_ID[k] if isinstance(k, str) else int(k) for k in kernel]
+        ids = [_kernel_id(k) for k in kernel]
         return self._with_kernel_params(ids, degree, coef0, lambda: self._kernel_svm(
             self._L.gs_nusvc if nu else self._L.gs_svc, ids, C, [], gamma, tol, max_iter, shrinking, return_train, flags))
 
@@ -261,7 +273,7 @@ class Engine:
         coef = np.zeros((n_pairs, self.n))
         rho = np.zeros(n_pairs)
         it = np.zeros(n_pairs, np.int32)
-        k = KERNEL_ID[kernel] if isinstance(kernel, str) else int(kernel)
+        k = _kernel_id(kernel)
         fn = self._L.gs_nusvc_refit if nu else self._L.gs_svc_refit
         self._with_kernel_params([k], degree, coef0, lambda: self._check(fn(
             self._h, k, float(C), float(gamma), float(tol), int(max_iter), 0 if shrinking else GS_NO_SHRINKING, _ptr(coef),
@@ -287,7 +299,7 @@ class Engine:
         coef = np.zeros(self.n)
         rho = np.zeros(1)
         it = np.zeros(1, np.int32)
-        k = KERNEL_ID[kernel] if isinstance(kernel, str) else int(kernel)
+        k = _kernel_id(kernel)
         fl = int(flags) | (0 if shrinking else GS_NO_SHRINKING)
         self._check((self._L.gs_nusvr_refit if nu else self._L.gs_svr_refit)(self._h, k, float(C), float(epsilon), float(gamma), float(tol), int(max_iter),
                                          fl, _ptr(coef), _ptr(rho), _ptr(it)))
@@ -295,15 +307,9 @@ class Engine:
 
     def ridge(self, alpha, fit_intercept=True, return_train=True):
         alpha = np.ascontiguousarray(alpha, np.float64)
-        shape = (len(alpha), self.n_splits)
-        out = dict(test=np.zeros(shape), train=np.zeros(shape), fit_ms=np.zeros(shape, np.float32),
-                   score_ms=np.zeros(shape, np.float32))
-        self._check(self._L.gs_ridge(self._h, len(alpha), _ptr(alpha), int(bool(fit_intercept)),
-                                     GS_RETURN_TRAIN if return_train else 0, _ptr(out["test"]), _ptr(out["train"]),
-                                     _ptr(out["fit_ms"]), _ptr(out["score_ms"])))
-        if not return_train:
-            out["train"] = None
-        return out
+        return self._search(len(alpha), return_train, lambda out: self._L.gs_ridge(
+            self._h, len(alpha), _ptr(alpha), int(bool(fit_intercept)), GS_RETURN_TRAIN if return_train else 0,
+            _ptr(out["test"]), _ptr(out["train"]), _ptr(out["fit_ms"]), _ptr(out["score_ms"])))
 
     def ridge_refit(self, alpha, fit_intercept=True):
         coef = np.zeros(self.d + 1)
@@ -313,15 +319,10 @@ class Engine:
     def enet(self, alpha, l1_ratio, fit_intercept=True, tol=1e-4, max_iter=1000, return_train=True):
         alpha = np.ascontiguousarray(alpha, np.float64)
         l1_ratio = np.ascontiguousarray(np.broadcast_to(np.asarray(l1_ratio, np.float64), alpha.shape))
-        shape = (len(alpha), self.n_splits)
-        out = dict(test=np.zeros(shape), train=np.zeros(shape), n_iter=np.zeros(shape, np.int32),
-                   fit_ms=np.zeros(shape, np.float32), score_ms=np.zeros(shape, np.float32))
-        self._check(self._L.gs_enet(self._h, len(alpha), _ptr(alpha), _ptr(l1_ratio), int(bool(fit_intercept)), float(tol),
-                                    int(max_iter), GS_RETURN_TRAIN if return_train else 0, _ptr(out["test"]), _ptr(out["train"]),
-                                    _ptr(out["n_iter"]), _ptr(out["fit_ms"]), _ptr(out["score_ms"])))
-        if not return_train:
-            out["train"] = None
-        return out
+        return self._search(len(alpha), return_train, lambda out: self._L.gs_enet(
+            self._h, len(alpha), _ptr(alpha), _ptr(l1_ratio), int(bool(fit_intercept)), float(tol), int(max_iter),
+            GS_RETURN_TRAIN if return_train else 0, _ptr(out["test"]), _ptr(out["train"]), _ptr(out["n_iter"]),
+            _ptr(out["fit_ms"]), _ptr(out["score_ms"])), ("n_iter",))
 
     def enet_refit(self, alpha, l1_ratio=1.0, fit_intercept=True, tol=1e-4, max_iter=1000):
         coef = np.zeros(self.d + 1)
@@ -333,15 +334,9 @@ class Engine:
 
     def logreg(self, C, tol=1e-4, max_iter=100, fit_intercept=True, return_train=True):
         C = np.ascontiguousarray(C, np.float64)
-        shape = (len(C), self.n_splits)
-        out = dict(test=np.zeros(shape), train=np.zeros(shape), n_iter=np.zeros(shape, np.int32),
-                   fit_ms=np.zeros(shape, np.float32), score_ms=np.zeros(shape, np.float32))
-        self._check(self._L.gs_logreg(self._h, len(C), _ptr(C), float(tol), int(max_iter), int(bool(fit_intercept)),
-                                      GS_RETURN_TRAIN if return_train else 0, _ptr(out["test"]), _ptr(out["train"]),
-                                      _ptr(out["n_iter"]), _ptr(out["fit_ms"]), _ptr(out["score_ms"])))
-        if not return_train:
-            out["train"] = None
-        return out
+        return self._search(len(C), return_train, lambda out: self._L.gs_logreg(
+            self._h, len(C), _ptr(C), float(tol), int(max_iter), int(bool(fit_intercept)), GS_RETURN_TRAIN if return_train else 0,
+            _ptr(out["test"]), _ptr(out["train"]), _ptr(out["n_iter"]), _ptr(out["fit_ms"]), _ptr(out["score_ms"])), ("n_iter",))
 
     def logreg_refit(self, C, tol=1e-4, max_iter=100, fit_intercept=True):
         """-> (coef, intercept, n_iter): binary [d], float; three or more classes (multinomial) [n_classes][d], [n_classes]"""
@@ -357,15 +352,10 @@ class Engine:
     def linsvc(self, C, tol=1e-4, max_iter=1000, fit_intercept=True, intercept_scaling=1.0, return_train=True):
         """LinearSVC (squared hinge, L2, primal TRON) per (candidate, split); n_iter = LinearSVC.n_iter_ of each fit"""
         C = np.ascontiguousarray(C, np.float64)
-        shape = (len(C), self.n_splits)
-        out = dict(test=np.zeros(shape), train=np.zeros(shape), n_iter=np.zeros(shape, np.int32),
-                   fit_ms=np.zeros(shape, np.float32), score_ms=np.zeros(shape, np.float32))
-        self._check(self._L.gs_linsvc(self._h, len(C), _ptr(C), float(tol), int(max_iter), int(bool(fit_intercept)),
-                                      float(intercept_scaling), GS_RETURN_TRAIN if return_train else 0, _ptr(out["test"]),
-                                      _ptr(out["train"]), _ptr(out["n_iter"]), _ptr(out["fit_ms"]), _ptr(out["score_ms"])))
-        if not return_train:
-            out["train"] = None
-        return out
+        return self._search(len(C), return_train, lambda out: self._L.gs_linsvc(
+            self._h, len(C), _ptr(C), float(tol), int(max_iter), int(bool(fit_intercept)), float(intercept_scaling),
+            GS_RETURN_TRAIN if return_train else 0, _ptr(out["test"]), _ptr(out["train"]), _ptr(out["n_iter"]),
+            _ptr(out["fit_ms"]), _ptr(out["score_ms"])), ("n_iter",))
 
     def linsvc_refit(self, C, tol=1e-4, max_iter=1000, fit_intercept=True, intercept_scaling=1.0):
         """-> (raw [rows][d + 1]: liblinear's weights, the bias feature's last; n_iter [rows]); rows = 1 (binary) or n_classes"""
@@ -397,16 +387,12 @@ class Engine:
         epsilon = np.ascontiguousarray(np.broadcast_to(np.asarray(epsilon, np.float64), (n_cand,)))
         solver = np.ascontiguousarray(np.broadcast_to(np.asarray(solver, np.int64), shape), np.int32)
         seed = np.ascontiguousarray(np.broadcast_to(np.asarray(seed, np.int64), shape), np.uint32)
-        out = dict(test=np.zeros(shape), train=np.zeros(shape), n_iter=np.zeros(shape, np.int32),
-                   fit_ms=np.zeros(shape, np.float32), score_ms=np.zeros(shape, np.float32))
         coef = np.zeros(shape + (self.d + 1,)) if return_coef else None
         stats = np.zeros(shape + (3,), np.int64) if return_stats else None
-        self._check(self._L.gs_linsvr(self._h, n_cand, _ptr(C), _ptr(epsilon), _ptr(solver), _ptr(seed), float(tol), int(max_iter),
-                                      int(bool(fit_intercept)), float(intercept_scaling), GS_RETURN_TRAIN if return_train else 0,
-                                      _ptr(out["test"]), _ptr(out["train"]), _ptr(out["n_iter"]), _ptr(out["fit_ms"]),
-                                      _ptr(out["score_ms"]), _ptr(coef), _ptr(stats)))
-        if not return_train:
-            out["train"] = None
+        out = self._search(n_cand, return_train, lambda out: self._L.gs_linsvr(
+            self._h, n_cand, _ptr(C), _ptr(epsilon), _ptr(solver), _ptr(seed), float(tol), int(max_iter), int(bool(fit_intercept)),
+            float(intercept_scaling), GS_RETURN_TRAIN if return_train else 0, _ptr(out["test"]), _ptr(out["train"]),
+            _ptr(out["n_iter"]), _ptr(out["fit_ms"]), _ptr(out["score_ms"]), _ptr(coef), _ptr(stats)), ("n_iter",))
         if return_coef:
             out["coef"] = coef
         if return_stats:
@@ -453,17 +439,13 @@ class Engine:
         kc = self.n_classes if self.n_classes > 2 else 1
         seed = np.ascontiguousarray(np.broadcast_to(np.asarray(seed, np.int64).reshape(n_cand, self.n_splits, -1),
                                                     shape + (kc,)), np.uint32)
-        out = dict(test=np.zeros(shape), train=np.zeros(shape), n_iter=np.zeros(shape, np.int32), status=np.zeros(shape, np.int32),
-                   fit_ms=np.zeros(shape, np.float32), score_ms=np.zeros(shape, np.float32))
         coef = np.zeros(shape + (kc, self.d + 1)) if return_coef else None
         stats = np.zeros(shape + (kc, 3), np.int64) if return_stats else None
-        self._check(self._L.gs_sgd(self._h, n_cand, *[_ptr(a) for a in cands], _ptr(seed), -np.inf if tol is None else float(tol),
-                                   int(max_iter), int(n_iter_no_change), int(bool(fit_intercept)), int(bool(shuffle)),
-                                   GS_RETURN_TRAIN if return_train else 0, _ptr(out["test"]), _ptr(out["train"]),
-                                   _ptr(out["n_iter"]), _ptr(out["status"]), _ptr(out["fit_ms"]), _ptr(out["score_ms"]),
-                                   _ptr(coef), _ptr(stats)))
-        if not return_train:
-            out["train"] = None
+        out = self._search(n_cand, return_train, lambda out: self._L.gs_sgd(
+            self._h, n_cand, *[_ptr(a) for a in cands], _ptr(seed), -np.inf if tol is None else float(tol), int(max_iter),
+            int(n_iter_no_change), int(bool(fit_intercept)), int(bool(shuffle)), GS_RETURN_TRAIN if return_train else 0,
+            _ptr(out["test"]), _ptr(out["train"]), _ptr(out["n_iter"]), _ptr(out["status"]), _ptr(out["fit_ms"]),
+            _ptr(out["score_ms"]), _ptr(coef), _ptr(stats)), ("n_iter", "status"))
         if return_coef:
             out["coef"] = coef
         if return_stats:
@@ -511,17 +493,13 @@ class Engine:
         a, b, st = f64(alpha_scaled), f64(beta_scaled), f64(step)
         lcode = self.SAG_LOSS[loss] if isinstance(loss, str) else int(loss)
         k = self.n_classes if lcode == 1 else 1
-        out = dict(test=np.zeros(shape), train=np.zeros(shape), n_iter=np.zeros(shape, np.int32), status=np.zeros(shape, np.int32),
-                   fit_ms=np.zeros(shape, np.float32), score_ms=np.zeros(shape, np.float32))
         coef = np.zeros(shape + (k, self.d + 1)) if return_coef or lcode == 2 else None
         stats = np.zeros(shape + (2,), np.int64) if return_stats else None
-        self._check(self._L.gs_logreg_sag(self._h, shape[0], _ptr(solver), _ptr(a), _ptr(b), _ptr(st), _ptr(seed), lcode,
-                                          float(tol), int(max_iter), int(bool(fit_intercept)),
-                                          GS_RETURN_TRAIN if return_train else 0, _ptr(out["test"]), _ptr(out["train"]),
-                                          _ptr(out["n_iter"]), _ptr(out["status"]), _ptr(out["fit_ms"]), _ptr(out["score_ms"]),
-                                          _ptr(coef), _ptr(stats)))
-        if not return_train:
-            out["train"] = None
+        out = self._search(shape[0], return_train, lambda out: self._L.gs_logreg_sag(
+            self._h, shape[0], _ptr(solver), _ptr(a), _ptr(b), _ptr(st), _ptr(seed), lcode, float(tol), int(max_iter),
+            int(bool(fit_intercept)), GS_RETURN_TRAIN if return_train else 0, _ptr(out["test"]), _ptr(out["train"]),
+            _ptr(out["n_iter"]), _ptr(out["status"]), _ptr(out["fit_ms"]), _ptr(out["score_ms"]), _ptr(coef), _ptr(stats)),
+            ("n_iter", "status"))
         if coef is not None:
             out["coef"] = coef
         if return_stats:
@@ -552,15 +530,10 @@ class Engine:
         nn = np.ascontiguousarray(n_neighbors, np.int32)
         w = np.ascontiguousarray([KNN_WEIGHTS[v] if isinstance(v, str) else int(v) for v in weights], np.int32)
         m = np.ascontiguousarray([KNN_METRIC[v] if isinstance(v, str) else int(v) for v in metric], np.int32)
-        shape = (len(nn), self.n_splits)
-        out = dict(test=np.zeros(shape), train=np.zeros(shape), fit_ms=np.zeros(shape, np.float32),
-                   score_ms=np.zeros(shape, np.float32))
         fl = (GS_RETURN_TRAIN if return_train else 0) | (GS_TARGET_F32 if y_f32 else 0)
-        self._check(self._L.gs_knn(self._h, len(nn), _ptr(nn), _ptr(w), _ptr(m), fl, _ptr(out["test"]), _ptr(out["train"]),
-                                   _ptr(out["fit_ms"]), _ptr(out["score_ms"])))
-        if not return_train:
-            out["train"] = None
-        return out
+        return self._search(len(nn), return_train, lambda out: self._L.gs_knn(
+            self._h, len(nn), _ptr(nn), _ptr(w), _ptr(m), fl, _ptr(out["test"]), _ptr(out["train"]), _ptr(out["fit_ms"]),
+            _ptr(out["score_ms"])))
 
     # -- test hooks --
     def debug_knn_neighbors(self, metric, k, split):
@@ -582,7 +555,7 @@ class Engine:
         """K [n][n] float32; with return_guard: (K, qd, flag), qd the float64 diagonal (poly / sigmoid, else None) and flag
         the kernel-matrix kernel's guard (1: K holds a zero, subnormal, negative or non-finite value)"""
         K = np.zeros((self.n, self.n), np.float32)
-        k = KERNEL_ID[kernel] if isinstance(kernel, str) else int(kernel)
+        k = _kernel_id(kernel)
         qd = np.zeros(self.n) if return_guard and k in _PARAM_KERNELS else None
         flag = np.zeros(1, np.int32) if return_guard else None
         self._with_kernel_params([k], degree, coef0, lambda: self._check(self._L.gs_debug_kernel_matrix(
@@ -596,7 +569,7 @@ class Engine:
             raise ValueError("debug_decision: coef has %d columns; expected n = %d" % (coef.shape[1], self.n))
         dec = np.zeros_like(coef)
         used = np.zeros(1, np.int32)
-        k = KERNEL_ID[kernel] if isinstance(kernel, str) else int(kernel)
+        k = _kernel_id(kernel)
         self._check(self._L.gs_debug_decision(self._h, k, float(gamma), int(degree), float(coef0), _ptr(coef), coef.shape[0],
                                               int(jchunks), _ptr(dec), _ptr(used)))
         return dec, int(used[0])

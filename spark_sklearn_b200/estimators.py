@@ -1,4 +1,4 @@
-"""Estimator adapters: turn (estimator, candidate dicts, folds) into the scalar tables the C ABI takes,
+"""Estimator plans: turn (estimator, candidate dicts, folds) into the scalar tables the C ABI takes,
 and turn refit buffers back into genuine fitted scikit-learn estimators for ``best_estimator_``
 (reference base_search.py:165-174 delegates ``predict`` & co. to it).
 
@@ -96,37 +96,26 @@ class Folds:
             return self.fold_id != k
         return (self.masks[1][:, k >> 6] >> np.uint64(k & 63)) & np.uint64(1) == 1
 
+    def test_rows(self, k):
+        """boolean [n]: the test rows of split k"""
+        if self.fold_id is not None:
+            return self.fold_id == k
+        return (self.masks[0][:, k >> 6] >> np.uint64(k & 63)) & np.uint64(1) == 1
+
 
 def adapter_for(estimator):
+    """The plan class of an estimator: plan(estimator, cands, X, y, fold_id, n_splits, device=None), multi_device, scorers"""
     from sklearn.linear_model import ElasticNet, Lasso, LogisticRegression, Ridge, SGDClassifier, SGDRegressor
     from sklearn.neighbors import KNeighborsClassifier, KNeighborsRegressor
     from sklearn.pipeline import Pipeline
     from sklearn.svm import SVC, SVR, LinearSVC, LinearSVR, NuSVC, NuSVR
+    plans = {SVC: SVCPlan, SVR: SVRPlan, NuSVC: NuSVCPlan, NuSVR: NuSVRPlan, Ridge: RidgePlan, Lasso: ENetPlan,
+             ElasticNet: ENetPlan, LogisticRegression: LogRegPlan, LinearSVC: LinearSVCPlan, LinearSVR: LinearSVRPlan,
+             SGDClassifier: SGDPlan, SGDRegressor: SGDRegressorPlan, KNeighborsClassifier: KNeighborsPlan,
+             KNeighborsRegressor: KNeighborsRegressorPlan}
     t = type(estimator)
-    if t is SVC:
-        return SVCAdapter
-    if t is SVR:
-        return SVRAdapter
-    if t is NuSVC:
-        return NuSVCAdapter
-    if t is NuSVR:
-        return NuSVRAdapter
-    if t is Ridge:
-        return RidgeAdapter
-    if t is LogisticRegression:
-        return LogRegAdapter
-    if t in (Lasso, ElasticNet):
-        return ENetAdapter
-    if t is LinearSVC:
-        return LinearSVCAdapter
-    if t is LinearSVR:
-        return LinearSVRAdapter
-    if t is SGDClassifier:
-        return SGDClassifierAdapter
-    if t is SGDRegressor:
-        return SGDRegressorAdapter
-    if t in (KNeighborsClassifier, KNeighborsRegressor):
-        return KNeighborsAdapter if t is KNeighborsClassifier else KNeighborsRegressorAdapter
+    if t in plans:
+        return plans[t]
     if t is Pipeline and len(estimator.steps) == 1:
         # the reference's own search tests wrap the estimator in a one-step Pipeline and search 'step__param'
         # (python/spark_sklearn/tests/test_search_2.py:69-93): the step's adapter runs, the names are translated
@@ -149,27 +138,169 @@ def _as_matrix(X):
     return np.ascontiguousarray(X, np.float64)        # scikit-learn upcasts everything else to float64
 
 
-def _pad_scores(arr_list, my):
-    return None if not my else np.concatenate(arr_list, 0)
-
-
 # scoring= names with a fused CUDA scorer (include/b200gs.h GS_SCORE_*); None = the estimator's own score
 CLASSIFICATION_SCORERS = {None: 0, "accuracy": 0, "balanced_accuracy": 1, "f1": 2, "precision": 3, "recall": 4, "roc_auc": 5,
                           "f1_macro": 6, "f1_micro": 7, "f1_weighted": 8}
 REGRESSION_SCORERS = {None: 0, "r2": 0, "neg_mean_squared_error": 16, "neg_root_mean_squared_error": 17}
 
 
+_INT_MAX = int(np.iinfo("i").max)
+_SEED_LOCK = threading.Lock()
+
+
+def _random_state(random_state):
+    """check_random_state(random_state) as one fit sees it: an int or a RandomState gives every fit the same draws (clone
+    deep-copies the parameter, so the caller's RandomState is not advanced); None draws from numpy's global RandomState."""
+    from sklearn.utils import check_random_state
+    if random_state is not None and not isinstance(random_state, (numbers.Integral, np.random.RandomState)):
+        raise ValueError("%r cannot be used to seed a numpy.random.RandomState instance" % (random_state,))
+    return check_random_state(copy.deepcopy(random_state) if isinstance(random_state, np.random.RandomState) else random_state)
+
+
+def fit_seed(random_state, low):
+    """The seed of one fit: check_random_state(random_state).randint(low, np.iinfo('i').max).  low 0: the seed
+    _fit_liblinear hands to liblinear; low 1: make_dataset's seed of a LogisticRegression(solver='sag' | 'saga') fit."""
+    return int(_random_state(random_state).randint(low, _INT_MAX))
+
+
+def _class_weight_key(cw):
+    """class_weight as a group key: None, 'balanced' or the sorted items of a dict"""
+    return cw if cw is None or isinstance(cw, str) else tuple(sorted(cw.items()))
+
+
+def _target_1d(y, name):
+    """scikit-learn's column_or_1d(y, warn=True): a column vector is raveled with a DataConversionWarning"""
+    y = np.asarray(y)
+    if y.ndim == 2 and y.shape[1] == 1:
+        from sklearn.exceptions import DataConversionWarning
+        warnings.warn("A column-vector y was passed when a 1d array was expected. Please change the shape of y to "
+                      "(n_samples, ), for example using ravel().", DataConversionWarning, stacklevel=3)
+        y = y[:, 0]
+    if y.ndim != 1:
+        raise ValueError("%s needs a 1d target; got y of shape %r" % (name, y.shape))
+    return y
+
+
+def _overflow(epoch):
+    """the ValueError of an SGD or SAG fit that went non-finite"""
+    return ValueError("Floating-point under-/overflow occurred at epoch #%d. Scaling input data with StandardScaler or "
+                      "MinMaxScaler might help." % epoch)
+
+
 class _Plan:
+    """One search of one estimator on one device.  A plan class is its own adapter: adapter_for(estimator).plan(...).
+    Each plan checks its candidates (_candidate) and makes one engine call per group of candidates (_search); evaluate
+    does the rest."""
+    multi_device = True        # plan(..., device=d): one plan per GPU of the in-process scheduler
+    scorers = {None: 0}
+    class_weighted = False     # the estimator has class_weight: one gs_set_class_weight per group
+    fail_warning = None        # fits can fail (SGD, SAG): the warning that gives them error_score
+    _seed = None               # random_state -> one fit's seeds: the plan draws a seed table (_seed_table)
+
+    @classmethod
+    def plan(cls, estimator, cands, X, y, fold_id, n_splits, device=None):
+        return cls(estimator, cands, X, y, fold_id, n_splits, device)
+
     def __init__(self, estimator, cands, X, y, fold_id, n_splits, device=None):
         self.estimator, self.cands = estimator, cands
         self.X, self.y, self.n_splits = _as_matrix(X), y, n_splits
         if isinstance(fold_id, Folds):
             self.folds, self.fold_id = fold_id, fold_id.fold_id
-        else:
+        else:                                             # a bare fold_id array: the splits are a partition
             self.folds, self.fold_id = None, fold_id
         self.engine = get_engine(device)
         self._prof = {}
+        self._seeds = None
         self.score_kind, self.score_pos = 0, 1
+
+    def _candidate(self, p, error_score):
+        """check one candidate's parameters p -> (group key, engine-call values)"""
+        raise NotImplementedError
+
+    def _prepare(self, my, error_score):
+        """every candidate of my checked, before any device work -> ([(params, group key, values)], the [len(my)][n_splits]
+        fits that fail on the host, or None)"""
+        prepared = []
+        for ci in my:
+            p = self._base_params(self.cands[ci])
+            prepared.append((p,) + tuple(self._candidate(p, error_score)))
+        return prepared, None
+
+    def _search(self, key, values, cands, return_train):
+        """one engine call for the candidates cands (indices into self.cands) of one group -> the engine's outputs"""
+        raise NotImplementedError
+
+    def _undefined(self):
+        """[n_splits] bool: the splits whose test score scikit-learn itself leaves NaN (None: none)"""
+        return None
+
+    def evaluate(self, my, return_train=True, error_score='raise'):
+        """the (candidate, split) fits of the candidates my: one engine call per group of candidates that share the call's
+        settings (and class weights), groups in order of first appearance"""
+        prepared, failed = self._prepare(my, error_score)
+        if self._seed is not None:
+            self._seed_table()
+        groups = {}
+        for j, (p, key, _) in enumerate(prepared):
+            cwk = _class_weight_key(p.get("class_weight")) if self.class_weighted else None
+            groups.setdefault((key, cwk), []).append(j)
+        shape = (len(my), self.n_splits)
+        res = dict(test=np.zeros(shape), train=np.zeros(shape), fit_ms=np.zeros(shape), score_ms=np.zeros(shape))
+        prof = {}
+        try:
+            for (key, _), idx in groups.items():
+                if self.class_weighted:
+                    self._set_class_weight(prepared[idx[0]][0].get("class_weight"))
+                self.engine.set_scoring(self.score_kind, self.score_pos)
+                r = self._search(key, [prepared[j][2] for j in idx], [my[j] for j in idx], return_train)
+                for k, v in r.items():
+                    if v is None:
+                        continue
+                    if k not in res:                          # n_iter, status, per-fit counters: int64
+                        res[k] = np.zeros(shape + v.shape[2:], np.float64 if v.dtype.kind == "f" else np.int64)
+                    res[k][idx] = v
+                for k, v in self.engine.profile().items():
+                    prof[k] = prof.get(k, 0) + v
+        finally:
+            if self.class_weighted:
+                self.engine.set_class_weight(None)
+        self._prof = prof
+        for k in ("n_iter", "stats", "cd_stats"):
+            if k in res:
+                setattr(self, k + "_", res[k])
+        bad = np.zeros(shape, bool) if failed is None else failed
+        if "status" in res:
+            bad = bad | (res["status"] == 2)                  # the engine's non-finite fits
+        if bad.any():
+            if self.fail_warning is None:
+                fill = np.nan                                 # k-NN: NaN, which _finish reports
+            elif error_score == 'raise':
+                j, k = map(int, np.argwhere(bad)[0])
+                raise _overflow(int(res["n_iter"][j, k]))
+            else:
+                warnings.warn(self.fail_warning % (int(bad.sum()), error_score))
+                fill = error_score
+            res["test"][bad] = fill
+            res["train"][bad] = fill
+        return self._finish(res, return_train, error_score, self._undefined())
+
+    def _seed_table(self):
+        """The seeds of every fit of the search, [n_cand][n_splits] + the shape of one fit's seeds, drawn as scikit-learn's
+        GridSearchCV draws them: candidate-major, split-minor, random_state=None from numpy's global RandomState.  A search
+        whose candidates draw from the global RandomState computes the table once for all of its per-GPU plans (they share
+        the Folds); the plan keeps it."""
+        if self._seeds is None:
+            states = [self._base_params(c)["random_state"] for c in self.cands]
+            draw = lambda: np.array([[self._seed(rs) for _ in range(self.n_splits)] if rs is None
+                                     else [self._seed(rs)] * self.n_splits for rs in states], np.int64)
+            if any(rs is None for rs in states) and self.folds is not None:
+                with _SEED_LOCK:
+                    if getattr(self.folds, "_search_seeds", None) is None:
+                        self.folds._search_seeds = draw()
+                    self._seeds = self.folds._search_seeds
+            else:
+                self._seeds = draw()
+        return self._seeds
 
     def profile(self):
         return dict(self._prof)
@@ -223,11 +354,14 @@ class _Plan:
         return w[0]
 
     def _train_rows(self, k):
+        """boolean [n]: the training rows of split k (all rows for k < 0)"""
         if self.folds is not None:
             return self.folds.train_rows(k)
         return self.fold_id != k if k >= 0 else np.ones(len(self.fold_id), bool)
 
-    scorers = {None: 0}
+    def _test_rows(self, k):
+        """boolean [n]: the test rows of split k"""
+        return self.folds.test_rows(k) if self.folds is not None else self.fold_id == k
 
     def set_scoring(self, scoring):
         """reference base_search.py:43: check_scoring(estimator, scoring).  Only scorers with a fused CUDA path are accepted
@@ -266,7 +400,7 @@ class _Plan:
         p.update(cand)
         return p
 
-    def _finish(self, res, return_train, error_score, n_my, undefined=None):
+    def _finish(self, res, return_train, error_score, undefined=None):
         """undefined: [n_splits] bool, the splits whose test score scikit-learn itself leaves NaN (kept, not an error)"""
         test, train = res["test"], res.get("train")
         bad = ~np.isfinite(test)
@@ -284,15 +418,6 @@ class _Plan:
 
 
 # ------------------------------------------------------------------ SVC -----------------------
-class SVCAdapter:
-    multi_device = True        # plan(..., device=d): one plan per GPU of the in-process scheduler
-    scorers = CLASSIFICATION_SCORERS
-
-    @staticmethod
-    def plan(estimator, cands, X, y, fold_id, n_splits, device=None):
-        return SVCPlan(estimator, cands, X, y, fold_id, n_splits, device)
-
-
 class _KernelGamma:
     """What the SVC and SVR plans share: the gamma of one libsvm fit (sklearn svm/_base.py:278-286) and the Gram mode."""
 
@@ -312,6 +437,10 @@ class _KernelGamma:
             raise ValueError("gamma must be >= 0 or 'scale'/'auto'; got %r" % (g,))
         return float(g)
 
+    def _gammas(self, p, kernels):
+        """[n_splits] gamma of candidate p's fits: 0 unless its kernel is one of kernels"""
+        return [self._gamma(p["gamma"], k) if p["kernel"] in kernels else 0.0 for k in range(self.n_splits)]
+
     def _nu_kw(self):
         """engine keyword of the nu solvers (NuSVCPlan / NuSVRPlan set nu = True)"""
         return {"nu": True} if self.nu else {}
@@ -326,6 +455,7 @@ class SVCPlan(_KernelGamma, _Plan):
     """sklearn.svm.SVC (C-SVC).  Scalars per candidate: kernel, C, gamma (resolved per fold for every kernel but linear),
     degree and coef0 (poly, sigmoid)."""
     scorers = CLASSIFICATION_SCORERS
+    class_weighted = True
 
     def __init__(self, estimator, cands, X, y, fold_id, n_splits, device=None):
         super().__init__(estimator, cands, X, y, fold_id, n_splits, device)
@@ -376,42 +506,16 @@ class SVCPlan(_KernelGamma, _Plan):
             return None                                 # invalid candidates are reported by evaluate()
         return out
 
-    def evaluate(self, my, return_train=True, error_score='raise'):
-        ns = self.n_splits
-        shape = (len(my), ns)
-        res = dict(test=np.zeros(shape), train=np.zeros(shape), fit_ms=np.zeros(shape), score_ms=np.zeros(shape),
-                   n_iter=np.zeros(shape, np.int64))
-        groups = {}
-        params = []
-        for j, ci in enumerate(my):
-            p = self._base_params(self.cands[ci])
-            self._check(p)
-            params.append(p)
-            cw = p.get("class_weight")
-            cwk = None if cw is None else (cw if isinstance(cw, str) else tuple(sorted(cw.items())))
-            groups.setdefault((float(p["tol"]), int(p["max_iter"]), bool(p["shrinking"]), cwk), []).append(j)
-        prof = {}
-        for (tol, max_iter, shrinking, _cwk), idx in groups.items():
-            self._set_class_weight(params[idx[0]].get("class_weight"))
-            kern = [params[j]["kernel"] for j in idx]
-            C = [float(params[j][self.penalty]) for j in idx]
-            gam = np.array([[self._gamma(params[j]["gamma"], k) if params[j]["kernel"] != "linear" else 0.0
-                             for k in range(ns)] for j in idx])
-            self.engine.set_scoring(self.score_kind, self.score_pos)
-            r = self.engine.svc(kern, C, gam, tol=tol, max_iter=max_iter, shrinking=shrinking,
-                                return_train=return_train, flags=self._flags(),
-                                degree=[int(params[j]["degree"]) for j in idx], coef0=[float(params[j]["coef0"]) for j in idx],
-                                **self._nu_kw())
-            for key in ("test", "fit_ms", "score_ms", "n_iter"):
-                res[key][idx] = r[key]
-            if return_train:
-                res["train"][idx] = r["train"]
-            for k, v in self.engine.profile().items():
-                prof[k] = prof.get(k, 0) + v
-        self.engine.set_class_weight(None)
-        self._prof = prof
-        self.n_iter_ = res["n_iter"]
-        return self._finish(res, return_train, error_score, len(my))
+    def _candidate(self, p, error_score):
+        self._check(p)
+        return (float(p["tol"]), int(p["max_iter"]), bool(p["shrinking"])), (p, self._gammas(p, ("rbf", "poly", "sigmoid")))
+
+    def _search(self, key, values, cands, return_train):
+        tol, max_iter, shrinking = key
+        ps = [p for p, _ in values]
+        return self.engine.svc([p["kernel"] for p in ps], [float(p[self.penalty]) for p in ps], np.array([g for _, g in values]),
+                               tol=tol, max_iter=max_iter, shrinking=shrinking, return_train=return_train, flags=self._flags(),
+                               degree=[int(p["degree"]) for p in ps], coef0=[float(p["coef0"]) for p in ps], **self._nu_kw())
 
     def refit(self, best_params):
         p = self._base_params(best_params)
@@ -473,12 +577,6 @@ def materialize_svc(est, X, y_class, classes, pair_coef, rho, n_iter, gamma):
 
 
 # ------------------------------------------------------------------ NuSVC ---------------------
-class NuSVCAdapter(SVCAdapter):
-    @staticmethod
-    def plan(estimator, cands, X, y, fold_id, n_splits, device=None):
-        return NuSVCPlan(estimator, cands, X, y, fold_id, n_splits, device)
-
-
 class NuSVCPlan(SVCPlan):
     """sklearn.svm.NuSVC (libsvm's nu-SVC): SVCPlan with nu in place of C.  class_weight is accepted and reported in
     class_weight_ but, as in libsvm, does not change a nu-SVC fit."""
@@ -498,14 +596,12 @@ class NuSVCPlan(SVCPlan):
     def costs(self):
         return None                                           # no iteration model for nu-SVC: candidates are dealt uniformly
 
-    def evaluate(self, my, return_train=True, error_score='raise'):
+    def _candidate(self, p, error_score):
         if error_score == 'raise':                            # scikit-learn's fit raises before any solve
-            for ci in my:
-                p = self._base_params(self.cands[ci])
-                self._check(p)
-                if any(self._infeasible(float(p["nu"]), k) for k in range(self.n_splits)):
-                    raise ValueError("specified nu is infeasible")
-        return super().evaluate(my, return_train, error_score)
+            self._check(p)
+            if any(self._infeasible(float(p["nu"]), k) for k in range(self.n_splits)):
+                raise ValueError("specified nu is infeasible")
+        return super()._candidate(p, error_score)
 
     def refit(self, best_params):
         p = self._base_params(best_params)
@@ -516,15 +612,6 @@ class NuSVCPlan(SVCPlan):
 
 
 # ------------------------------------------------------------------ SVR -----------------------
-class SVRAdapter:
-    multi_device = True        # plan(..., device=d): one plan per GPU of the in-process scheduler
-    scorers = REGRESSION_SCORERS
-
-    @staticmethod
-    def plan(estimator, cands, X, y, fold_id, n_splits, device=None):
-        return SVRPlan(estimator, cands, X, y, fold_id, n_splits, device)
-
-
 class SVRPlan(_KernelGamma, _Plan):
     """sklearn.svm.SVR (epsilon-SVR).  Scalars per candidate: kernel, C, epsilon, gamma (resolved per fold).  Each fit runs
     libsvm's solver on its training rows in ascending row order, as scikit-learn's X[train] does for KFold-like splitters."""
@@ -534,15 +621,7 @@ class SVRPlan(_KernelGamma, _Plan):
         super().__init__(estimator, cands, X, y, fold_id, n_splits, device)
         if y is None:
             raise ValueError("SVR needs y")
-        y = np.asarray(y)
-        if y.ndim == 2 and y.shape[1] == 1:               # scikit-learn: column_or_1d(y, warn=True)
-            from sklearn.exceptions import DataConversionWarning
-            warnings.warn("A column-vector y was passed when a 1d array was expected. Please change the shape of y to "
-                          "(n_samples, ), for example using ravel().", DataConversionWarning, stacklevel=2)
-            y = y[:, 0]
-        if y.ndim != 1:
-            raise ValueError("SVR needs a 1d target; got y of shape %r" % (y.shape,))
-        self.y = y.astype(np.float64)                     # scikit-learn fits SVR on float64 y
+        self.y = _target_1d(y, "SVR").astype(np.float64)  # scikit-learn fits SVR on float64 y
         self._set_data(self.X, y_target=self.y.astype(np.float32))
         self.engine.set_targets_f64(self.y)
 
@@ -572,39 +651,21 @@ class SVRPlan(_KernelGamma, _Plan):
         """the refit trains on every row: raise before the search when that fit is too large"""
         self._check_rows(-1)
 
-    def evaluate(self, my, return_train=True, error_score='raise'):
-        ns = self.n_splits
-        shape = (len(my), ns)
-        res = dict(test=np.zeros(shape), train=np.zeros(shape), fit_ms=np.zeros(shape), score_ms=np.zeros(shape),
-                   n_iter=np.zeros(shape, np.int64))
-        for k in range(ns):
+    def _prepare(self, my, error_score):
+        for k in range(self.n_splits):
             self._check_rows(k)
-        groups = {}
-        params = []
-        for j, ci in enumerate(my):
-            p = self._base_params(self.cands[ci])
-            self._check(p)
-            params.append(p)
-            groups.setdefault((float(p["tol"]), int(p["max_iter"]), bool(p["shrinking"])), []).append(j)
-        prof = {}
-        for (tol, max_iter, shrinking), idx in groups.items():
-            kern = [params[j]["kernel"] for j in idx]
-            C = [float(params[j]["C"]) for j in idx]
-            eps = [float(params[j][self.tube]) for j in idx]
-            gam = np.array([[self._gamma(params[j]["gamma"], k) if params[j]["kernel"] == "rbf" else 0.0
-                             for k in range(ns)] for j in idx])
-            self.engine.set_scoring(self.score_kind, self.score_pos)
-            r = self.engine.svr(kern, C, eps, gam, tol=tol, max_iter=max_iter, shrinking=shrinking,
-                                return_train=return_train, flags=self._flags(), **self._nu_kw())
-            for key in ("test", "fit_ms", "score_ms", "n_iter"):
-                res[key][idx] = r[key]
-            if return_train:
-                res["train"][idx] = r["train"]
-            for k, v in self.engine.profile().items():
-                prof[k] = prof.get(k, 0) + v
-        self._prof = prof
-        self.n_iter_ = res["n_iter"]
-        return self._finish(res, return_train, error_score, len(my))
+        return super()._prepare(my, error_score)
+
+    def _candidate(self, p, error_score):
+        self._check(p)
+        return (float(p["tol"]), int(p["max_iter"]), bool(p["shrinking"])), (p, self._gammas(p, ("rbf",)))
+
+    def _search(self, key, values, cands, return_train):
+        tol, max_iter, shrinking = key
+        ps = [p for p, _ in values]
+        return self.engine.svr([p["kernel"] for p in ps], [float(p["C"]) for p in ps], [float(p[self.tube]) for p in ps],
+                               np.array([g for _, g in values]), tol=tol, max_iter=max_iter, shrinking=shrinking,
+                               return_train=return_train, flags=self._flags(), **self._nu_kw())
 
     def refit(self, best_params):
         p = self._base_params(best_params)
@@ -652,12 +713,6 @@ def materialize_svr(est, X, coef, rho, n_iter, gamma):
 
 
 # ------------------------------------------------------------------ NuSVR ---------------------
-class NuSVRAdapter(SVRAdapter):
-    @staticmethod
-    def plan(estimator, cands, X, y, fold_id, n_splits, device=None):
-        return NuSVRPlan(estimator, cands, X, y, fold_id, n_splits, device)
-
-
 class NuSVRPlan(SVRPlan):
     """sklearn.svm.NuSVR (libsvm's nu-SVR): SVRPlan with nu in place of epsilon; materialize_svr builds the fitted NuSVR."""
     nu = True
@@ -668,15 +723,6 @@ class NuSVRPlan(SVRPlan):
 
 
 # ------------------------------------------------------------------ Ridge ---------------------
-class RidgeAdapter:
-    multi_device = True        # plan(..., device=d): one plan per GPU of the in-process scheduler
-    scorers = REGRESSION_SCORERS
-
-    @staticmethod
-    def plan(estimator, cands, X, y, fold_id, n_splits, device=None):
-        return RidgePlan(estimator, cands, X, y, fold_id, n_splits, device)
-
-
 class RidgePlan(_Plan):
     scorers = REGRESSION_SCORERS
     supports_sample_weight = True
@@ -698,13 +744,7 @@ class RidgePlan(_Plan):
         """r2 of a test set of fewer than two rows is NaN (r2_score: UndefinedMetricWarning), as in scikit-learn's search"""
         if self.score_kind != 0:
             return None
-        f = self.folds
-        if f is None or f.partition:
-            fid = np.asarray(self.fold_id)
-            n_test = np.bincount(fid[fid >= 0], minlength=self.n_splits)
-        else:
-            n_test = np.array([((f.masks[0][:, k >> 6] >> np.uint64(k & 63)) & np.uint64(1)).sum() for k in range(f.n_splits)])
-        return n_test < 2
+        return np.array([np.count_nonzero(self._test_rows(k)) < 2 for k in range(self.n_splits)])
 
     def _check(self, p):
         if p.get("solver", "auto") not in ("auto", "cholesky"):
@@ -714,27 +754,12 @@ class RidgePlan(_Plan):
         if not (isinstance(p["alpha"], numbers.Real) and p["alpha"] >= 0):
             raise ValueError("alpha must be a non-negative number; got %r" % (p["alpha"],))
 
-    def evaluate(self, my, return_train=True, error_score='raise'):
-        shape = (len(my), self.n_splits)
-        res = dict(test=np.zeros(shape), train=np.zeros(shape), fit_ms=np.zeros(shape), score_ms=np.zeros(shape))
-        groups = {}
-        for j, ci in enumerate(my):
-            p = self._base_params(self.cands[ci])
-            self._check(p)
-            groups.setdefault(bool(p["fit_intercept"]), []).append((j, float(p["alpha"])))
-        prof = {}
-        for fi, items in groups.items():
-            idx = [j for j, _ in items]
-            self.engine.set_scoring(self.score_kind, self.score_pos)
-            r = self.engine.ridge([a for _, a in items], fit_intercept=fi, return_train=return_train)
-            for key in ("test", "fit_ms", "score_ms"):
-                res[key][idx] = r[key]
-            if return_train:
-                res["train"][idx] = r["train"]
-            for k, v in self.engine.profile().items():
-                prof[k] = prof.get(k, 0) + v
-        self._prof = prof
-        return self._finish(res, return_train, error_score, len(my), self._undefined())
+    def _candidate(self, p, error_score):
+        self._check(p)
+        return bool(p["fit_intercept"]), float(p["alpha"])
+
+    def _search(self, fit_intercept, alpha, cands, return_train):
+        return self.engine.ridge(alpha, fit_intercept=fit_intercept, return_train=return_train)
 
     def refit(self, best_params):
         p = self._base_params(best_params)
@@ -751,15 +776,6 @@ class RidgePlan(_Plan):
 
 
 # ------------------------------------------------------------------ Lasso / ElasticNet -------
-class ENetAdapter:
-    multi_device = True
-    scorers = REGRESSION_SCORERS
-
-    @staticmethod
-    def plan(estimator, cands, X, y, fold_id, n_splits, device=None):
-        return ENetPlan(estimator, cands, X, y, fold_id, n_splits, device)
-
-
 class ENetPlan(RidgePlan):
     """sklearn.linear_model.Lasso / ElasticNet on the fold Grams of the Ridge path: cyclic coordinate descent with
     scikit-learn's stopping rule (linear_model/_cd_fast.pyx:243-506) in the Gram domain, csrc/linear.cu enet_cd_kernel."""
@@ -788,31 +804,14 @@ class ENetPlan(RidgePlan):
         if self.X.shape[1] > 1024:
             raise NotImplementedError("more than 1024 features is not supported by the coordinate-descent kernel")
 
-    def evaluate(self, my, return_train=True, error_score='raise'):
-        shape = (len(my), self.n_splits)
-        res = dict(test=np.zeros(shape), train=np.zeros(shape), fit_ms=np.zeros(shape), score_ms=np.zeros(shape),
-                   n_iter=np.zeros(shape, np.int64))
-        groups = {}
-        for j, ci in enumerate(my):
-            p = self._base_params(self.cands[ci])
-            self._check(p)
-            key = (bool(p["fit_intercept"]), float(p["tol"]), int(p["max_iter"]))
-            groups.setdefault(key, []).append((j, float(p["alpha"]), float(p.get("l1_ratio", 1.0))))
-        prof = {}
-        for (fi, tol, max_iter), items in groups.items():
-            idx = [j for j, _, _ in items]
-            self.engine.set_scoring(self.score_kind, self.score_pos)
-            r = self.engine.enet([a for _, a, _ in items], [l for _, _, l in items], fit_intercept=fi, tol=tol,
-                                 max_iter=max_iter, return_train=return_train)
-            for key in ("test", "fit_ms", "score_ms", "n_iter"):
-                res[key][idx] = r[key]
-            if return_train:
-                res["train"][idx] = r["train"]
-            for k, v in self.engine.profile().items():
-                prof[k] = prof.get(k, 0) + v
-        self._prof = prof
-        self.n_iter_ = res["n_iter"]
-        return self._finish(res, return_train, error_score, len(my), self._undefined())
+    def _candidate(self, p, error_score):
+        self._check(p)
+        return (bool(p["fit_intercept"]), float(p["tol"]), int(p["max_iter"])), (float(p["alpha"]), float(p.get("l1_ratio", 1.0)))
+
+    def _search(self, key, values, cands, return_train):
+        fi, tol, max_iter = key
+        return self.engine.enet([a for a, _ in values], [l for _, l in values], fit_intercept=fi, tol=tol, max_iter=max_iter,
+                                return_train=return_train)
 
     def refit(self, best_params):
         p = self._base_params(best_params)
@@ -872,12 +871,13 @@ class _PipelinePlan:
 
 
 # ------------------------------------------------------------------ LogisticRegression --------
-class LogRegAdapter:
-    multi_device = True        # plan(..., device=d): one plan per GPU of the in-process scheduler
+class LogRegPlan(_Plan):
     scorers = CLASSIFICATION_SCORERS
+    supports_sample_weight = True
+    class_weighted = True
 
-    @staticmethod
-    def plan(estimator, cands, X, y, fold_id, n_splits, device=None):
+    @classmethod
+    def plan(cls, estimator, cands, X, y, fold_id, n_splits, device=None):
         """lbfgs candidates run LogRegPlan, sag / saga candidates LogRegSAGPlan; one search runs one of the two"""
         base = estimator.get_params(deep=False).get("solver", "lbfgs")
         solvers = {c.get("solver", base) for c in cands} or {base}
@@ -886,12 +886,7 @@ class LogRegAdapter:
                 raise NotImplementedError("LogisticRegression: a search that mixes solver='sag' / 'saga' with %s has no CUDA path "
                                           "(search the two in separate searches)" % sorted(solvers - {"sag", "saga"}))
             return LogRegSAGPlan(estimator, cands, X, y, fold_id, n_splits, device)
-        return LogRegPlan(estimator, cands, X, y, fold_id, n_splits, device)
-
-
-class LogRegPlan(_Plan):
-    scorers = CLASSIFICATION_SCORERS
-    supports_sample_weight = True
+        return cls(estimator, cands, X, y, fold_id, n_splits, device)
 
     def __init__(self, estimator, cands, X, y, fold_id, n_splits, device=None):
         super().__init__(estimator, cands, X, y, fold_id, n_splits, device)
@@ -916,32 +911,13 @@ class LogRegPlan(_Plan):
         if not (isinstance(p["C"], numbers.Real) and p["C"] > 0):
             raise ValueError("C must be a positive number; got %r" % (p["C"],))
 
-    def evaluate(self, my, return_train=True, error_score='raise'):
-        shape = (len(my), self.n_splits)
-        res = dict(test=np.zeros(shape), train=np.zeros(shape), fit_ms=np.zeros(shape), score_ms=np.zeros(shape))
-        groups = {}
-        for j, ci in enumerate(my):
-            p = self._base_params(self.cands[ci])
-            self._check(p)
-            cw = p.get("class_weight")
-            cwk = None if cw is None else (cw if isinstance(cw, str) else tuple(sorted(cw.items())))
-            groups.setdefault((float(p["tol"]), int(p["max_iter"]), bool(p["fit_intercept"]), cwk), []).append((j, float(p["C"]), cw))
-        prof = {}
-        for (tol, mi, fi, _cwk), items in groups.items():
-            idx = [j for j, _, _ in items]
-            self._set_class_weight(items[0][2])
-            self.engine.set_scoring(self.score_kind, self.score_pos)
-            r = self.engine.logreg([c for _, c, _ in items], tol=tol, max_iter=mi, fit_intercept=fi,
-                                   return_train=return_train)
-            for key in ("test", "fit_ms", "score_ms"):
-                res[key][idx] = r[key]
-            if return_train:
-                res["train"][idx] = r["train"]
-            for k, v in self.engine.profile().items():
-                prof[k] = prof.get(k, 0) + v
-        self.engine.set_class_weight(None)
-        self._prof = prof
-        return self._finish(res, return_train, error_score, len(my))
+    def _candidate(self, p, error_score):
+        self._check(p)
+        return (float(p["tol"]), int(p["max_iter"]), bool(p["fit_intercept"])), float(p["C"])
+
+    def _search(self, key, C, cands, return_train):
+        tol, max_iter, fit_intercept = key
+        return self.engine.logreg(C, tol=tol, max_iter=max_iter, fit_intercept=fit_intercept, return_train=return_train)
 
     def refit(self, best_params):
         p = self._base_params(best_params)
@@ -962,17 +938,6 @@ class LogRegPlan(_Plan):
         return est
 
 
-def sag_seed(random_state):
-    """make_dataset's draw for one LogisticRegression(solver='sag' | 'saga') fit: check_random_state(random_state).randint(1,
-    np.iinfo(np.int32).max).  An int or a RandomState gives the same seed to every fit (clone deep-copies the parameter, so
-    the caller's RandomState is not advanced); None draws from numpy's global RandomState."""
-    from sklearn.utils import check_random_state
-    if random_state is not None and not isinstance(random_state, (numbers.Integral, np.random.RandomState)):
-        raise ValueError("%r cannot be used to seed a numpy.random.RandomState instance" % (random_state,))
-    rs = copy.deepcopy(random_state) if isinstance(random_state, np.random.RandomState) else random_state
-    return int(check_random_state(rs).randint(1, _INT_MAX))
-
-
 class LogRegSAGPlan(_Plan):
     """sklearn.linear_model.LogisticRegression(solver='sag' | 'saga') (csrc/sag.cu): sag_solver restated step for step, one
     warp per (candidate, split) fit.  X reaches the device dense in its own dtype (float32 runs sag32, float64 sag64, as
@@ -980,6 +945,9 @@ class LogRegSAGPlan(_Plan):
     fit's training rows, which reach the device in the splitter's order (the sample draws index them)."""
     scorers = CLASSIFICATION_SCORERS
     supports_sample_weight = True
+    class_weighted = True
+    fail_warning = ("%d fits failed (a floating-point under-/overflow, or step_size * alpha_scaled == 1); their scores are "
+                    "error_score=%r")
     max_coef = 512             # features x weight rows held in registers (include/b200gs.h GS_SAG_MAX_COEF)
 
     def __init__(self, estimator, cands, X, y, fold_id, n_splits, device=None):
@@ -1004,7 +972,6 @@ class LogRegSAGPlan(_Plan):
         self._set_data(self.X, y_class=self.y_class.astype(np.int32))
         if self.folds is not None:
             self.engine.set_train_order(self.folds.train_order)
-        self._seeds = None
         self._mss = {}
 
     def _resolve(self, p):
@@ -1077,76 +1044,41 @@ class LogRegSAGPlan(_Plan):
         sw = np.ones(int(rows.sum())) if sw is None else sw[rows]
         return compute_class_weight(cw, classes=self.classes, y=np.asarray(self.y)[rows], sample_weight=sw.astype(self.X.dtype))
 
-    def _draw_seeds(self, states):
-        table = np.zeros((len(states), self.n_splits), np.int64)
-        for c, rs in enumerate(states):
-            if rs is None:
-                for k in range(self.n_splits):
-                    table[c, k] = sag_seed(None)
-            else:
-                table[c, :] = sag_seed(rs)
-        return table
+    def _seed(self, random_state):
+        return fit_seed(random_state, 1)
 
-    def evaluate(self, my, return_train=True, error_score='raise'):
-        ns = self.n_splits
-        shape = (len(my), ns)
-        res = dict(test=np.zeros(shape), train=np.zeros(shape), fit_ms=np.zeros(shape), score_ms=np.zeros(shape),
-                   n_iter=np.zeros(shape, np.int64), status=np.zeros(shape, np.int64))
-        params = [self._base_params(self.cands[ci]) for ci in my]
-        resolved = [self._resolve(p) for p in params]
-        fits = np.zeros(shape + (4,))                       # solver, step, alpha_scaled, beta_scaled
-        zero_div = np.zeros(shape, bool)
-        for j, (p, (solver, alpha, beta)) in enumerate(zip(params, resolved)):
-            for k in range(ns):
-                try:
-                    fits[j, k] = (solver == "saga",) + self._step(k, solver, alpha, beta, bool(p["fit_intercept"]))
-                except ZeroDivisionError:
-                    if error_score == 'raise':
-                        raise
-                    zero_div[j, k] = True
-                    fits[j, k] = (solver == "saga", 1.0, 0.0, 0.0)
-        seeds = search_seed_table(self, self._draw_seeds)
-        groups = {}
-        for j, p in enumerate(params):
-            cw = p["class_weight"]
-            cwk = None if cw is None else (cw if isinstance(cw, str) else tuple(sorted(cw.items())))
-            groups.setdefault((float(p["tol"]), int(p["max_iter"]), bool(p["fit_intercept"]), cwk), []).append(j)
-        prof = {}
-        self.stats_ = np.zeros(shape + (2,), np.int64)
-        for (tol, mi, fi, _cwk), idx in groups.items():
-            self._set_class_weight(params[idx[0]]["class_weight"])
-            self.engine.set_scoring(self.score_kind, self.score_pos)
-            f = fits[idx]
-            r = self.engine.logreg_sag(f[..., 0].astype(np.int64), f[..., 2], f[..., 3], f[..., 1], seeds[[my[j] for j in idx]],
-                                       self.loss, tol=tol, max_iter=mi, fit_intercept=fi, return_train=return_train,
-                                       return_stats=True)
-            for key in ("test", "fit_ms", "score_ms", "n_iter", "status"):
-                res[key][idx] = r[key]
-            if return_train:
-                res["train"][idx] = r["train"]
-            self.stats_[idx] = r["stats"]
-            for k, v in self.engine.profile().items():
-                prof[k] = prof.get(k, 0) + v
-        self.engine.set_class_weight(None)
-        self._prof = prof
-        self.n_iter_ = res["n_iter"]
-        bad = (res["status"] == 2) | zero_div
-        if bad.any():
-            if error_score == 'raise':
-                j, k = map(int, np.argwhere(bad)[0])
-                raise SGDPlan._overflow(int(res["n_iter"][j, k]))
-            warnings.warn("%d fits failed (a floating-point under-/overflow, or step_size * alpha_scaled == 1); their scores "
-                          "are error_score=%r" % (int(bad.sum()), error_score))
-            res["test"][bad] = error_score
-            if return_train:
-                res["train"][bad] = error_score
-        return self._finish(res, return_train, error_score, len(my))
+    def _candidate(self, p, error_score):
+        """-> [n_splits][4] (solver, step, alpha_scaled, beta_scaled) and the [n_splits] fits where sag_solver raises
+        ZeroDivisionError"""
+        solver, alpha, beta = self._resolve(p)
+        fits = np.zeros((self.n_splits, 4))
+        zero_div = np.zeros(self.n_splits, bool)
+        for k in range(self.n_splits):
+            try:
+                fits[k] = (solver == "saga",) + self._step(k, solver, alpha, beta, bool(p["fit_intercept"]))
+            except ZeroDivisionError:
+                if error_score == 'raise':
+                    raise
+                zero_div[k] = True
+                fits[k] = (solver == "saga", 1.0, 0.0, 0.0)
+        return (float(p["tol"]), int(p["max_iter"]), bool(p["fit_intercept"])), (fits, zero_div)
+
+    def _prepare(self, my, error_score):
+        prepared, _ = super()._prepare(my, error_score)
+        return prepared, np.array([zd for _, _, (_, zd) in prepared], bool).reshape(len(my), self.n_splits)
+
+    def _search(self, key, values, cands, return_train):
+        tol, max_iter, fit_intercept = key
+        f = np.array([fits for fits, _ in values])
+        return self.engine.logreg_sag(f[..., 0].astype(np.int64), f[..., 2], f[..., 3], f[..., 1], self._seed_table()[cands],
+                                      self.loss, tol=tol, max_iter=max_iter, fit_intercept=fit_intercept,
+                                      return_train=return_train, return_stats=True)
 
     def refit(self, best_params):
         p = self._base_params(best_params)
         solver, alpha, beta = self._resolve(p)
         step, a, b = self._step(-1, solver, alpha, beta, bool(p["fit_intercept"]))
-        seed = sag_seed(p["random_state"])                    # the refit's own draw, after every search fit's
+        seed = self._seed(p["random_state"])                  # the refit's own draw, after every search fit's
         self._set_class_weight(p["class_weight"], refit=True)
         try:
             coef, n_iter, status = self.engine.logreg_sag_refit(solver, a, b, step, seed, self.loss, tol=p["tol"],
@@ -1154,7 +1086,7 @@ class LogRegSAGPlan(_Plan):
         finally:
             self.engine.set_class_weight(None)
         if status == 2:
-            raise SGDPlan._overflow(n_iter)
+            raise _overflow(n_iter)
         est = clone(self.estimator).set_params(**best_params)
         return materialize_logreg_sag(est, self.X, coef, n_iter, self.classes)
 
@@ -1178,21 +1110,13 @@ def materialize_logreg_sag(est, X, coef, n_iter, classes):
 
 
 # ------------------------------------------------------------------ LinearSVC -----------------
-class LinearSVCAdapter:
-    multi_device = True        # plan(..., device=d): one plan per GPU of the in-process scheduler
-    scorers = CLASSIFICATION_SCORERS
-
-    @staticmethod
-    def plan(estimator, cands, X, y, fold_id, n_splits, device=None):
-        return LinearSVCPlan(estimator, cands, X, y, fold_id, n_splits, device)
-
-
 class LinearSVCPlan(_Plan):
     """sklearn.svm.LinearSVC with liblinear's primal solver (L2R_L2LOSS_SVC: TRON, csrc/linsvc.cu).  X reaches the device in
     float32 or float64 and is widened exactly, as scikit-learn's fit converts it to float64.  Every fit resolves dual='auto'
     from its own training set, as LinearSVC.fit does; a fit that resolves to the dual solver has no CUDA path."""
     scorers = CLASSIFICATION_SCORERS
     supports_sample_weight = True
+    class_weighted = True
 
     def __init__(self, estimator, cands, X, y, fold_id, n_splits, device=None):
         super().__init__(estimator, cands, X, y, fold_id, n_splits, device)
@@ -1225,43 +1149,19 @@ class LinearSVCPlan(_Plan):
         if p["penalty"] != "l2":
             raise NotImplementedError("LinearSVC penalty=%r has no CUDA path (l2 does)" % (p["penalty"],))
 
-    def _params(self, cand, ks):
-        p = self._base_params(cand)
-        for k in ks:
+    def _candidate(self, p, error_score):
+        for k in range(self.n_splits):
             self._check(p, int(np.count_nonzero(self._train_rows(k))))
-        return p
+        return (float(p["tol"]), int(p["max_iter"]), bool(p["fit_intercept"]), float(p["intercept_scaling"])), float(p["C"])
 
-    def evaluate(self, my, return_train=True, error_score='raise'):
-        shape = (len(my), self.n_splits)
-        res = dict(test=np.zeros(shape), train=np.zeros(shape), fit_ms=np.zeros(shape), score_ms=np.zeros(shape),
-                   n_iter=np.zeros(shape, np.int64))
-        groups = {}
-        for j, ci in enumerate(my):
-            p = self._params(self.cands[ci], range(self.n_splits))
-            cw = p.get("class_weight")
-            cwk = None if cw is None else (cw if isinstance(cw, str) else tuple(sorted(cw.items())))
-            key = (float(p["tol"]), int(p["max_iter"]), bool(p["fit_intercept"]), float(p["intercept_scaling"]), cwk)
-            groups.setdefault(key, []).append((j, float(p["C"]), cw))
-        prof = {}
-        for (tol, mi, fi, isc, _cwk), items in groups.items():
-            idx = [j for j, _, _ in items]
-            self._set_class_weight(items[0][2])
-            self.engine.set_scoring(self.score_kind, self.score_pos)
-            r = self.engine.linsvc([c for _, c, _ in items], tol=tol, max_iter=mi, fit_intercept=fi, intercept_scaling=isc,
-                                   return_train=return_train)
-            for key in ("test", "fit_ms", "score_ms", "n_iter"):
-                res[key][idx] = r[key]
-            if return_train:
-                res["train"][idx] = r["train"]
-            for k, v in self.engine.profile().items():
-                prof[k] = prof.get(k, 0) + v
-        self.engine.set_class_weight(None)
-        self._prof = prof
-        self.n_iter_ = res["n_iter"]
-        return self._finish(res, return_train, error_score, len(my))
+    def _search(self, key, C, cands, return_train):
+        tol, max_iter, fit_intercept, intercept_scaling = key
+        return self.engine.linsvc(C, tol=tol, max_iter=max_iter, fit_intercept=fit_intercept,
+                                  intercept_scaling=intercept_scaling, return_train=return_train)
 
     def refit(self, best_params):
-        p = self._params(best_params, [-1])
+        p = self._base_params(best_params)
+        self._check(p, len(self.X))
         self._set_class_weight(p.get("class_weight"), refit=True)
         raw, n_iter = self.engine.linsvc_refit(p["C"], p["tol"], p["max_iter"], p["fit_intercept"], p["intercept_scaling"])
         self.engine.set_class_weight(None)
@@ -1290,48 +1190,6 @@ def materialize_linsvc(est, classes, raw, n_iter, n_features):
 
 
 # ------------------------------------------------------------------ LinearSVR -----------------
-class LinearSVRAdapter:
-    multi_device = True        # plan(..., device=d): one plan per GPU of the in-process scheduler
-    scorers = REGRESSION_SCORERS
-
-    @staticmethod
-    def plan(estimator, cands, X, y, fold_id, n_splits, device=None):
-        return LinearSVRPlan(estimator, cands, X, y, fold_id, n_splits, device)
-
-
-_INT_MAX = int(np.iinfo("i").max)
-_SEED_LOCK = threading.Lock()
-
-
-def liblinear_seed(random_state):
-    """The seed _fit_liblinear hands to liblinear: check_random_state(random_state).randint(np.iinfo('i').max).  An int or a
-    RandomState gives the same seed to every fit (clone deep-copies the parameter, so the caller's RandomState is not
-    advanced); None draws from numpy's global RandomState."""
-    from sklearn.utils import check_random_state
-    if random_state is not None and not isinstance(random_state, (numbers.Integral, np.random.RandomState)):
-        raise ValueError("%r cannot be used to seed a numpy.random.RandomState instance" % (random_state,))
-    rs = copy.deepcopy(random_state) if isinstance(random_state, np.random.RandomState) else random_state
-    return int(check_random_state(rs).randint(_INT_MAX))
-
-
-def search_seed_table(plan, draw):
-    """The seeds of every fit of a search, drawn by draw(random_states) as scikit-learn's GridSearchCV draws them:
-    candidate-major, split-minor, random_state=None from numpy's global RandomState.  A search whose candidates draw from the
-    global RandomState computes the table once for all of its per-GPU plans (they share the Folds); the plan keeps it."""
-    if plan._seeds is not None:
-        return plan._seeds
-    states = [plan._base_params(c)["random_state"] for c in plan.cands]
-    if any(rs is None for rs in states) and plan.folds is not None:
-        with _SEED_LOCK:
-            table = getattr(plan.folds, "_search_seeds", None)
-            if table is None:
-                table = plan.folds._search_seeds = draw(states)
-    else:
-        table = draw(states)
-    plan._seeds = table
-    return table
-
-
 class LinearSVRPlan(_Plan):
     """sklearn.svm.LinearSVR with liblinear's solvers (csrc/linsvr.cu): the dual coordinate descent for
     loss='epsilon_insensitive' (13) and for the squared loss when dual resolves to True (12), TRON otherwise (11).  dual='auto'
@@ -1346,14 +1204,7 @@ class LinearSVRPlan(_Plan):
         super().__init__(estimator, cands, X, y, fold_id, n_splits, device)
         if y is None:
             raise ValueError("LinearSVR needs y")
-        y = np.asarray(y)
-        if y.ndim == 2 and y.shape[1] == 1:               # scikit-learn: column_or_1d(y, warn=True)
-            from sklearn.exceptions import DataConversionWarning
-            warnings.warn("A column-vector y was passed when a 1d array was expected. Please change the shape of y to "
-                          "(n_samples, ), for example using ravel().", DataConversionWarning, stacklevel=2)
-            y = y[:, 0]
-        if y.ndim != 1:
-            raise ValueError("LinearSVR needs a 1d target; got y of shape %r" % (y.shape,))
+        y = _target_1d(y, "LinearSVR")
         if self.X.shape[1] > self.max_features:
             raise NotImplementedError("LinearSVR on %d features: the CUDA path handles up to %d"
                                       % (self.X.shape[1], self.max_features))
@@ -1362,7 +1213,6 @@ class LinearSVRPlan(_Plan):
         self.engine.set_targets_f64(self.y)
         if self.folds is not None:
             self.engine.set_train_order(self.folds.train_order)
-        self._seeds = None
 
     def _check(self, p, n_rows):
         """scikit-learn's own checks in LinearSVR.fit's order (parameter constraints, dual resolution on a training set of
@@ -1381,55 +1231,24 @@ class LinearSVRPlan(_Plan):
             raise NotImplementedError("LinearSVR epsilon=%r has no CUDA path (epsilon >= 0 does)" % (p["epsilon"],))
         return int(solver)
 
-    def _seed_table(self):
-        """[n_cand][n_splits] liblinear seeds of every fit of the search (search_seed_table)"""
-        return search_seed_table(self, self._draw_seeds)
+    def _seed(self, random_state):
+        return fit_seed(random_state, 0)
 
-    def _draw_seeds(self, states):
-        table = np.zeros((len(states), self.n_splits), np.int64)
-        for c, rs in enumerate(states):
-            if rs is None:
-                for k in range(self.n_splits):
-                    table[c, k] = liblinear_seed(None)
-            else:
-                table[c, :] = liblinear_seed(rs)
-        return table
+    def _candidate(self, p, error_score):
+        solvers = [self._check(p, int(np.count_nonzero(self._train_rows(k)))) for k in range(self.n_splits)]
+        return ((float(p["tol"]), int(p["max_iter"]), bool(p["fit_intercept"]), float(p["intercept_scaling"])),
+                (float(p["C"]), float(p["epsilon"]), solvers))
 
-    def evaluate(self, my, return_train=True, error_score='raise'):
-        ns = self.n_splits
-        shape = (len(my), ns)
-        res = dict(test=np.zeros(shape), train=np.zeros(shape), fit_ms=np.zeros(shape), score_ms=np.zeros(shape),
-                   n_iter=np.zeros(shape, np.int64))
-        rows = [int(np.count_nonzero(self._train_rows(k))) for k in range(ns)]
-        params = [self._base_params(self.cands[ci]) for ci in my]
-        solvers = [[self._check(p, rows[k]) for k in range(ns)] for p in params]
-        seeds = self._seed_table()
-        groups = {}
-        for j, (ci, p) in enumerate(zip(my, params)):
-            key = (float(p["tol"]), int(p["max_iter"]), bool(p["fit_intercept"]), float(p["intercept_scaling"]))
-            groups.setdefault(key, []).append(j)
-        prof = {}
-        self.cd_stats_ = np.zeros(shape + (3,), np.int64)
-        for (tol, mi, fi, isc), idx in groups.items():
-            self.engine.set_scoring(self.score_kind, self.score_pos)
-            r = self.engine.linsvr([float(params[j]["C"]) for j in idx], [float(params[j]["epsilon"]) for j in idx],
-                                   [solvers[j] for j in idx], seeds[[my[j] for j in idx]], tol=tol, max_iter=mi,
-                                   fit_intercept=fi, intercept_scaling=isc, return_train=return_train, return_stats=True)
-            for key in ("test", "fit_ms", "score_ms", "n_iter"):
-                res[key][idx] = r[key]
-            if return_train:
-                res["train"][idx] = r["train"]
-            self.cd_stats_[idx] = r["cd_stats"]
-            for k, v in self.engine.profile().items():
-                prof[k] = prof.get(k, 0) + v
-        self._prof = prof
-        self.n_iter_ = res["n_iter"]
-        return self._finish(res, return_train, error_score, len(my))
+    def _search(self, key, values, cands, return_train):
+        tol, max_iter, fit_intercept, intercept_scaling = key
+        return self.engine.linsvr([v[0] for v in values], [v[1] for v in values], [v[2] for v in values],
+                                  self._seed_table()[cands], tol=tol, max_iter=max_iter, fit_intercept=fit_intercept,
+                                  intercept_scaling=intercept_scaling, return_train=return_train, return_stats=True)
 
     def refit(self, best_params):
         p = self._base_params(best_params)
         solver = self._check(p, len(self.X))
-        seed = liblinear_seed(p["random_state"])            # the refit's own draw, after every search fit's
+        seed = self._seed(p["random_state"])                # the refit's own draw, after every search fit's
         raw, n_iter = self.engine.linsvr_refit(p["C"], p["epsilon"], solver, seed, p["tol"], p["max_iter"], p["fit_intercept"],
                                                p["intercept_scaling"])
         est = clone(self.estimator).set_params(**best_params)
@@ -1453,29 +1272,12 @@ def materialize_linsvr(est, raw, n_iter, n_features):
 
 
 # ------------------------------------------------------------------ SGDClassifier / SGDRegressor
-class SGDClassifierAdapter:
-    multi_device = True        # plan(..., device=d): one plan per GPU of the in-process scheduler
-    scorers = CLASSIFICATION_SCORERS
-
-    @staticmethod
-    def plan(estimator, cands, X, y, fold_id, n_splits, device=None):
-        return SGDPlan(estimator, cands, X, y, fold_id, n_splits, device)
-
-
-class SGDRegressorAdapter(SGDClassifierAdapter):
-    scorers = REGRESSION_SCORERS
-
-
 def sgd_seeds(random_state, n_classes):
     """The shuffle seeds scikit-learn hands to _plain_sgd for one fit (n_classes 0: a regressor), drawing from
     check_random_state(random_state) as fit does: binary fit_binary draws make_dataset's seed, then the shuffle seed;
     one-vs-rest draws one seed per class and each class fit makes those two draws from RandomState(seed); _fit_regressor
-    draws the shuffle seed, then make_dataset's.  An int or a RandomState gives the same seeds to every fit (clone
-    deep-copies the parameter, so the caller's RandomState is not advanced); None draws from numpy's global RandomState."""
-    from sklearn.utils import check_random_state
-    if random_state is not None and not isinstance(random_state, (numbers.Integral, np.random.RandomState)):
-        raise ValueError("%r cannot be used to seed a numpy.random.RandomState instance" % (random_state,))
-    rs = check_random_state(copy.deepcopy(random_state) if isinstance(random_state, np.random.RandomState) else random_state)
+    draws the shuffle seed, then make_dataset's (_random_state)."""
+    rs = _random_state(random_state)
     if n_classes == 0:
         seed = int(rs.randint(0, _INT_MAX))
         rs.randint(1, _INT_MAX)
@@ -1496,7 +1298,10 @@ class SGDPlan(_Plan):
     (candidate, split, one-vs-rest class) fit.  X reaches the device in its own dtype (float32 runs _plain_sgd32, as
     scikit-learn does), dense; the shuffle permutes the positions of X[train], so every split's training rows reach the
     device in the splitter's order."""
+    scorers = CLASSIFICATION_SCORERS
     supports_sample_weight = True
+    class_weighted = True
+    fail_warning = "%d fits failed with a floating-point under-/overflow; their scores are error_score=%r"
     max_features = 512         # w and q live in registers (include/b200gs.h GS_SGD_MAX_FEATURES)
 
     def __init__(self, estimator, cands, X, y, fold_id, n_splits, device=None):
@@ -1510,7 +1315,6 @@ class SGDPlan(_Plan):
         if y is None:
             raise ValueError("%s needs y" % name)
         self.classifier = isinstance(estimator, SGDClassifier)
-        self.scorers = CLASSIFICATION_SCORERS if self.classifier else REGRESSION_SCORERS
         if self.X.shape[1] > self.max_features:
             raise NotImplementedError("%s on %d features: the CUDA path handles up to %d" % (name, self.X.shape[1], self.max_features))
         y = np.asarray(y)
@@ -1531,7 +1335,6 @@ class SGDPlan(_Plan):
             self.kc = 1
         if self.folds is not None:
             self.engine.set_train_order(self.folds.train_order)
-        self._seeds = None
 
     def _check(self, p):
         """scikit-learn's own checks (ValueError), then the settings without a CUDA path"""
@@ -1552,16 +1355,8 @@ class SGDPlan(_Plan):
         from sklearn.utils.class_weight import compute_class_weight
         return compute_class_weight(cw, classes=self.classes, y=np.asarray(self.y)[self._train_rows(k)])
 
-    def _draw_seeds(self, states):
-        nc = len(self.classes) if self.classifier else 0
-        table = np.zeros((len(states), self.n_splits, self.kc), np.int64)
-        for c, rs in enumerate(states):
-            if rs is None:
-                for k in range(self.n_splits):
-                    table[c, k] = sgd_seeds(None, nc)
-            else:
-                table[c, :] = sgd_seeds(rs, nc)
-        return table
+    def _seed(self, random_state):
+        return sgd_seeds(random_state, len(self.classes) if self.classifier else 0)
 
     @staticmethod
     def _fit_args(p):
@@ -1569,66 +1364,23 @@ class SGDPlan(_Plan):
                     l1_ratio=float(0.0 if p["l1_ratio"] is None else p["l1_ratio"]), epsilon=float(p["epsilon"]),
                     learning_rate=p["learning_rate"], eta0=float(p["eta0"]), power_t=float(p["power_t"]))
 
-    @staticmethod
-    def _overflow(epoch):
-        return ValueError("Floating-point under-/overflow occurred at epoch #%d. Scaling input data with StandardScaler or "
-                          "MinMaxScaler might help." % epoch)
+    def _candidate(self, p, error_score):
+        self._check(p)
+        key = (None if p["tol"] is None else float(p["tol"]), int(p["max_iter"]), int(p["n_iter_no_change"]),
+               bool(p["fit_intercept"]), bool(p["shuffle"]))
+        return key, self._fit_args(p)
 
-    def evaluate(self, my, return_train=True, error_score='raise'):
-        ns = self.n_splits
-        shape = (len(my), ns)
-        res = dict(test=np.zeros(shape), train=np.zeros(shape), fit_ms=np.zeros(shape), score_ms=np.zeros(shape),
-                   n_iter=np.zeros(shape, np.int64), status=np.zeros(shape, np.int64))
-        params = [self._base_params(self.cands[ci]) for ci in my]
-        for p in params:
-            self._check(p)
-        seeds = search_seed_table(self, self._draw_seeds)
-        groups = {}
-        for j, p in enumerate(params):
-            cw = p["class_weight"] if self.classifier else None
-            cwk = None if cw is None else (cw if isinstance(cw, str) else tuple(sorted(cw.items())))
-            key = (None if p["tol"] is None else float(p["tol"]), int(p["max_iter"]), int(p["n_iter_no_change"]),
-                   bool(p["fit_intercept"]), bool(p["shuffle"]), cwk)
-            groups.setdefault(key, []).append(j)
-        prof = {}
-        self.stats_ = np.zeros(shape + (self.kc, 3), np.int64)
-        for (tol, mi, nic, fi, sh, _cwk), idx in groups.items():
-            if self.classifier:
-                self._set_class_weight(params[idx[0]]["class_weight"])
-            self.engine.set_scoring(self.score_kind, self.score_pos)
-            args = [self._fit_args(params[j]) for j in idx]
-            r = self.engine.sgd(*[[a[k] for a in args] for k in ("loss", "penalty", "alpha", "l1_ratio", "epsilon", "learning_rate",
-                                                                 "eta0", "power_t")],
-                                seeds[[my[j] for j in idx]], tol=tol, max_iter=mi, n_iter_no_change=nic, fit_intercept=fi,
-                                shuffle=sh, return_train=return_train, return_stats=True)
-            for key in ("test", "fit_ms", "score_ms", "n_iter", "status"):
-                res[key][idx] = r[key]
-            if return_train:
-                res["train"][idx] = r["train"]
-            self.stats_[idx] = r["stats"]
-            for k, v in self.engine.profile().items():
-                prof[k] = prof.get(k, 0) + v
-        if self.classifier:
-            self.engine.set_class_weight(None)
-        self._prof = prof
-        self.n_iter_ = res["n_iter"]
-        bad = res["status"] == 2
-        if bad.any():
-            if error_score == 'raise':
-                j, k = map(int, np.argwhere(bad)[0])
-                raise self._overflow(int(res["n_iter"][j, k]))
-            warnings.warn("%d fits failed with a floating-point under-/overflow; their scores are error_score=%r"
-                          % (int(bad.sum()), error_score))
-            res["test"][bad] = error_score
-            if return_train:
-                res["train"][bad] = error_score
-        return self._finish(res, return_train, error_score, len(my))
+    def _search(self, key, args, cands, return_train):
+        tol, max_iter, n_iter_no_change, fit_intercept, shuffle = key
+        return self.engine.sgd(*[[a[k] for a in args] for k in ("loss", "penalty", "alpha", "l1_ratio", "epsilon", "learning_rate",
+                                                                "eta0", "power_t")],
+                               self._seed_table()[cands], tol=tol, max_iter=max_iter, n_iter_no_change=n_iter_no_change,
+                               fit_intercept=fit_intercept, shuffle=shuffle, return_train=return_train, return_stats=True)
 
     def refit(self, best_params):
         p = self._base_params(best_params)
         self._check(p)
-        nc = len(self.classes) if self.classifier else 0
-        seeds = sgd_seeds(p["random_state"], nc)                # the refit's own draw, after every search fit's
+        seeds = self._seed(p["random_state"])                   # the refit's own draw, after every search fit's
         cw_ = self._set_class_weight(p["class_weight"], refit=True) if self.classifier else None
         try:
             coef, n_iter, status = self.engine.sgd_refit(**self._fit_args(p), seed=seeds, tol=p["tol"], max_iter=p["max_iter"],
@@ -1638,9 +1390,14 @@ class SGDPlan(_Plan):
             if self.classifier:
                 self.engine.set_class_weight(None)
         if (status == 2).any():
-            raise self._overflow(int(n_iter[int(np.argmax(status == 2))]))
+            raise _overflow(int(n_iter[int(np.argmax(status == 2))]))
         est = clone(self.estimator).set_params(**best_params)
         return materialize_sgd(est, self.X, coef, n_iter, self.classes if self.classifier else None, cw_)
+
+
+class SGDRegressorPlan(SGDPlan):
+    scorers = REGRESSION_SCORERS
+    class_weighted = False
 
 
 def materialize_sgd(est, X, coef, n_iter, classes, class_weight):
@@ -1672,21 +1429,6 @@ def materialize_sgd(est, X, coef, n_iter, classes, class_weight):
 
 
 # ------------------------------------------------------------------ k-nearest neighbours ------
-class KNeighborsAdapter:
-    # One GPU: the neighbour selection is the cost of the whole search and every candidate shares it, so dealing candidates
-    # to several GPUs would repeat it on each.  Under torchrun each rank still evaluates the candidates it is dealt.
-    multi_device = False
-    scorers = CLASSIFICATION_SCORERS
-
-    @staticmethod
-    def plan(estimator, cands, X, y, fold_id, n_splits, device=None):
-        return KNeighborsPlan(estimator, cands, X, y, fold_id, n_splits, device)
-
-
-class KNeighborsRegressorAdapter(KNeighborsAdapter):
-    scorers = REGRESSION_SCORERS
-
-
 _KNN_METRICS = {"euclidean": "euclidean", "l2": "euclidean", "manhattan": "manhattan", "l1": "manhattan",
                 "cityblock": "manhattan"}
 
@@ -1697,6 +1439,10 @@ class KNeighborsPlan(_Plan):
     rows).  The engine selects the max n_neighbors nearest training rows once per (split, metric) and every candidate votes
     from those lists.  The refit is scikit-learn's own fit (it stores the data, plus a tree index when scikit-learn builds
     one: there is no arithmetic for the device to take over)."""
+    # One GPU: the neighbour selection is the cost of the whole search and every candidate shares it, so dealing candidates
+    # to several GPUs would repeat it on each.  Under torchrun each rank still evaluates the candidates it is dealt.
+    multi_device = False
+    scorers = CLASSIFICATION_SCORERS
     max_neighbors = 256
 
     def __init__(self, estimator, cands, X, y, fold_id, n_splits, device=None):
@@ -1706,7 +1452,6 @@ class KNeighborsPlan(_Plan):
         if y is None:
             raise ValueError("%s needs y" % name)
         self.classifier = isinstance(estimator, KNeighborsClassifier)
-        self.scorers = CLASSIFICATION_SCORERS if self.classifier else REGRESSION_SCORERS
         y = np.asarray(y)
         if y.ndim != 1:
             raise NotImplementedError("multi-output %s is not supported by the CUDA path" % name)
@@ -1743,38 +1488,38 @@ class KNeighborsPlan(_Plan):
                                       % (metric, ", ".join(sorted(_KNN_METRICS))))
         return int(nn), p["weights"], _KNN_METRICS[metric]
 
-    def evaluate(self, my, return_train=True, error_score='raise'):
-        ns = self.n_splits
-        shape = (len(my), ns)
-        checked = [self._check(self._base_params(self.cands[ci])) for ci in my]
-        m_train = [int(np.count_nonzero(self._train_rows(k))) for k in range(ns)]
-        too_many = np.array([[nn > m_train[k] for k in range(ns)] for nn, _, _ in checked], bool).reshape(shape)
+    def _candidate(self, p, error_score):
+        return (), self._check(p)                         # one group: every candidate shares the neighbour selection
+
+    def _prepare(self, my, error_score):
+        """a fit whose n_neighbors exceeds its training rows fails, as scikit-learn's predict does"""
+        prepared, _ = super()._prepare(my, error_score)
+        m_train = [int(np.count_nonzero(self._train_rows(k))) for k in range(self.n_splits)]
+        too_many = np.array([[nn > m_train[k] for k in range(self.n_splits)] for _, _, (nn, _, _) in prepared],
+                            bool).reshape(len(my), self.n_splits)
         if too_many.any() and error_score == 'raise':
             j, k = map(int, np.argwhere(too_many)[0])
             n_test = int(np.count_nonzero(self._test_rows(k)))
             raise ValueError("Expected n_neighbors <= n_samples_fit, but n_neighbors = %d, n_samples_fit = %d, n_samples = %d"
-                             % (checked[j][0], m_train[k], n_test))
-        res = dict(test=np.full(shape, np.nan), train=np.full(shape, np.nan), fit_ms=np.zeros(shape), score_ms=np.zeros(shape))
-        if my:
-            self.engine.set_scoring(self.score_kind, self.score_pos)
-            r = self.engine.knn([c[0] for c in checked], [c[1] for c in checked], [c[2] for c in checked],
-                                return_train=return_train, y_f32=not self.classifier and self.y_f32)
-            for key in ("test", "fit_ms", "score_ms"):
-                res[key][:] = r[key]
-            if return_train:
-                res["train"][:] = r["train"]
-            self._prof = self.engine.profile()
-        res["test"][too_many] = np.nan
-        res["train"][too_many] = np.nan
-        return self._finish(res, return_train, error_score, len(my))
+                             % (prepared[j][2][0], m_train[k], n_test))
+        return prepared, too_many
 
-    def _test_rows(self, k):
-        if self.folds is not None and not self.folds.partition:
-            return (self.folds.masks[0][:, k >> 6] >> np.uint64(k & 63)) & np.uint64(1) == 1
-        fold_id = self.fold_id if self.folds is None else self.folds.fold_id
-        return fold_id == k
+    def _search(self, key, values, cands, return_train):
+        return self.engine.knn([v[0] for v in values], [v[1] for v in values], [v[2] for v in values],
+                               return_train=return_train, y_f32=not self.classifier and self.y_f32)
 
     def refit(self, best_params):
         p = self._base_params(best_params)
         self._check(p)
         return clone(self.estimator).set_params(**best_params).fit(self.X, self.y)
+
+
+class KNeighborsRegressorPlan(KNeighborsPlan):
+    scorers = REGRESSION_SCORERS
+
+
+# The names the plan classes had when adapters were separate classes: code that imports them keeps working.
+SVCAdapter, NuSVCAdapter, SVRAdapter, NuSVRAdapter = SVCPlan, NuSVCPlan, SVRPlan, NuSVRPlan
+RidgeAdapter, ENetAdapter, LogRegAdapter = RidgePlan, ENetPlan, LogRegPlan
+LinearSVCAdapter, LinearSVRAdapter, SGDClassifierAdapter, SGDRegressorAdapter = LinearSVCPlan, LinearSVRPlan, SGDPlan, SGDRegressorPlan
+KNeighborsAdapter, KNeighborsRegressorAdapter = KNeighborsPlan, KNeighborsRegressorPlan

@@ -46,7 +46,7 @@ def test_linsvc_vs_golden(engine, key, variant):
     X, y = w["X"], w["y"]
     g = golden(key)
     cands = W.candidates(w)
-    plan = E.LinearSVCAdapter.plan(LinearSVC(**VARIANTS[variant]), cands, X, y,
+    plan = E.LinearSVCPlan.plan(LinearSVC(**VARIANTS[variant]), cands, X, y,
                                    E.Folds(list(StratifiedKFold(w["cv"]).split(X, y)), len(X)), w["cv"])
     plan.set_scoring(None)
     plan.set_fit_params({"sample_weight": sample_weight(len(X))} if variant == "sw" else None)

@@ -115,7 +115,7 @@ def test_linsvr_vs_golden(engine, key, variant):
     X, y = w["X"], w["y"]
     g = golden(key)
     cands = W.candidates(w)
-    plan = E.LinearSVRAdapter.plan(LinearSVR(**w["est_params"], **V[variant]), cands, X, y,
+    plan = E.LinearSVRPlan.plan(LinearSVR(**w["est_params"], **V[variant]), cands, X, y,
                                    E.Folds(list(KFold(w["cv"]).split(X, y)), len(X)), w["cv"])
     plan.set_scoring(None)
     plan.set_fit_params({"sample_weight": sample_weight(len(X))} if variant == "sw" else None)

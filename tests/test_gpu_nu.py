@@ -54,7 +54,7 @@ def _plan_n_iter(adapter, est, cands, X, y, splits):
 @pytest.mark.parametrize("kernel", ["rbf", "linear", "poly", "sigmoid"])
 def test_nusvc_matches_sklearn(engine, n_classes, kernel):
     """Split scores identical to scikit-learn's GridSearchCV and n_iter equal per fit, for every kernel."""
-    from spark_sklearn_b200.estimators import NuSVCAdapter
+    from spark_sklearn_b200.estimators import NuSVCPlan
     X, y = _clf(n_classes)
     grid = {"nu": [0.1, 0.3, 0.5], "gamma": ["scale", 0.05]}
     base = {"kernel": kernel}
@@ -67,7 +67,7 @@ def test_nusvc_matches_sklearn(engine, n_classes, kernel):
     assert ours.best_params_ == ref.best_params_
     cands = list(ParameterGrid(grid))
     splits = list(StratifiedKFold(5).split(X, y))
-    got, want = _plan_n_iter(NuSVCAdapter, NuSVC(**base), cands, X, y, splits), _n_iter_nusvc(X, y, cands, splits, base)
+    got, want = _plan_n_iter(NuSVCPlan, NuSVC(**base), cands, X, y, splits), _n_iter_nusvc(X, y, cands, splits, base)
     if kernel in ("rbf", "sigmoid"):
         # exp / tanh: the device's float64 kernel value can differ from the host libm's in the last bit, which can move a
         # trajectory by an iteration without changing a score.  Measured on one H100: one fit of the 60 (sigmoid, 3
@@ -80,7 +80,7 @@ def test_nusvc_matches_sklearn(engine, n_classes, kernel):
 
 def test_nusvc_variants_match_sklearn(engine):
     """shrinking off, a max_iter stop, a larger problem that shrinks and unshrinks, and a class_weight (no effect on nu-SVC)"""
-    from spark_sklearn_b200.estimators import NuSVCAdapter
+    from spark_sklearn_b200.estimators import NuSVCPlan
     X, y = _clf(3, n=1200, seed=1)
     splits = list(StratifiedKFold(3).split(X, y))
     for base, grid in [({"shrinking": False}, {"nu": [0.2, 0.4]}),
@@ -95,7 +95,7 @@ def test_nusvc_variants_match_sklearn(engine):
         cands = list(ParameterGrid(grid))
         with warnings.catch_warnings():
             warnings.simplefilter("ignore")
-            np.testing.assert_array_equal(_plan_n_iter(NuSVCAdapter, NuSVC(**base), cands, X, y, splits),
+            np.testing.assert_array_equal(_plan_n_iter(NuSVCPlan, NuSVC(**base), cands, X, y, splits),
                                           _n_iter_nusvc(X, y, cands, splits, base), err_msg=str(base))
 
 
@@ -163,7 +163,7 @@ def test_nusvc_one_step_pipeline(engine):
 @pytest.mark.parametrize("kernel", ["rbf", "linear"])
 def test_nusvr_matches_sklearn(engine, kernel):
     """Split scores within 1e-12 and n_iter equal per fit; the refit equals a real fit"""
-    from spark_sklearn_b200.estimators import NuSVRAdapter
+    from spark_sklearn_b200.estimators import NuSVRPlan
     X, y = _reg()
     grid = {"nu": [0.1, 0.5, 0.9], "C": [1.0, 10.0]}
     ours = GridSearchCV(None, NuSVR(kernel=kernel), grid, cv=5, return_train_score=True).fit(X, y)
@@ -173,7 +173,7 @@ def test_nusvr_matches_sklearn(engine, kernel):
     cands = list(ParameterGrid(grid))
     splits = list(KFold(5).split(X))
     sit = np.array([[NuSVR(kernel=kernel, **c).fit(X[a], y[a]).n_iter_ for a, _ in splits] for c in cands])
-    np.testing.assert_array_equal(_plan_n_iter(NuSVRAdapter, NuSVR(kernel=kernel), cands, X, y, splits), sit)
+    np.testing.assert_array_equal(_plan_n_iter(NuSVRPlan, NuSVR(kernel=kernel), cands, X, y, splits), sit)
     best = ours.best_estimator_
     assert type(best) is NuSVR
     real = NuSVR(**best.get_params()).fit(X, y)

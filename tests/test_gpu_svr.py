@@ -35,9 +35,9 @@ def _sk_fits(X, y, cands, cv, base=None, scoring=None):
 
 def _engine_run(engine, X, y, cands, cv, base=None):
     """the engine directly (n_iter per fit is not part of cv_results_)"""
-    from spark_sklearn_b200.estimators import Folds, SVRAdapter
+    from spark_sklearn_b200.estimators import Folds, SVRPlan
     splits = list(KFold(cv).split(X))
-    plan = SVRAdapter.plan(SVR(**(base or {})), cands, X, y, Folds(splits, len(X)), cv)
+    plan = SVRPlan.plan(SVR(**(base or {})), cands, X, y, Folds(splits, len(X)), cv)
     r = plan.evaluate(list(range(len(cands))), return_train=True)
     return plan.n_iter_, r["test"], r["train"]
 
@@ -122,8 +122,8 @@ def test_svr_max_iter_after_shrinking(engine):
     w = W.make_workload("svr_small")
     X, y = w["X"], w["y"]
     _check(engine, X, y, [{"C": 100.0, "gamma": 1 / 32, "epsilon": 0.05}], base={"max_iter": 1500})   # ~1850 to converge
-    from spark_sklearn_b200.estimators import Folds, SVRAdapter
-    plan = SVRAdapter.plan(SVR(max_iter=1500), [{}], X, y, Folds(list(KFold(5).split(X)), len(X)), 5)   # 2428 to converge
+    from spark_sklearn_b200.estimators import Folds, SVRPlan
+    plan = SVRPlan.plan(SVR(max_iter=1500), [{}], X, y, Folds(list(KFold(5).split(X)), len(X)), 5)   # 2428 to converge
     with pytest.warns(ConvergenceWarning):
         got = plan.refit({"C": 100.0, "gamma": 1 / 32, "epsilon": 0.05})
     with pytest.warns(ConvergenceWarning):

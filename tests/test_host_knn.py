@@ -64,13 +64,13 @@ def _plan(est, cands, X, y, cv=5):
 
 
 def test_adapter_resolution():
-    assert E.adapter_for(KNeighborsClassifier()) is E.KNeighborsAdapter
-    assert E.adapter_for(KNeighborsRegressor()) is E.KNeighborsRegressorAdapter
-    assert E.KNeighborsAdapter.scorers is E.CLASSIFICATION_SCORERS
-    assert E.KNeighborsRegressorAdapter.scorers is E.REGRESSION_SCORERS
-    assert not E.KNeighborsAdapter.multi_device and not E.KNeighborsRegressorAdapter.multi_device
+    assert E.adapter_for(KNeighborsClassifier()) is E.KNeighborsPlan
+    assert E.adapter_for(KNeighborsRegressor()) is E.KNeighborsRegressorPlan
+    assert E.KNeighborsPlan.scorers is E.CLASSIFICATION_SCORERS
+    assert E.KNeighborsRegressorPlan.scorers is E.REGRESSION_SCORERS
+    assert not E.KNeighborsPlan.multi_device and not E.KNeighborsRegressorPlan.multi_device
     a = E.adapter_for(Pipeline([("knn", KNeighborsClassifier())]))
-    assert isinstance(a, E.PipelineAdapter) and a.inner is E.KNeighborsAdapter and not a.multi_device
+    assert isinstance(a, E.PipelineAdapter) and a.inner is E.KNeighborsPlan and not a.multi_device
     with pytest.raises(NotImplementedError, match="KNeighborsClassifier and KNeighborsRegressor"):
         from sklearn.tree import DecisionTreeClassifier
         E.adapter_for(DecisionTreeClassifier())

@@ -67,12 +67,12 @@ def _data(n=300, key="linsvc_small"):
 
 def _plan(est, cands, X, y, cv=5):
     splits = list(StratifiedKFold(cv).split(X, y))
-    return E.LinearSVCAdapter.plan(est, cands, X, y, E.Folds(splits, len(X)), len(splits))
+    return E.LinearSVCPlan.plan(est, cands, X, y, E.Folds(splits, len(X)), len(splits))
 
 
 def test_adapter_and_arrays_handed_to_the_engine(fake):
     from sklearn.pipeline import Pipeline
-    assert E.adapter_for(LinearSVC()) is E.LinearSVCAdapter
+    assert E.adapter_for(LinearSVC()) is E.LinearSVCPlan
     assert isinstance(E.adapter_for(Pipeline([("s", LinearSVC())])), E.PipelineAdapter)
     X, y = _data()
     X64 = X.astype(np.float64)

@@ -80,13 +80,13 @@ def _data(n=300, key="linsvr_small"):
 
 def _plan(est, cands, X, y, cv=None):
     splits = list((cv or KFold(5)).split(X, y))
-    return E.LinearSVRAdapter.plan(est, cands, X, y, E.Folds(splits, len(X)), len(splits)), splits
+    return E.LinearSVRPlan.plan(est, cands, X, y, E.Folds(splits, len(X)), len(splits)), splits
 
 
 def test_adapter_and_arrays_handed_to_the_engine(fake):
     from sklearn.pipeline import Pipeline
-    assert E.adapter_for(LinearSVR()) is E.LinearSVRAdapter
-    assert E.LinearSVRAdapter.multi_device and E.LinearSVRAdapter.scorers is E.REGRESSION_SCORERS
+    assert E.adapter_for(LinearSVR()) is E.LinearSVRPlan
+    assert E.LinearSVRPlan.multi_device and E.LinearSVRPlan.scorers is E.REGRESSION_SCORERS
     assert isinstance(E.adapter_for(Pipeline([("s", LinearSVR())])), E.PipelineAdapter)
     X, y = _data()
     plan, splits = _plan(LinearSVR(random_state=0), [{"C": 0.5, "epsilon": 0.1}, {"C": 2.0}], X, y)
@@ -127,7 +127,7 @@ def test_dual_resolution_per_fold_and_refit(fake):
     assert fake.calls[-1]["solver"] == 11
     # a mixed search: folds of unequal size resolve differently
     cv = [(np.arange(10, 60), np.arange(10)), (np.arange(15, 60), np.arange(15))]   # 50 and 45 training rows
-    plan = E.LinearSVRAdapter.plan(LinearSVR(loss="squared_epsilon_insensitive"), [{}], X, y, E.Folds(cv, 60), 2)
+    plan = E.LinearSVRPlan.plan(LinearSVR(loss="squared_epsilon_insensitive"), [{}], X, y, E.Folds(cv, 60), 2)
     plan.evaluate([0])
     np.testing.assert_array_equal(fake.calls[-1]["solver"], [[11, 12]])
 

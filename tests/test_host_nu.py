@@ -75,22 +75,22 @@ def _data(n=100, weights=(0.5, 0.5), seed=0):
 
 
 def _plan(adapter, est, cands, X, y, cv=5):
-    splits = list((StratifiedKFold(cv) if adapter is E.NuSVCAdapter else KFold(cv)).split(X, y))
+    splits = list((StratifiedKFold(cv) if adapter is E.NuSVCPlan else KFold(cv)).split(X, y))
     return adapter.plan(est, cands, X, y, E.Folds(splits, len(X)), len(splits))
 
 
 def test_dispatch():
-    assert E.adapter_for(NuSVC()) is E.NuSVCAdapter
-    assert E.adapter_for(NuSVR()) is E.NuSVRAdapter
+    assert E.adapter_for(NuSVC()) is E.NuSVCPlan
+    assert E.adapter_for(NuSVR()) is E.NuSVRPlan
     pa = E.adapter_for(Pipeline([("m", NuSVR())]))
-    assert isinstance(pa, E.PipelineAdapter) and pa.inner is E.NuSVRAdapter
+    assert isinstance(pa, E.PipelineAdapter) and pa.inner is E.NuSVRPlan
     assert pa._strip({"m__nu": 0.3, "m__C": 2.0}) == {"nu": 0.3, "C": 2.0}
-    assert E.NuSVCAdapter.multi_device and E.NuSVRAdapter.multi_device
+    assert E.NuSVCPlan.multi_device and E.NuSVRPlan.multi_device
 
 
 def test_nusvc_hands_nu_to_the_nu_solver(fake):
     X, y = _data()
-    plan = _plan(E.NuSVCAdapter, NuSVC(), [{"nu": 0.2}, {"nu": 0.5, "kernel": "poly"}], X, y)
+    plan = _plan(E.NuSVCPlan, NuSVC(), [{"nu": 0.2}, {"nu": 0.5, "kernel": "poly"}], X, y)
     plan.evaluate([0, 1])
     assert fake.calls == [("svc", ["rbf", "poly"], [0.2, 0.5], True)]
     assert plan.costs() is None
@@ -98,7 +98,7 @@ def test_nusvc_hands_nu_to_the_nu_solver(fake):
 
 def test_nusvr_hands_c_and_nu_to_the_nu_solver(fake):
     X, y = _data()
-    plan = _plan(E.NuSVRAdapter, NuSVR(C=3.0), [{"nu": 0.2}, {"nu": 0.7, "kernel": "linear"}], X, y.astype(float))
+    plan = _plan(E.NuSVRPlan, NuSVR(C=3.0), [{"nu": 0.2}, {"nu": 0.7, "kernel": "linear"}], X, y.astype(float))
     plan.evaluate([0, 1])
     assert fake.calls == [("svr", ["rbf", "linear"], [3.0, 3.0], [0.2, 0.7], True)]
 
@@ -107,9 +107,9 @@ def test_nusvr_hands_c_and_nu_to_the_nu_solver(fake):
                                        (NuSVR(), {"C": 0.0})])
 def test_invalid_values_raise_sklearns_value_error(fake, est, cand):
     X, y = _data()
-    adapter = E.NuSVCAdapter if isinstance(est, NuSVC) else E.NuSVRAdapter
+    adapter = E.NuSVCPlan if isinstance(est, NuSVC) else E.NuSVRPlan
     with pytest.raises(ValueError, match="parameter"):
-        _plan(adapter, est, [cand], X, y.astype(float) if adapter is E.NuSVRAdapter else y).evaluate([0])
+        _plan(adapter, est, [cand], X, y.astype(float) if adapter is E.NuSVRPlan else y).evaluate([0])
     assert fake.calls == []
 
 
@@ -118,18 +118,18 @@ def test_invalid_values_raise_sklearns_value_error(fake, est, cand):
                                        (NuSVR(), {"kernel": "sigmoid"})])
 def test_unsupported_options_raise(fake, est, cand):
     X, y = _data()
-    adapter = E.NuSVCAdapter if isinstance(est, NuSVC) else E.NuSVRAdapter
+    adapter = E.NuSVCPlan if isinstance(est, NuSVC) else E.NuSVRPlan
     with pytest.raises(NotImplementedError):
-        _plan(adapter, est, [cand], X, y.astype(float) if adapter is E.NuSVRAdapter else y).evaluate([0])
+        _plan(adapter, est, [cand], X, y.astype(float) if adapter is E.NuSVRPlan else y).evaluate([0])
 
 
 def test_sample_weight_and_oversize_nusvr_raise(fake):
     X, y = _data()
-    plan = _plan(E.NuSVCAdapter, NuSVC(), [{"nu": 0.3}], X, y)
+    plan = _plan(E.NuSVCPlan, NuSVC(), [{"nu": 0.3}], X, y)
     with pytest.raises(NotImplementedError):
         plan.set_fit_params({"sample_weight": np.ones(len(X))})
     X = np.zeros((8193, 2))
-    plan = _plan(E.NuSVRAdapter, NuSVR(), [{"nu": 0.3}], X, np.zeros(len(X)), cv=2)
+    plan = _plan(E.NuSVRPlan, NuSVR(), [{"nu": 0.3}], X, np.zeros(len(X)), cv=2)
     with pytest.raises(NotImplementedError, match="8192"):
         plan.check_refit()
 
@@ -145,7 +145,7 @@ def test_feasibility_follows_libsvm():
 
 def test_infeasible_nu_raises_before_device_work(fake):
     X, y = _data(weights=(0.7, 0.3))
-    plan = _plan(E.NuSVCAdapter, NuSVC(), [{"nu": 0.3}, {"nu": 0.9}], X, y)
+    plan = _plan(E.NuSVCPlan, NuSVC(), [{"nu": 0.3}, {"nu": 0.9}], X, y)
     with pytest.raises(ValueError, match="specified nu is infeasible"):
         plan.evaluate([0, 1], error_score="raise")
     assert fake.calls == []
@@ -156,7 +156,7 @@ def test_infeasible_nu_raises_before_device_work(fake):
 
 def test_infeasible_tasks_take_error_score(fake):
     X, y = _data(weights=(0.7, 0.3))
-    plan = _plan(E.NuSVCAdapter, NuSVC(), [{"nu": 0.3}, {"nu": 0.9}], X, y)
+    plan = _plan(E.NuSVCPlan, NuSVC(), [{"nu": 0.3}, {"nu": 0.9}], X, y)
     fake.nan_tasks = (slice(1, 2), slice(None))
     with warnings.catch_warnings():
         warnings.simplefilter("ignore")

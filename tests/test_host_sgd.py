@@ -89,9 +89,9 @@ def _plan(est, cands, y, cv=None, X=X):
 
 def test_adapters(fake):
     from sklearn.pipeline import Pipeline
-    assert E.adapter_for(SGDClassifier()) is E.SGDClassifierAdapter and E.SGDClassifierAdapter.multi_device
-    assert E.adapter_for(SGDRegressor()) is E.SGDRegressorAdapter
-    assert E.SGDRegressorAdapter.scorers is E.REGRESSION_SCORERS and E.SGDClassifierAdapter.scorers is E.CLASSIFICATION_SCORERS
+    assert E.adapter_for(SGDClassifier()) is E.SGDPlan and E.SGDPlan.multi_device
+    assert E.adapter_for(SGDRegressor()) is E.SGDRegressorPlan
+    assert E.SGDRegressorPlan.scorers is E.REGRESSION_SCORERS and E.SGDPlan.scorers is E.CLASSIFICATION_SCORERS
     assert isinstance(E.adapter_for(Pipeline([("s", SGDClassifier())])), E.PipelineAdapter)
 
 
@@ -178,7 +178,7 @@ def test_too_many_features_and_sparse(fake):
     with pytest.raises(NotImplementedError, match="512"):
         _plan(SGDClassifier(), [{}], Y2, X=np.zeros((120, 513)))
     with pytest.raises(NotImplementedError, match="sparse"):
-        E.SGDClassifierAdapter.plan(SGDClassifier(), [{}], sp.csr_matrix(X), Y2, None, 4)
+        E.SGDPlan.plan(SGDClassifier(), [{}], sp.csr_matrix(X), Y2, None, 4)
 
 
 def test_non_finite_fit(fake):

@@ -51,7 +51,7 @@ def fake(monkeypatch):
 def _plan(est, cands, X, y, cv=5):
     from sklearn.model_selection import StratifiedKFold
     splits = list(StratifiedKFold(cv).split(X, y))
-    return E.SVCAdapter.plan(est, cands, X, y, E.Folds(splits, len(X)), len(splits)), splits
+    return E.SVCPlan.plan(est, cands, X, y, E.Folds(splits, len(X)), len(splits)), splits
 
 
 def _data():

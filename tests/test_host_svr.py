@@ -55,13 +55,13 @@ def fake(monkeypatch):
 def _plan(est, cands, X, y, cv=5):
     from sklearn.model_selection import KFold
     splits = list(KFold(cv).split(X, y))
-    return E.SVRAdapter.plan(est, cands, X, y, E.Folds(splits, len(X)), len(splits))
+    return E.SVRPlan.plan(est, cands, X, y, E.Folds(splits, len(X)), len(splits))
 
 
 def test_adapter_resolution():
-    assert E.adapter_for(SVR()) is E.SVRAdapter
+    assert E.adapter_for(SVR()) is E.SVRPlan
     a = E.adapter_for(Pipeline([("svr", SVR())]))
-    assert isinstance(a, E.PipelineAdapter) and a.inner is E.SVRAdapter
+    assert isinstance(a, E.PipelineAdapter) and a.inner is E.SVRPlan
     assert a.scorers is E.REGRESSION_SCORERS and a.multi_device
     with pytest.raises(NotImplementedError):
         E.adapter_for(Pipeline([("a", SVR()), ("b", SVR())]))

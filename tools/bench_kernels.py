@@ -27,7 +27,7 @@ def main():
 
     from sklearn.model_selection import check_cv
     from sklearn.svm import SVC
-    from spark_sklearn_b200.estimators import Folds, SVCAdapter
+    from spark_sklearn_b200.estimators import Folds, SVCPlan
     from spark_sklearn_b200 import workloads as W
 
     w = W.make_workload(a.workload)
@@ -35,7 +35,7 @@ def main():
     cands = W.candidates(w)
     splits = list(check_cv(w["cv"], y, classifier=True).split(X, y))
     ns = len(splits)
-    plan = SVCAdapter.plan(SVC(**w["est_params"]), cands, X, y, Folds(splits, len(X)), ns)   # X, y resident from here
+    plan = SVCPlan.plan(SVC(**w["est_params"]), cands, X, y, Folds(splits, len(X)), ns)   # X, y resident from here
     plan.evaluate([0])                                            # warm-up: library load, kernel attributes, buffers
     if a.timeline:
         os.environ["B200GS_SMO_TIMELINE"] = "1"

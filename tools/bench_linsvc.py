@@ -38,14 +38,14 @@ def main():
 
     from sklearn.model_selection import GridSearchCV as SkGridSearchCV, StratifiedKFold
     from sklearn.svm import LinearSVC
-    from spark_sklearn_b200.estimators import Folds, LinearSVCAdapter
+    from spark_sklearn_b200.estimators import Folds, LinearSVCPlan
     from spark_sklearn_b200 import workloads as W
 
     w = W.make_workload(a.workload)
     X, y, cv = w["X"], w["y"], w["cv"]
     cands = W.candidates(w)
     splits = list(StratifiedKFold(cv).split(X, y))
-    plan = LinearSVCAdapter.plan(LinearSVC(**w["est_params"]), cands, X, y, Folds(splits, len(X)), cv)   # X resident from here
+    plan = LinearSVCPlan.plan(LinearSVC(**w["est_params"]), cands, X, y, Folds(splits, len(X)), cv)   # X resident from here
     plan.set_scoring(None)
     n_fits = len(cands) * cv
 

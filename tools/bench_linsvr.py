@@ -38,14 +38,14 @@ def main():
     from sklearn.exceptions import ConvergenceWarning
     from sklearn.model_selection import GridSearchCV as SkGridSearchCV, KFold
     from sklearn.svm import LinearSVR
-    from spark_sklearn_b200.estimators import Folds, LinearSVRAdapter
+    from spark_sklearn_b200.estimators import Folds, LinearSVRPlan
     from spark_sklearn_b200 import workloads as W
 
     w = W.make_workload(a.workload)
     X, y, cv = w["X"], w["y"], w["cv"]
     cands = W.candidates(w)
     splits = list(KFold(cv).split(X, y))
-    plan = LinearSVRAdapter.plan(LinearSVR(**w["est_params"]), cands, X, y, Folds(splits, len(X)), cv)   # X resident from here
+    plan = LinearSVRPlan.plan(LinearSVR(**w["est_params"]), cands, X, y, Folds(splits, len(X)), cv)   # X resident from here
     plan.set_scoring(None)
     n_fits = len(cands) * cv
 

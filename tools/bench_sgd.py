@@ -23,9 +23,9 @@ from bench_linsvr import card  # noqa: E402
 
 def _plan(X, y, cands, cv, est):
     from sklearn.model_selection import StratifiedKFold
-    from spark_sklearn_b200.estimators import Folds, SGDClassifierAdapter
+    from spark_sklearn_b200.estimators import Folds, SGDPlan
     splits = list(StratifiedKFold(cv).split(X, y))
-    plan = SGDClassifierAdapter.plan(est, cands, X, y, Folds(splits, len(X)), cv)
+    plan = SGDPlan.plan(est, cands, X, y, Folds(splits, len(X)), cv)
     plan.set_scoring(None)
     return plan
 

@@ -30,14 +30,14 @@ def main():
 
     from sklearn.model_selection import GridSearchCV as SkGridSearchCV, KFold, ParameterGrid
     from sklearn.svm import SVR
-    from spark_sklearn_b200.estimators import Folds, SVRAdapter
+    from spark_sklearn_b200.estimators import Folds, SVRPlan
     from spark_sklearn_b200 import workloads as W
 
     w = W.make_workload(a.workload)
     X, y, cv = w["X"], w["y"], w["cv"]
     cands = list(ParameterGrid(w["param_grid"]))
     splits = list(KFold(cv).split(X))
-    plan = SVRAdapter.plan(SVR(**w["est_params"]), cands, X, y, Folds(splits, len(X)), cv)   # X, y resident from here
+    plan = SVRPlan.plan(SVR(**w["est_params"]), cands, X, y, Folds(splits, len(X)), cv)   # X, y resident from here
     n_fits = len(cands) * cv
 
     plan.evaluate([0])                                            # warm-up: library load, kernel attributes, buffers
