@@ -347,8 +347,17 @@ typedef struct gs_linear_debug {
 int gs_debug_linear(gs_handle *h, int32_t mode, int32_t n_cand, const double *alpha, const double *l1_ratio, int32_t fit_intercept,
                     double tol, int32_t max_iter, int32_t refit, gs_linear_debug *out);
 
-/* C[M][N] = sum_k A[M][k]*B[N][k] on the wgmma tensor-core path (3xTF32 split), host fp32 row-major in/out. */
-int gs_debug_gemm_nt(gs_handle *h, const float *A, int32_t M, const float *B, int32_t N, int32_t K, float *C);
+/* Test hook: one batched launch of the wgmma tensor-core contraction (3xTF32 split) as its callers make it.  A [rows_a][K]
+ * and B [rows_b][K] are host float32 row-major (symmetric: B is NULL and A is both operands, M == N).  batches [n_batches][6]
+ * = a_row0, b_row0, k0, k1, c_offset, ldc: batch z writes C[c_offset + m ldc + n] = sum_{k0 <= k < k1} A[a_row0 + m][k]
+ * B[b_row0 + n][k] for m < M, n < N.  C [c_elems] is in/out: elements outside every window keep the caller's values.
+ * n_sum > 0 then also sums the first n_sum blocks of per floats of C in float64 in block order into S [per] (the split-K
+ * partial sum).  GS_ERR_ARG, before anything runs, for a K range that is not whole 32-wide blocks inside [0, K), rows
+ * a_row0 .. a_row0 + M - 1 or b_row0 .. b_row0 + N - 1 outside their operand, ldc < N, a window past c_elems, a partial
+ * sum past c_elems, or symmetric with M != N. */
+int gs_debug_gemm_tc(gs_handle *h, const float *A, int64_t rows_a, const float *B, int64_t rows_b, int32_t K, const int64_t *batches,
+                     int32_t n_batches, int32_t M, int32_t N, int32_t symmetric, float *C, int64_t c_elems, int32_t n_sum, int64_t per,
+                     float *S);
 /*
  * LinearSVR (csrc/linsvr.cu).  Replaces: sklearn.svm.LinearSVR.fit / score per (candidate, split) (reference
  * base_search.py:83-87) with liblinear's three SVR solvers, chosen per fit by solver[c * n_splits + k]:
@@ -448,9 +457,10 @@ int gs_logreg_sag_refit(gs_handle *h, int32_t solver, double alpha_scaled, doubl
 /* Test hook: the first count sample positions (of n) the device SAG draws from this seed. */
 int gs_debug_sag_draws(gs_handle *h, uint32_t seed, int32_t n, int32_t count, int32_t *out);
 
-/* C[M][N] = sum_k A[M][k]*B[N][k] on the FP64 tensor-core path of gs_linsvc (K > 1024: split-K with the fixed-order sum of
- * the partials), host float64 row-major in/out. */
-int gs_debug_gemm_f64(gs_handle *h, const double *A, int32_t M, const double *B, int32_t N, int32_t K, double *C);
+/* Test hook: C[M][N] = sum_k A[M][k]*B[N][k] on the FP64 tensor-core path of gs_linsvc, host float64 row-major in/out.  M, N
+ * and K are zero padded to 64, 64 and 16; K is split into chunks of kchunk (the last one ragged) whose partials are summed
+ * in place in chunk order, as TRON's gradient does.  GS_ERR_ARG for a kchunk that is not a positive multiple of 16. */
+int gs_debug_gemm_f64(gs_handle *h, const double *A, int32_t M, const double *B, int32_t N, int32_t K, int32_t kchunk, double *C);
 
 /* ---- planning helpers (host only, no device work; used by gs_svc itself and by the multi-GPU host driver) -------- */
 /* Predicted SMO iterations (thousands, for ~8000 training rows) of one C-SVC sub-problem: the model that orders the

@@ -434,8 +434,7 @@ cudaError_t launch_sum_partials(const float *partial, int n_chunks, int64_t per,
 // symmetric: the A and B operands are the same matrix (M == N): tiles below the diagonal are not computed, their values are
 // stored as transposes of the tiles above it (bitwise symmetric result)
 cudaError_t launch_gemm_nt_tf32x3(const TcMap &a_hi, const TcMap &a_lo, const TcMap &b_hi, const TcMap &b_lo,
-                                  const TcBatch *d_batches, int n_batches, int M, int N, float alpha, bool accumulate,
-                                  cudaStream_t st, bool symmetric = false);
+                                  const TcBatch *d_batches, int n_batches, int M, int N, cudaStream_t st, bool symmetric = false);
 
 // ---- gemm_f64.cu: FP64 tensor-core (DMMA) contraction  C[M][N] = sum_k A[M][k] B[N][k], float64 throughout ----
 // M, N multiples of 64; K and kchunk multiples of 16; every row read (A rows < M, B rows < N, k < K) must exist.

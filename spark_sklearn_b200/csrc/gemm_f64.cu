@@ -94,14 +94,20 @@ cudaError_t launch_gemm_nt_f64(const double *A, int64_t lda, const double *B, in
     return cudaGetLastError();
 }
 
-extern "C" int gs_debug_gemm_f64(gs_handle *h, const double *A, int32_t M, const double *B, int32_t N, int32_t K, double *C)
+extern "C" int gs_debug_gemm_f64(gs_handle *h, const double *A, int32_t M, const double *B, int32_t N, int32_t K, int32_t kchunk,
+                                 double *C)
 {
-    if (!h || !A || !B || !C || M <= 0 || N <= 0 || K <= 0) return GS_ERR_ARG;
+    if (!h) return GS_ERR_ARG;
+    if (!A || !B || !C || M <= 0 || N <= 0 || K <= 0 || kchunk <= 0 || kchunk % BK) {
+        gs_set_error(h, "gs_debug_gemm_f64: bad arguments (kchunk must be a positive multiple of 16)");
+        return GS_ERR_ARG;
+    }
     GS_CUDA(cudaSetDevice(h->device));
     cudaStream_t st = h->stream;
+    // M, N padded to whole 64x64 tiles and K to whole 16-wide steps with zeros; split-K into kchunk-long chunks (the last one
+    // ragged) and the fixed-order in-place sum of the partials, as the TRON gradient runs it
     const int Mp = (M + BM - 1) / BM * BM, Np = (N + BN - 1) / BN * BN, Kp = (K + BK - 1) / BK * BK;
-    // K above 1024 goes through the split-K path and the fixed-order partial sum the TRON gradient uses
-    const int kchunk = Kp > 1024 ? 512 : Kp, nchunk = (Kp + kchunk - 1) / kchunk;
+    const int nchunk = (Kp + kchunk - 1) / kchunk;
     DevBuf a, b, c;
     GS_CUDA(a.reserve((size_t)Mp * Kp * 8)); GS_CUDA(b.reserve((size_t)Np * Kp * 8));
     GS_CUDA(c.reserve((size_t)nchunk * Mp * Np * 8));

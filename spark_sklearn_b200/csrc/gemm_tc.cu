@@ -115,16 +115,15 @@ __device__ __forceinline__ void decode_tile(int t, int tiles_m, int tiles_n, int
     ni = mi + r;
 }
 
-__device__ __forceinline__ void store_c(float *c, int64_t ldc, int row, int col, float v, int accumulate_c)
+__device__ __forceinline__ void store_c(float *c, int64_t ldc, int row, int col, float v)
 {
-    float *dst = c + (size_t)row * ldc + col;
-    *dst = accumulate_c ? *dst + v : v;
+    c[(size_t)row * ldc + col] = v;
 }
 
 __global__ void __launch_bounds__(NTHREADS, 1)
 gemm_nt_tf32x3_kernel(const __grid_constant__ CUtensorMap a_hi, const __grid_constant__ CUtensorMap a_lo,
                       const __grid_constant__ CUtensorMap b_hi, const __grid_constant__ CUtensorMap b_lo,
-                      const TcBatch *__restrict__ batches, int n_batches, int M, int N, float alpha, int accumulate_c, int symmetric)
+                      const TcBatch *__restrict__ batches, int n_batches, int M, int N, int symmetric)
 {
     extern __shared__ unsigned char smem_dyn[];
     unsigned char *smem = (unsigned char *)(((uintptr_t)smem_dyn + 1023) & ~(uintptr_t)1023);
@@ -216,20 +215,17 @@ gemm_nt_tf32x3_kernel(const __grid_constant__ CUtensorMap a_hi, const __grid_con
         for (int i = 0; i < 64; i += 2) {
             const int row = r0 + 8 * ((i >> 1) & 1), col = c0 + 8 * (i >> 2);
             if (row >= M || col >= N) continue;
-            const float v0 = alpha * d[i], v1 = alpha * d[i + 1];
+            const float v0 = d[i], v1 = d[i + 1];
             const bool two = col + 1 < N;
             if (vec && two) {
-                float2 *dst = reinterpret_cast<float2 *>(bt.c + (size_t)row * bt.ldc + col);
-                float2 o = make_float2(v0, v1);
-                if (accumulate_c) { const float2 p = *dst; o.x += p.x; o.y += p.y; }
-                *dst = o;
+                *reinterpret_cast<float2 *>(bt.c + (size_t)row * bt.ldc + col) = make_float2(v0, v1);
             } else {
-                if (!(diag && col < row)) store_c(bt.c, bt.ldc, row, col, v0, accumulate_c);
-                if (two && !(diag && col + 1 < row)) store_c(bt.c, bt.ldc, row, col + 1, v1, accumulate_c);
+                if (!(diag && col < row)) store_c(bt.c, bt.ldc, row, col, v0);
+                if (two && !(diag && col + 1 < row)) store_c(bt.c, bt.ldc, row, col + 1, v1);
             }
             if (symmetric) {                                                     // C[n][m] = C[m][n]
-                if (!(diag && col <= row)) store_c(bt.c, bt.ldc, col, row, v0, accumulate_c);
-                if (two && !(diag && col + 1 <= row)) store_c(bt.c, bt.ldc, col + 1, row, v1, accumulate_c);
+                if (!(diag && col <= row)) store_c(bt.c, bt.ldc, col, row, v0);
+                if (two && !(diag && col + 1 <= row)) store_c(bt.c, bt.ldc, col + 1, row, v1);
             }
         }
     }
@@ -303,8 +299,7 @@ cudaError_t launch_split_tf32(const float *x, float *hi, float *lo, size_t n, cu
 }
 
 cudaError_t launch_gemm_nt_tf32x3(const TcMap &a_hi, const TcMap &a_lo, const TcMap &b_hi, const TcMap &b_lo,
-                                  const TcBatch *d_batches, int n_batches, int M, int N, float alpha, bool accumulate,
-                                  cudaStream_t st, bool symmetric)
+                                  const TcBatch *d_batches, int n_batches, int M, int N, cudaStream_t st, bool symmetric)
 {
     // per device and per launch (cheap): a handle per GPU may launch this kernel from its own host thread
     cudaError_t e = cudaFuncSetAttribute(gemm_nt_tf32x3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
@@ -319,7 +314,62 @@ cudaError_t launch_gemm_nt_tf32x3(const TcMap &a_hi, const TcMap &a_lo, const Tc
     gemm_nt_tf32x3_kernel<<<grid, NTHREADS, SMEM_BYTES, st>>>(*reinterpret_cast<const CUtensorMap *>(&a_hi),
                                                               *reinterpret_cast<const CUtensorMap *>(&a_lo),
                                                               *reinterpret_cast<const CUtensorMap *>(&b_hi),
-                                                              *reinterpret_cast<const CUtensorMap *>(&b_lo), d_batches, n_batches, M, N, alpha,
-                                                              accumulate ? 1 : 0, symmetric ? 1 : 0);
+                                                              *reinterpret_cast<const CUtensorMap *>(&b_lo), d_batches, n_batches, M, N,
+                                                              symmetric ? 1 : 0);
     return cudaGetLastError();
+}
+
+// ---- test hook: one batched launch with host buffers, every argument checked before anything runs (include/b200gs.h) ----
+extern "C" int gs_debug_gemm_tc(gs_handle *h, const float *A, int64_t rows_a, const float *B, int64_t rows_b, int32_t K,
+                                const int64_t *batches, int32_t n_batches, int32_t M, int32_t N, int32_t symmetric, float *C,
+                                int64_t c_elems, int32_t n_sum, int64_t per, float *S)
+{
+    if (!h) return GS_ERR_ARG;
+    auto bad = [h](const char *why) { gs_set_error(h, std::string("gs_debug_gemm_tc: ") + why); return GS_ERR_ARG; };
+    if (!A || !C || !batches || K <= 0 || K % 4 || M <= 0 || N <= 0 || n_batches <= 0 || c_elems <= 0) return bad("bad sizes");
+    if (symmetric && (B || M != N)) return bad("symmetric takes A as both operands (B null) and M == N");
+    if (!symmetric && !B) return bad("B is null");
+    if (symmetric) rows_b = rows_a;
+    if (rows_a <= 0 || rows_b <= 0 || rows_a > INT32_MAX || rows_b > INT32_MAX) return bad("bad operand rows");
+    std::vector<TcBatch> hb((size_t)n_batches);
+    for (int z = 0; z < n_batches; z++) {
+        const int64_t *g = batches + (size_t)z * 6;
+        const int64_t a0 = g[0], b0 = g[1], k0 = g[2], k1 = g[3], off = g[4], ldc = g[5];
+        // the TcBatch contract: [k0, k1) in whole 32-wide k-blocks inside the operands
+        if (k0 < 0 || k1 < k0 || k1 > K || k0 % 32 || (k1 - k0) % 32) return bad("K range not 32-aligned inside [0, K)");
+        // the rows that reach the window must exist; the rest of a 128-row tile past an operand's end is the tensor map's zero fill
+        if (a0 < 0 || a0 + M > rows_a || b0 < 0 || b0 + N > rows_b) return bad("row offset outside its operand");
+        if (ldc < N || (M > 1 && ldc > c_elems) || off < 0 || off > c_elems || (int64_t)(M - 1) * ldc + N > c_elems - off) return bad("output window outside C");
+        hb[z] = TcBatch{(int)a0, (int)b0, (int)k0, (int)k1, nullptr, ldc};
+    }
+    if (n_sum < 0 || (n_sum > 0 && (!S || per <= 0 || per > c_elems / n_sum))) return bad("partial sum outside C");
+
+    GS_CUDA(cudaSetDevice(h->device));
+    cudaStream_t st = h->stream;
+    const size_t na = (size_t)rows_a * K, nb = symmetric ? 0 : (size_t)rows_b * K;
+    DevBuf a, b, c, bt, s;
+    GS_CUDA(a.reserve(na * 12));                                     // A, A_hi, A_lo
+    if (nb) GS_CUDA(b.reserve(nb * 12));
+    GS_CUDA(c.reserve((size_t)c_elems * 4)); GS_CUDA(bt.reserve(hb.size() * sizeof(TcBatch)));
+    if (n_sum) GS_CUDA(s.reserve((size_t)per * 4));
+    for (int z = 0; z < n_batches; z++) hb[z].c = c.as<float>() + batches[(size_t)z * 6 + 4];
+    float *ah = a.as<float>() + na, *al = ah + na, *bh = nb ? b.as<float>() + nb : ah, *bl = nb ? bh + nb : al;
+    GS_CUDA(cudaMemcpyAsync(a.p, A, na * 4, cudaMemcpyHostToDevice, st));
+    GS_CUDA(launch_split_tf32(a.as<float>(), ah, al, na, st));
+    if (nb) {
+        GS_CUDA(cudaMemcpyAsync(b.p, B, nb * 4, cudaMemcpyHostToDevice, st));
+        GS_CUDA(launch_split_tf32(b.as<float>(), bh, bl, nb, st));
+    }
+    GS_CUDA(cudaMemcpyAsync(c.p, C, (size_t)c_elems * 4, cudaMemcpyHostToDevice, st));
+    GS_CUDA(cudaMemcpyAsync(bt.p, hb.data(), hb.size() * sizeof(TcBatch), cudaMemcpyHostToDevice, st));
+    TcMap mah, mal, mbh, mbl;
+    GS_CUDA(tc_make_map(&mah, ah, rows_a, K, K)); GS_CUDA(tc_make_map(&mal, al, rows_a, K, K));
+    GS_CUDA(tc_make_map(&mbh, bh, rows_b, K, K)); GS_CUDA(tc_make_map(&mbl, bl, rows_b, K, K));
+    GS_CUDA(launch_gemm_nt_tf32x3(mah, mal, mbh, mbl, bt.as<TcBatch>(), n_batches, M, N, st, symmetric != 0));
+    if (n_sum) GS_CUDA(launch_sum_partials(c.as<float>(), n_sum, per, s.as<float>(), st));
+    GS_CUDA(cudaMemcpyAsync(C, c.p, (size_t)c_elems * 4, cudaMemcpyDeviceToHost, st));
+    if (n_sum) GS_CUDA(cudaMemcpyAsync(S, s.p, (size_t)per * 4, cudaMemcpyDeviceToHost, st));
+    GS_CUDA(cudaStreamSynchronize(st));
+    a.release(); b.release(); c.release(); bt.release(); s.release();
+    return GS_OK;
 }

@@ -30,7 +30,7 @@ int build_gram(gs_handle *h, uint32_t flags, cudaStream_t st)
         TcBatch hb{0, 0, 0, dpad, bs.as<float>(), ld32};
         GS_CUDA(cudaMemcpyAsync(bb.p, &hb, sizeof hb, cudaMemcpyHostToDevice, st));
         h->tt.begin(h->evp, st);
-        GS_CUDA(launch_gemm_nt_tf32x3(mh, ml, mh, ml, bb.as<TcBatch>(), 1, n, n, 1.0f, false, st, true));
+        GS_CUDA(launch_gemm_nt_tf32x3(mh, ml, mh, ml, bb.as<TcBatch>(), 1, n, n, st, true));
         h->tt.end(h->evp, st, 3.0 * 2.0 * n * (double)n * dpad);
         GS_CUDA(launch_widen_gram(bs.as<float>(), n, ld32, h->dS.as<double>(), h->dXsq.as<double>(), st));
         pf.launches += 3;

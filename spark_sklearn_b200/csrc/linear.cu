@@ -755,7 +755,7 @@ int ridge_run(gs_handle *h, int n_cand, const double *alpha, int fit_intercept, 
     GS_CUDA(tc_make_map(&mzh, bZh.as<float>(), Dp, ldz, ldz));
     GS_CUDA(tc_make_map(&mzl, bZl.as<float>(), Dp, ldz, ldz));
     h->tt.begin(h->evp, st);
-    GS_CUDA(launch_gemm_nt_tf32x3(mzh, mzl, mzh, mzl, dBatchG, nq, D, D, 1.0f, false, st, true));   // Gram: upper tiles + mirror
+    GS_CUDA(launch_gemm_nt_tf32x3(mzh, mzl, mzh, mzl, dBatchG, nq, D, D, st, true));   // Gram: upper tiles + mirror
     h->tt.end(h->evp, st, 3.0 * 2.0 * (double)D * D * (double)ldz * (((D + 127) / 128 + 1) / (2.0 * ((D + 127) / 128))));   // tiles on/above the diagonal
     ones_row_kernel<<<(nb * Dp + 255) / 256, 256, 0, st>>>(dGq, dQs, nb, Dp, d, dE);
     sum_grams_kernel<<<528, 256, 0, st>>>(dGq, dQs, nb, nb_plain, Dp, d, dBshift, dShift, dE, dG, dT, weighted ? dTw : nullptr);
@@ -798,7 +798,7 @@ int ridge_run(gs_handle *h, int n_cand, const double *alpha, int fit_intercept, 
         while (open > 0 && it < CG_MAX_ITER) {
             for (int rep = 0; rep < 4; rep++, it++) {
                 h->tt.begin(h->evp, st);
-                GS_CUDA(launch_gemm_nt_tf32x3(mph, mpl, mah, mal, dBatchCG, groups * nkc, n_cand, dp, 1.0f, false, st));
+                GS_CUDA(launch_gemm_nt_tf32x3(mph, mpl, mah, mal, dBatchCG, groups * nkc, n_cand, dp, st));
                 h->tt.end(h->evp, st, 3.0 * 2.0 * (double)groups * n_cand * (double)dp * dp);
                 if (nkc > 1) GS_CUDA(launch_sum_partials(dQp, nkc, (int64_t)nsys * dp, dQ, st));
                 GS_CUDA(cudaMemsetAsync(dOpen, 0, 4, st));
@@ -1012,35 +1012,6 @@ int gs_debug_linear(gs_handle *h, int32_t mode, int32_t n_cand, const double *al
     std::vector<double> te((size_t)n_cand * ns), tr((size_t)n_cand * ns), coef((size_t)h->d + 1);
     return ridge_run(h, n_cand, alpha, fit_intercept, refit != 0, te.data(), tr.data(), coef.data(), &t,
                      mode == GS_DEBUG_ENET ? &en : nullptr, out);
-}
-
-// ---- test hook: one tensor-core GEMM with host buffers ----
-int gs_debug_gemm_nt(gs_handle *h, const float *A, int32_t M, const float *B, int32_t N, int32_t K, float *C)
-{
-    if (!h || !A || !B || !C || M <= 0 || N <= 0 || K <= 0) return GS_ERR_ARG;
-    GS_CUDA(cudaSetDevice(h->device));
-    cudaStream_t st = h->stream;
-    const int Kp = (K + 31) & ~31;                                   // zero-padded contraction length
-    DevBuf a, ah, al, b, bh, bl, c, bt;
-    GS_CUDA(a.reserve((size_t)M * Kp * 4)); GS_CUDA(ah.reserve((size_t)M * Kp * 4)); GS_CUDA(al.reserve((size_t)M * Kp * 4));
-    GS_CUDA(b.reserve((size_t)N * Kp * 4)); GS_CUDA(bh.reserve((size_t)N * Kp * 4)); GS_CUDA(bl.reserve((size_t)N * Kp * 4));
-    GS_CUDA(c.reserve((size_t)M * N * 4)); GS_CUDA(bt.reserve(sizeof(TcBatch)));
-    GS_CUDA(cudaMemsetAsync(a.p, 0, (size_t)M * Kp * 4, st));
-    GS_CUDA(cudaMemsetAsync(b.p, 0, (size_t)N * Kp * 4, st));
-    GS_CUDA(cudaMemcpy2DAsync(a.p, (size_t)Kp * 4, A, (size_t)K * 4, (size_t)K * 4, M, cudaMemcpyHostToDevice, st));
-    GS_CUDA(cudaMemcpy2DAsync(b.p, (size_t)Kp * 4, B, (size_t)K * 4, (size_t)K * 4, N, cudaMemcpyHostToDevice, st));
-    GS_CUDA(launch_split_tf32(a.as<float>(), ah.as<float>(), al.as<float>(), (size_t)M * Kp, st));
-    GS_CUDA(launch_split_tf32(b.as<float>(), bh.as<float>(), bl.as<float>(), (size_t)N * Kp, st));
-    TcMap mah, mal, mbh, mbl;
-    GS_CUDA(tc_make_map(&mah, ah.as<float>(), M, Kp, Kp)); GS_CUDA(tc_make_map(&mal, al.as<float>(), M, Kp, Kp));
-    GS_CUDA(tc_make_map(&mbh, bh.as<float>(), N, Kp, Kp)); GS_CUDA(tc_make_map(&mbl, bl.as<float>(), N, Kp, Kp));
-    TcBatch hb{0, 0, 0, Kp, c.as<float>(), (int64_t)N};
-    GS_CUDA(cudaMemcpyAsync(bt.p, &hb, sizeof hb, cudaMemcpyHostToDevice, st));
-    GS_CUDA(launch_gemm_nt_tf32x3(mah, mal, mbh, mbl, bt.as<TcBatch>(), 1, M, N, 1.0f, false, st, A == B && M == N));   // same matrix: Gram mode
-    GS_CUDA(cudaMemcpyAsync(C, c.p, (size_t)M * N * 4, cudaMemcpyDeviceToHost, st));
-    GS_CUDA(cudaStreamSynchronize(st));
-    a.release(); ah.release(); al.release(); b.release(); bh.release(); bl.release(); c.release(); bt.release();
-    return GS_OK;
 }
 
 }  // extern "C"

@@ -667,14 +667,14 @@ int logreg_run(gs_handle *h, int n_cand, const double *Cv, double tol, int max_i
     while (open > 0 && rounds < 4000) {
         // f, g at every open column's trial point: Z^T = W Xa^T ; R = residual(Z) ; G = R Xa
         h->tt.begin(h->evp, st);
-        GS_CUDA(launch_gemm_nt_tf32x3(mWh, mWl, mXh, mXl, dBatch, 1, ncol, n, 1.0f, false, st));
+        GS_CUDA(launch_gemm_nt_tf32x3(mWh, mWl, mXh, mXl, dBatch, 1, ncol, n, st));
         h->tt.end(h->evp, st, 3.0 * 2.0 * (double)ncol * n * nvp);
         dim3 grid(64, nfit);
         if (multi) multinomial_residual_kernel<<<grid, 256, 0, st>>>(dZ, npad, n, KC, h->dY.as<int>(), h->masks(), dFoldOf, dInv, dCw, dSw, dS, dRh, dRl);
         else logistic_residual_kernel<<<grid, 256, 0, st>>>(dZ, npad, n, h->dY.as<int>(), h->masks(), dFoldOf, dInv, dCw, dSw, dS, dRh, dRl);
         GS_CUDA(cudaGetLastError());
         h->tt.begin(h->evp, st);
-        GS_CUDA(launch_gemm_nt_tf32x3(mRh, mRl, mXth, mXtl, dBatch + 1, nchunk, ncol, nv, 1.0f, false, st));
+        GS_CUDA(launch_gemm_nt_tf32x3(mRh, mRl, mXth, mXtl, dBatch + 1, nchunk, ncol, nv, st));
         h->tt.end(h->evp, st, 3.0 * 2.0 * (double)ncol * nv * (double)npad);
         GS_CUDA(launch_sum_partials(dGp, nchunk, (int64_t)ncol * nvp, dG, st));
         GS_CUDA(cudaMemsetAsync(dOpen, 0, 4, st));
@@ -695,7 +695,7 @@ int logreg_run(gs_handle *h, int n_cand, const double *Cv, double tol, int max_i
         lbfgs_export_kernel<<<nfit, 128, 0, st>>>(dV, nfit, nv, nvp, KC, dWh, dWl, (int64_t)nvp * KC);
         GS_CUDA(cudaGetLastError());
         h->tt.begin(h->evp, st);
-        GS_CUDA(launch_gemm_nt_tf32x3(mWh, mWl, mXh, mXl, dBatch, 1, ncol, n, 1.0f, false, st));
+        GS_CUDA(launch_gemm_nt_tf32x3(mWh, mWl, mXh, mXl, dBatch, 1, ncol, n, st));
         h->tt.end(h->evp, st, 3.0 * 2.0 * (double)ncol * n * nvp);
         GS_CUDA(cudaMemsetAsync(dCounts, 0, (size_t)nfit * 16, st));
         dim3 grid(64, nfit);

@@ -92,7 +92,7 @@ def load_library():
     L.gs_logreg_refit.argtypes = [vp, dbl, dbl, i32, i32, vp, vp]
     L.gs_linsvc.argtypes = [vp, i32, vp, dbl, i32, i32, dbl, u32, vp, vp, vp, vp, vp]
     L.gs_linsvc_refit.argtypes = [vp, dbl, dbl, i32, i32, dbl, vp, vp]
-    L.gs_debug_gemm_f64.argtypes = [vp, vp, i32, vp, i32, i32, vp]
+    L.gs_debug_gemm_f64.argtypes = [vp, vp, i32, vp, i32, i32, i32, vp]
     L.gs_linsvr.argtypes = [vp, i32, vp, vp, vp, vp, dbl, i32, i32, dbl, u32, vp, vp, vp, vp, vp, vp, vp]
     L.gs_linsvr_refit.argtypes = [vp, dbl, dbl, i32, u32, dbl, i32, i32, dbl, vp, vp]
     L.gs_set_train_order.argtypes = [vp, vp, vp, i32]
@@ -110,7 +110,7 @@ def load_library():
     L.gs_debug_kernel_matrix.argtypes = [vp, i32, dbl, vp, vp, vp]
     L.gs_debug_decision.argtypes = [vp, i32, dbl, i32, dbl, vp, i32, i32, vp, vp]
     L.gs_debug_score.argtypes = [vp, i32, vp, vp, i32, vp, vp, i32, vp]
-    L.gs_debug_gemm_nt.argtypes = [vp, vp, i32, vp, i32, i32, vp]
+    L.gs_debug_gemm_tc.argtypes = [vp, vp, i64, vp, i64, i32, vp, i32, i32, i32, i32, vp, i64, i32, i64, vp]
     L.gs_debug_linear.argtypes = [vp, i32, i32, vp, vp, i32, dbl, i32, i32, vp]
     L.gs_svc_predicted_iterations.argtypes = [i32, dbl, dbl, i32]
     L.gs_svc_predicted_iterations.restype = dbl
@@ -121,7 +121,7 @@ def load_library():
     for f in ("gs_create", "gs_set_data", "gs_svc", "gs_svc_refit", "gs_ridge", "gs_ridge_refit", "gs_enet", "gs_enet_refit", "gs_set_targets_f64",
               "gs_svr", "gs_svr_refit", "gs_nusvc", "gs_nusvc_refit", "gs_nusvr", "gs_nusvr_refit", "gs_logreg",
               "gs_logreg_refit", "gs_linsvc", "gs_linsvc_refit", "gs_get_profile", "gs_debug_gram", "gs_debug_kernel_matrix",
-              "gs_debug_decision", "gs_debug_score", "gs_debug_linear", "gs_debug_gemm_nt", "gs_debug_gemm_f64", "gs_knn", "gs_debug_knn_neighbors",
+              "gs_debug_decision", "gs_debug_score", "gs_debug_linear", "gs_debug_gemm_tc", "gs_debug_gemm_f64", "gs_knn", "gs_debug_knn_neighbors",
               "gs_linsvr", "gs_linsvr_refit", "gs_set_train_order", "gs_debug_mt19937", "gs_sgd", "gs_sgd_refit", "gs_debug_sgd_perm",
               "gs_logreg_sag", "gs_logreg_sag_refit", "gs_debug_sag_draws"):
         getattr(L, f).restype = c.c_int
@@ -639,17 +639,43 @@ class Engine:
         return out
 
     def debug_gemm_nt(self, A, B):
+        """C = A B^T on the tensor-core path as one batch over the whole (zero-padded) K; B is A: the symmetric Gram mode."""
+        symmetric = B is A
         A = np.ascontiguousarray(A, np.float32)
         B = np.ascontiguousarray(B, np.float32)
-        C = np.zeros((A.shape[0], B.shape[0]), np.float32)
-        self._check(self._L.gs_debug_gemm_nt(self._h, _ptr(A), A.shape[0], _ptr(B), B.shape[0], A.shape[1], _ptr(C)))
-        return C
+        (M, K), N = A.shape, B.shape[0]
+        Kp = (K + 31) // 32 * 32
+        pad = lambda X: np.pad(X, ((0, 0), (0, Kp - K)))
+        C = np.zeros(M * N, np.float32)
+        C = self.debug_gemm_tc(pad(A), None if symmetric else pad(B), [[0, 0, 0, Kp, 0, N]], M, N, C, symmetric=symmetric)
+        return C.reshape(M, N)
 
-    def debug_gemm_f64(self, A, B):
+    def debug_gemm_tc(self, A, B, batches, M, N, C, symmetric=False, n_sum=0, per=0):
+        """One batched tensor-core launch (include/b200gs.h gs_debug_gemm_tc): A [rows_a][K], B [rows_b][K] (None when
+        symmetric), batches [n][6] of a_row0, b_row0, k0, k1, c_offset, ldc, C [c_elems] float32 in/out.  Returns the new C,
+        and with n_sum > 0 also the float64-ordered sum of its first n_sum blocks of per floats: (C, S)."""
+        A = np.ascontiguousarray(A, np.float32)
+        B = None if B is None else np.ascontiguousarray(B, np.float32)
+        bt = np.ascontiguousarray(batches, np.int64).reshape(-1, 6)
+        C = np.array(C, np.float32, copy=True).ravel()
+        S = np.zeros(max(int(per), 1), np.float32) if n_sum else None
+        rows_b = 0 if B is None else B.shape[0]
+        if B is not None and B.shape[1] != A.shape[1]:
+            raise ValueError("A and B have different K")
+        self._check(self._L.gs_debug_gemm_tc(self._h, _ptr(A), A.shape[0], _ptr(B), rows_b, A.shape[1], _ptr(bt), bt.shape[0],
+                                             int(M), int(N), int(bool(symmetric)), _ptr(C), C.size, int(n_sum), int(per), _ptr(S)))
+        return (C, S) if n_sum else C
+
+    def debug_gemm_f64(self, A, B, kchunk=None):
+        """C = A B^T on the FP64 tensor-core path, K split into kchunk-long chunks (default: 512 above K = 1024, else one)"""
         A = np.ascontiguousarray(A, np.float64)
         B = np.ascontiguousarray(B, np.float64)
+        K = A.shape[1]
+        if kchunk is None:
+            Kp = (K + 15) // 16 * 16
+            kchunk = 512 if Kp > 1024 else Kp
         C = np.zeros((A.shape[0], B.shape[0]))
-        self._check(self._L.gs_debug_gemm_f64(self._h, _ptr(A), A.shape[0], _ptr(B), B.shape[0], A.shape[1], _ptr(C)))
+        self._check(self._L.gs_debug_gemm_f64(self._h, _ptr(A), A.shape[0], _ptr(B), B.shape[0], K, int(kchunk), _ptr(C)))
         return C
 
     def profile(self):

@@ -24,16 +24,6 @@ def _split_scores(search, ns, which="test"):
     return np.stack([search.cv_results_["split%d_%s_score" % (k, which)] for k in range(ns)], 1)
 
 
-def test_gemm_f64_matches_numpy(engine):
-    rng = np.random.RandomState(0)
-    for M, N, K in [(5, 7, 3), (70, 130, 257), (64, 300, 5000)]:          # the last one runs split-K (K > 1024)
-        A, B = rng.standard_normal((M, K)), rng.standard_normal((N, K))
-        got = engine.debug_gemm_f64(A, B)
-        ref = A @ B.T
-        bound = 2 * K * np.finfo(np.float64).eps * (np.abs(A) @ np.abs(B).T)   # float64 rounding of a K-term sum
-        assert np.all(np.abs(got - ref) <= bound)
-
-
 @pytest.mark.parametrize("key", ["linsvc_small", "linsvc_multi"])
 @pytest.mark.parametrize("variant", ["none", "balanced", "dict", "sw"])
 def test_linsvc_vs_golden(engine, key, variant):
