@@ -217,28 +217,26 @@ struct SmoProblem {
     int nseg, seg_start[4], seg_len[4];
     int nslots;           // sum of seg_len: size of the slot space of smo_lean.cu (0 when nseg == 0)
 };
-// Solve problems order[0..n_prob) (one CTA each); lmax = max l (selects the template instance).
-cudaError_t launch_smo(const SmoProblem *d_probs, const int *d_order, int n_prob, int lmax, bool fast, int rowcap,
-                       cudaStream_t st, std::string *why);
 int smo_max_rows();   // largest sub-problem the resident-state kernel supports
 // epsilon-SVR data of one problem (parallel to SmoProblem; only the SVR instances read it)
 struct SvrData {
     const double *z;      // [n] float64 targets by dataset row
     double eps;           // SVR epsilon (libsvm's p)
 };
-// epsilon-SVR on the position-owned kernel: problem q has l = 2 x (training rows) positions, rows[] = the training rows
-// (ascending original index) twice, n_pos = l / 2; svr[q] holds its targets and epsilon.  coef gets alpha+ - alpha- by row.
-cudaError_t launch_smo_svr(const SmoProblem *d_probs, const SvrData *d_svr, const int *d_order, int n_prob, int lmax, bool fast,
-                           int rowcap, cudaStream_t st, std::string *why);
 // nu-SVC / nu-SVR starting point of one problem (parallel to SmoProblem; only the nu instances read it): the sums that
 // libsvm hands out greedily, min(C, remaining) in position order, to the +1 positions and to the -1 positions
 struct NuData {
     double sum_pos, sum_neg;
 };
-// libsvm's Solver_NU on the position-owned kernel.  d_svr == nullptr: nu-SVC (C = Cn = 1, coef = alpha y / r, rho / r);
-// otherwise nu-SVR on the SVR layout of launch_smo_svr with svr[q].eps = 0 (linear term -/+ z).
-cudaError_t launch_smo_nu(const SmoProblem *d_probs, const SvrData *d_svr, const NuData *d_nu, const int *d_order, int n_prob,
-                          int lmax, bool fast, cudaStream_t st, std::string *why);
+// The position-owned kernel: solves problems order[0..n_prob) (one CTA each); lmax = max l selects the template instance,
+// *why says why an lmax is not supported.  Parallel to d_probs, d_svr and d_nu (each may be null) select the model:
+//   * neither: C-SVC;
+//   * d_svr: epsilon-SVR: problem q has l = 2 x (training rows) positions, rows[] = the training rows (ascending original
+//     index) twice, n_pos = l / 2; svr[q] holds its targets and epsilon.  coef gets alpha+ - alpha- by row;
+//   * d_nu: libsvm's Solver_NU, nu-SVC (C = Cn = 1, coef = alpha y / r, rho / r), or with d_svr nu-SVR on the SVR layout
+//     with svr[q].eps = 0 (linear term -/+ z).
+cudaError_t launch_smo(const SmoProblem *d_probs, const SvrData *d_svr, const NuData *d_nu, const int *d_order, int n_prob,
+                       int lmax, bool fast, int rowcap, cudaStream_t st, std::string *why);
 // smo_lean.cu: the throughput instance (static slots = the problem's column runs, two or more sub-problems per SM).  Every
 // problem of the launch needs a slot layout: nseg > 0, nslots <= smo_lean_max_slots(), l < 16383; alpha and Gbar hold nslots doubles.
 int smo_lean_max_slots();
@@ -301,7 +299,7 @@ struct SplitScoreStats {
     double regression(int k, int sp, double rss) const;                // r2 / neg MSE / neg RMSE from a residual sum of squares
 };
 
-// ---- kernel_svm.cu: the host steps the SVC and SVR searches share (an int return is a GS_* status) ----
+// ---- kernel_svm.cu: the batch loop of the SVC, NuSVC, SVR and NuSVR searches and refits (an int return is a GS_* status) ----
 int build_gram(gs_handle *h, uint32_t flags, cudaStream_t st);   // S = X X^T -> h->dS, diag(S) -> h->dXsq
 // One kernel matrix: the kernel and the parameters it reads.  Parameters a kernel ignores are stored as 0 (linear: all three,
 // rbf: degree and coef0, sigmoid: degree), so candidates that differ only in them share the matrix.
@@ -322,7 +320,29 @@ struct KernelSpec {
         return coef0 < o.coef0;
     }
 };
-struct SvmSearch {                                 // the state of one svc_run / svr_run call
+// The SMO problems of one batch on the host, in column order
+struct SmoBatch {
+    std::vector<SmoProblem> probs;
+    std::vector<double> cost;                      // predicted solve cost of each problem: the costliest are launched first
+    std::vector<SvrData> svr;                      // one per problem for SVR, else empty
+    std::vector<NuData> nu;                        // one per problem for the nu models, else empty
+};
+// What one kernel-SVM model gives the batch loop.  Task t is candidate t / n_splits on split t % n_splits.
+struct SvmModel {
+    const char *who;                               // the C function, for error messages
+    bool refit;
+    int n_splits, kind;                            // kind: the scorer
+    double tol;
+    int max_iter;
+    uint32_t flags;
+    std::vector<int> rows;                         // the dataset rows of every problem
+    int lmax;                                      // the most positions of a problem
+    std::vector<char> skip;                        // per task, or empty: a task not solved scores NaN with n_iter -1
+    // Appends task t's problems to b, made from base (its model-independent fields set, rows at the device copy of rows),
+    // with their cost and, for SVR and nu, their SvrData / NuData.  ks: the task's kernel matrix.
+    std::function<void(int t, const KernelSpec &ks, const SmoProblem &base, SmoBatch &b)> add_task;
+};
+struct SvmSearch {                                 // the state of one kernel-SVM search or refit
     gs_handle *h;
     cudaStream_t st;
     int n;
@@ -343,17 +363,34 @@ struct SvmSearch {                                 // the state of one svc_run /
     std::vector<int> info;
     std::vector<unsigned long long> ns;
     std::vector<double> rho, coef;
+    std::vector<unsigned long long> auc_pairs;     // host copies of the batch's ROC-AUC pair counts / class counts
+    std::vector<int> class_counts;
     SvmSearch(gs_handle *h_, cudaStream_t st_) : h(h_), st(st_), n((int)h_->n), ldk(((int64_t)h_->n + 31) & ~31LL), tm(st_, h_->evp) {}
-    void begin();                                  // resets h->prof but gs_set_data's ms_h2d / h2d_bytes; begin event
+    // resets h->prof but gs_set_data's ms_h2d / h2d_bytes, records the begin event and enqueues the Gram
+    int start(uint32_t flags);
     // groups the tasks by kernel matrix; rejects an rbf gamma that is not finite and > 0, a poly / sigmoid gamma that is not
     // finite and >= 0, with who in the message.  degree / coef0: per candidate, or null for scikit-learn's 3 / 0.
     int group(const char *who, int n_cand, int n_splits, const int32_t *kernel, const double *gamma, const int32_t *degree,
               const double *coef0);
+    // Solves, scores and finishes every task in batches of kernel matrices, and writes the outputs (any may be null but a
+    // search's test_scores).  A search writes per task; a refit writes rho, n_iter and coef ([n] by original row) per problem.
+    int run(const SvmModel &m, double *test_scores, double *train_scores, int32_t *n_iter, int32_t *n_sv, float *fit_ms,
+            float *score_ms, double *coef, double *rho_out);
+    // the steps of run
     int plan_batches();                            // per_batch; reserves h->dK (and room for the diagonals when a group has one)
     int kernel_matrices(int g0, int g1);           // group g at h->dK + (g - g0) n ldk, its diagonal, the guard flag, fast
     const double *qd(int g, int g0) const;         // SmoProblem::qd of group g in the batch from g0
     int workspaces(std::vector<SmoProblem> &probs);   // alpha / Gbar / scratch / coef / outputs of every problem
+    // enqueues the SMO launches of a batch in launch order d_order (its problems by cost, descending) and counts them in
+    // h->prof.launches: C-SVC on the cluster / exclusive-SM / shared-SM tiers, nu and SVR on one position-owned launch.
+    // *n_cl / *n_ex: how many went on clusters / exclusive SMs.
+    int solve(const SmoBatch &b, const std::vector<int> &order, const SmoProblem *d_probs, const SvrData *d_svr,
+              const NuData *d_nu, const int *d_order, int lmax, int *n_cl, int *n_ex);
     int decisions(int g0, int g1, const std::vector<int> &group_first);   // group g: columns from group_first[g - g0]
+    // enqueues what kind's score of every vote task is computed from, from the decision values: a classifier's vote counts
+    // or a regressor's residual sums of squares into d_votes (16 bytes per task), or AUC pair / class counts copied to
+    // auc_pairs / class_counts (read after the next sync)
+    int score(int kind, const std::vector<VoteTask> &vtasks, const VoteTask *d_vt, void *d_votes);
     int results(int np, bool with_coef);           // downloads the batch's outputs, syncs, collects its phase times
     int finish(int64_t smo_iterations, double solve_bytes);   // end event, sync, the profile's times and totals
 };

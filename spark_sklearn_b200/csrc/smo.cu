@@ -1,6 +1,6 @@
 // smo.cu -- batched C-SVC dual solver: one CTA per (candidate, fold, class-pair) sub-problem; its epsilon-SVR instance
-// (smo_svr_kernel, driven by svr.cu) solves one (candidate, fold) SVR fit per CTA; its nu instances (smo_nu_kernel) run
-// libsvm's Solver_NU for nu-SVC (api.cu) and nu-SVR (svr.cu).
+// (smo_svr_kernel) solves one (candidate, fold) SVR fit per CTA; its nu instances (smo_nu_kernel) run libsvm's Solver_NU
+// for nu-SVC and nu-SVR.  launch_smo, at the end of the file, launches all of them.
 //
 // Restates scikit-learn's libsvm Solver (svm.cpp:670-944 Solve, :946-1047 select_working_set,
 // :1049-1129 do_shrinking, :629-668 reconstruct_gradient, :1131-1168 calculate_rho) as a
@@ -900,32 +900,9 @@ cudaError_t launch_cfg(const SmoProblem *probs, const int *order, int n_prob, bo
                 : launch_one<NT, KPT, SMEM_STATE, false, false, ROWBUF, SVR>(probs, order, n_prob, rowcap, svr, st);
 }
 
-// the tier choice of launch_smo / launch_smo_svr: lmax positions (C-SVC rows, or twice the SVR training rows)
-template <bool SVR>
-cudaError_t launch_tiers(const SmoProblem *d_probs, const int *d_order, int n_prob, int lmax, bool fast, int rowcap,
-                         const SvrData *svr, cudaStream_t st, std::string *why)
-{
-    if (n_prob <= 0) return cudaSuccess;
-    const bool prof = prof_enabled();
-    if (lmax <= 512) return launch_cfg<128, 4, true, false, SVR>(d_probs, d_order, n_prob, fast, prof, 0, svr, st);
-    if (lmax <= 2048) return launch_cfg<256, 8, true, false, SVR>(d_probs, d_order, n_prob, fast, prof, 0, svr, st);
-    if (lmax <= 4096) return launch_cfg<512, 8, true, false, SVR>(d_probs, d_order, n_prob, fast, prof, 0, svr, st);
-    if (lmax <= 8192) {
-        // 8192 rows of state without G_bar = 152 KB; the row buffer may use what is left of the 227 KB
-        const bool rowbuf_fits = (size_t)8192 * 19 + 128 + (size_t)rowcap * 4 + 4096 <= 227 * 1024;
-        if (rowbuf_fits)
-            return launch_cfg<1024, 8, true, true, SVR>(d_probs, d_order, n_prob, fast, prof, rowcap, svr, st);
-        return launch_cfg<1024, 8, true, false, SVR>(d_probs, d_order, n_prob, fast, prof, 0, svr, st);
-    }
-    if (lmax <= 16384) return launch_cfg<1024, 16, false, false, SVR>(d_probs, d_order, n_prob, fast, prof, 0, svr, st);
-    if (why) *why = SVR ? "SVR fit with more than 8192 training rows is not supported by the resident-state SMO kernel"
-                        : "SVC sub-problem larger than 16384 rows is not supported by the resident-state SMO kernel";
-    return cudaErrorInvalidValue;
-}
-
 template <int NT, int KPT, bool SMEM_STATE, bool SVR>
-cudaError_t launch_nu_cfg(const SmoProblem *probs, const int *order, int n_prob, bool fast, const SvrData *svr, const NuData *nu,
-                          cudaStream_t st)
+cudaError_t launch_nu(const SmoProblem *probs, const int *order, int n_prob, bool fast, const SvrData *svr, const NuData *nu,
+                      cudaStream_t st)
 {
     constexpr int LCAP = NT * KPT;
     const size_t smem = (size_t)LCAP * (SMEM_STATE ? (8 + 8 + 8 + 2 + 1) : (8 + 2 + 1));
@@ -936,43 +913,44 @@ cudaError_t launch_nu_cfg(const SmoProblem *probs, const int *order, int n_prob,
     return cudaGetLastError();
 }
 
-// the tiers of launch_tiers without the bulk-row-copy instance
-template <bool SVR>
-cudaError_t launch_nu_tiers(const SmoProblem *d_probs, const int *d_order, int n_prob, int lmax, bool fast, const SvrData *svr,
-                            const NuData *nu, cudaStream_t st, std::string *why)
+// One tier of launch_smo.  The nu instances have neither a bulk-row-copy (ROWBUF) nor a profiling instance.
+template <int NT, int KPT, bool SMEM_STATE, bool ROWBUF = false>
+cudaError_t launch_tier(const SmoProblem *probs, const SvrData *svr, const NuData *nu, const int *order, int n_prob, bool fast,
+                        int rowcap, cudaStream_t st)
 {
-    if (n_prob <= 0) return cudaSuccess;
-    if (lmax <= 512) return launch_nu_cfg<128, 4, true, SVR>(d_probs, d_order, n_prob, fast, svr, nu, st);
-    if (lmax <= 2048) return launch_nu_cfg<256, 8, true, SVR>(d_probs, d_order, n_prob, fast, svr, nu, st);
-    if (lmax <= 4096) return launch_nu_cfg<512, 8, true, SVR>(d_probs, d_order, n_prob, fast, svr, nu, st);
-    if (lmax <= 8192) return launch_nu_cfg<1024, 8, true, SVR>(d_probs, d_order, n_prob, fast, svr, nu, st);
-    if (lmax <= 16384) return launch_nu_cfg<1024, 16, false, SVR>(d_probs, d_order, n_prob, fast, svr, nu, st);
-    if (why) *why = SVR ? "NuSVR fit with more than 8192 training rows is not supported by the resident-state SMO kernel"
-                        : "NuSVC sub-problem larger than 16384 rows is not supported by the resident-state SMO kernel";
-    return cudaErrorInvalidValue;
+    if constexpr (!ROWBUF)
+        if (nu) return svr ? launch_nu<NT, KPT, SMEM_STATE, true>(probs, order, n_prob, fast, svr, nu, st)
+                           : launch_nu<NT, KPT, SMEM_STATE, false>(probs, order, n_prob, fast, nullptr, nu, st);
+    const bool prof = prof_enabled();
+    if (!ROWBUF) rowcap = 0;
+    return svr ? launch_cfg<NT, KPT, SMEM_STATE, ROWBUF, true>(probs, order, n_prob, fast, prof, rowcap, svr, st)
+               : launch_cfg<NT, KPT, SMEM_STATE, ROWBUF, false>(probs, order, n_prob, fast, prof, rowcap, nullptr, st);
 }
 
 }  // namespace
 
 int smo_max_rows() { return 1024 * 16; }
 
+// The tier is chosen by lmax positions (C-SVC rows, or twice the SVR training rows).
 // fast: every problem is rbf and every kernel matrix of the launch holds only positive normal floats
 // rowcap: row length of the K matrices in floats (ldk); enables the bulk-copy row path when the row fits in shared memory
-cudaError_t launch_smo(const SmoProblem *d_probs, const int *d_order, int n_prob, int lmax, bool fast, int rowcap, cudaStream_t st,
-                       std::string *why)
+cudaError_t launch_smo(const SmoProblem *d_probs, const SvrData *d_svr, const NuData *d_nu, const int *d_order, int n_prob,
+                       int lmax, bool fast, int rowcap, cudaStream_t st, std::string *why)
 {
-    return launch_tiers<false>(d_probs, d_order, n_prob, lmax, fast, rowcap, nullptr, st, why);
-}
-
-cudaError_t launch_smo_svr(const SmoProblem *d_probs, const SvrData *d_svr, const int *d_order, int n_prob, int lmax, bool fast,
-                           int rowcap, cudaStream_t st, std::string *why)
-{
-    return launch_tiers<true>(d_probs, d_order, n_prob, lmax, fast, rowcap, d_svr, st, why);
-}
-
-cudaError_t launch_smo_nu(const SmoProblem *d_probs, const SvrData *d_svr, const NuData *d_nu, const int *d_order, int n_prob,
-                          int lmax, bool fast, cudaStream_t st, std::string *why)
-{
-    return d_svr ? launch_nu_tiers<true>(d_probs, d_order, n_prob, lmax, fast, d_svr, d_nu, st, why)
-                 : launch_nu_tiers<false>(d_probs, d_order, n_prob, lmax, fast, nullptr, d_nu, st, why);
+    if (n_prob <= 0) return cudaSuccess;
+    if (lmax <= 512) return launch_tier<128, 4, true>(d_probs, d_svr, d_nu, d_order, n_prob, fast, rowcap, st);
+    if (lmax <= 2048) return launch_tier<256, 8, true>(d_probs, d_svr, d_nu, d_order, n_prob, fast, rowcap, st);
+    if (lmax <= 4096) return launch_tier<512, 8, true>(d_probs, d_svr, d_nu, d_order, n_prob, fast, rowcap, st);
+    if (lmax <= 8192) {
+        // 8192 rows of state without G_bar = 152 KB; the row buffer may use what is left of the 227 KB
+        const bool rowbuf_fits = (size_t)8192 * 19 + 128 + (size_t)rowcap * 4 + 4096 <= 227 * 1024;
+        if (rowbuf_fits && !d_nu) return launch_tier<1024, 8, true, true>(d_probs, d_svr, d_nu, d_order, n_prob, fast, rowcap, st);
+        return launch_tier<1024, 8, true>(d_probs, d_svr, d_nu, d_order, n_prob, fast, rowcap, st);
+    }
+    if (lmax <= 16384) return launch_tier<1024, 16, false>(d_probs, d_svr, d_nu, d_order, n_prob, fast, rowcap, st);
+    if (why) {
+        if (d_svr) *why = std::string(d_nu ? "NuSVR" : "SVR") + " fit with more than 8192 training rows is not supported by the resident-state SMO kernel";
+        else *why = std::string(d_nu ? "NuSVC" : "SVC") + " sub-problem larger than 16384 rows is not supported by the resident-state SMO kernel";
+    }
+    return cudaErrorInvalidValue;
 }
